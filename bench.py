@@ -3,6 +3,7 @@
 
     python bench.py --gpus N --steps K --warmup W            (N>1: launched by torch.distributed.run)
     python bench.py --impl reference --gpus N --steps K --warmup W
+    python bench.py --gpus 1 --steps K --warmup W --dump-outputs DIR     (also writes the last timed step's outputs as DIR/*.npy)
 
 Workload (BASELINE.json configs[1], SURVEY.md 8d "Config 2"): 4 096 SMPL envs per GPU, env=speed, flat ground,
 state_init=Default, self_obs_v=1 (obs 292), control_mode=uhc_pd (the reference's yaml default: stable PD), actions
@@ -60,21 +61,11 @@ def make_cfg(wl=None):
     return mk(env=w["env"], robot=w["robot"], overrides=w["overrides"])
 
 
-PEAK_FP32_TFLOPS = 148 * 128 * 2 * 1.965e9 / 1e12     # 148 SMs x 128 FP32 lanes x 2 (FMA) x clocks.max.sm: 74.5 TFLOP/s nominal
-
-
-def kernel_counters():
-    """ncu counters of the dominant kernel (profiles/k_step5_counters.json, written from the committed ncu capture):
-    issue-slot utilisation, active threads per instruction, resident warps, FP32 operations per env-step."""
-    p = os.path.join(ROOT, "profiles", "k_step5_counters.json")
-    try:
-        return json.load(open(p))
-    except Exception:
-        return None
+DUMP_MAX_BYTES = 60 * 1024 * 1024   # --dump-outputs: larger outputs are stored as a fixed, seeded sample of env rows (< 64 MB with headers)
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region (read-only queries)."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -128,7 +119,7 @@ def measured_peak_hbm():
             return float(json.load(open(p))["hbm_gbs"]), "measured"
         except Exception:
             pass
-    return 6650.0, "fallback"
+    return 3350.0, "H100 SXM data sheet"
 
 
 def host_cores():
@@ -264,7 +255,7 @@ def measure(wl, args, torch, dist, world, rank, local, K, W, headline):
     def draw(k):
         return torch.clamp(torch.randn(k, N, nu, generator=gen, device=dev) * SIGMA, -1, 1)
 
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)      # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)      # > 50 MB L2 (H100)
 
     def barrier():
         if world > 1:
@@ -303,6 +294,8 @@ def measure(wl, args, torch, dist, world, rank, local, K, W, headline):
     ev1.record()
     barrier()
     ms = ev0.elapsed_time(ev1)
+    # what a caller of the timed path holds after its last step (step + autoreset), copied before anything else runs
+    last = {"obs": env.obs_buf.cpu(), "reward": env.rew_buf.cpu(), "terminated": env.terminate_buf.cpu(), "truncated": env.truncate_buf.cpu()}
     launches = env.gpu_launches - launches0
     # ---------------- the L2 flush alone (it sits inside the timed region above: `value` is conservative by this much)
     f0, f1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -356,7 +349,7 @@ def measure(wl, args, torch, dist, world, rank, local, K, W, headline):
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     ms, e2e_ms, k_ms, flush_ms = [float(x) for x in t.tolist()]
-    out = dict(N=N, K=K, ms=ms, e2e_ms=e2e_ms, Ke=Ke, k_ms=k_ms, flush_ms=flush_ms, launches=launches, clocks=clocks, env=env, cfg=cfg)
+    out = dict(N=N, K=K, ms=ms, e2e_ms=e2e_ms, Ke=Ke, k_ms=k_ms, flush_ms=flush_ms, launches=launches, clocks=clocks, env=env, cfg=cfg, last=last)
     return out
 
 
@@ -406,6 +399,21 @@ def measure_ppo(torch, dist, world, rank, local, horizon=12, iters=2):
             "collective": "NCCL all-reduce of policy+value gradients (per-layer buckets, async) and of the advantage / RunningNorm moments"}
 
 
+def dump_outputs(d, last):
+    """Each output as d/<name>.npy (float32).  Above DUMP_MAX_BYTES in all, the same seeded sample of env rows is taken from every
+    output and the row numbers are written as env_index.npy."""
+    os.makedirs(d, exist_ok=True)
+    arrs = {k: v.numpy().astype(np.float32) for k, v in last.items()}
+    n = arrs["reward"].shape[0]
+    row_bytes = sum(a.nbytes // n for a in arrs.values())
+    if row_bytes * n > DUMP_MAX_BYTES:
+        idx = np.sort(np.random.default_rng(0).choice(n, DUMP_MAX_BYTES // (row_bytes + 8), replace=False))   # + 8: env_index
+        arrs = {k: a[idx] for k, a in arrs.items()}
+        arrs["env_index"] = idx.astype(np.float64)
+    for k, a in arrs.items():
+        np.save(os.path.join(d, f"{k}.npy"), a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -416,6 +424,7 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--workload", default="cfg2", choices=sorted(WORKLOADS))
     ap.add_argument("--no-extra", action="store_true", help="skip the short cfg4 / cfg5 runs appended to the headline line")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's obs / reward / terminated / truncated as DIR/<name>.npy")
     args = ap.parse_args()
     global _WL, WORKLOAD, B_ALG_BYTES
     _WL = args.workload
@@ -438,6 +447,8 @@ def main():
     K, W = args.steps, max(3, args.warmup)
     r = measure(_WL, args, torch, dist, world, rank, local, K, W, True)
     env, cfg, N = r["env"], r["cfg"], r["N"]
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, r["last"])
     extra = {}
     if not args.no_extra and _WL == "cfg2":
         # the configurations north_star states its target on (cfg4: 65 536 envs + motion feed on 8 GPUs; cfg5: SMPL-X), short runs
@@ -458,18 +469,7 @@ def main():
         peak, peak_src = measured_peak_hbm()
         balg = B_ALG_BYTES + (B_ALG_STALE_BYTES if env.envcfg.spd_stale and env.envcfg.control_mode == 0 else 0)
         achieved = balg * N / (k_ms * 1e-3) / 1e9
-        traffic = None
-        kc = kernel_counters() if _WL == "cfg2" else None
-        secondary = None
-        if kc:
-            traffic = kc.get("dram_bytes_per_launch")
-            flops = kc.get("fp32_flops_per_env_step")
-            secondary = {"issue_active_pct": kc.get("issue_active_pct"), "threads_per_inst": kc.get("threads_per_inst"),
-                         "warps_per_sm": kc.get("warps_per_sm"), "warp_inst_per_env_step": kc.get("warp_inst_per_env_step"),
-                         "fp32_flops_per_env_step": flops,
-                         "fp32_tflops": (flops * N / (k_ms * 1e-3) / 1e12) if flops else None,
-                         "fp32_flop_frac": (flops * N / (k_ms * 1e-3) / 1e12 / PEAK_FP32_TFLOPS) if flops else None,
-                         "fp32_peak_tflops": PEAK_FP32_TFLOPS, "source": kc.get("source")}
+        traffic = secondary = None
         line = {
             "metric": "env-steps/sec SMPL humanoid (speed task, 15 substeps/step)", "value": value, "unit": "env-steps/s", "n_gpus": world,
             "steps": K, "warmup": W, "ms_per_step": ms / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32",
@@ -477,7 +477,7 @@ def main():
             "config": {"workload": WORKLOAD, "envs_per_gpu": N, "global_envs": total_envs, "substeps_per_step": int(env.envcfg.nsubsteps),
                        "control_mode": str(cfg.env.control_mode), "spd_inertia": "stale" if env.envcfg.spd_stale else "fresh", "parallelism": f"env-shard x{world}",
                        "kernel": f"v{env.kernel_version}", "smem_bytes_per_env": env.smem_bytes_per_env(),
-                       "l2": "256 MiB flush buffer zeroed after every step inside the timed region (state ~11 MB < 126 MB L2)",
+                       "l2": "256 MiB flush buffer zeroed after every step inside the timed region (state ~11 MB < 50 MB L2)",
                        "flush_ms_per_step": r["flush_ms"], "value_excluding_flush": total_envs * K / (max(ms - K * r["flush_ms"], 1e-9) * 1e-3)},
             "substeps_per_s": value * int(env.envcfg.nsubsteps),
             "e2e": {"value": e2e, "unit": "env-steps/s", "h2d_bytes_per_step": N * nu * 4, "d2h_bytes_per_step": N * (env.num_obs * 4 + 4 + 2),
@@ -487,7 +487,7 @@ def main():
                          "peak_source": peak_src, "kernel": f"k_step{env.kernel_version}", "kernel_ms": k_ms, "alg_bytes_per_env_step": balg,
                          "secondary": secondary,
                          "note": "15 fused substeps keep state on-chip: the kernel is FP32-issue / latency bound, not HBM bound (SURVEY.md 8d); "
-                                 "`secondary` carries the issue-slot and FP32 fractions"},
+                                 "`secondary` (hardware counters) is not measured"},
         }
         if extra:
             line["other_workloads"] = extra

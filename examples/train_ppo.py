@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""PPO on the B200 stepper -- the loop of smpl_sim/run.py (AgentHumanoid.optimize_policy: sample -> update_params -> log) with
+"""PPO on the GPU stepper -- the loop of smpl_sim/run.py (AgentHumanoid.optimize_policy: sample -> update_params -> log) with
 the batched pieces of this repo: HumanoidBatchB200 (env shard on this GPU), BatchedSampler (device-resident rollout),
 smplsim_gae (advantages), PPOLearner (AgentPPO.update_params semantics, gradients / moments all-reduced over ranks).
 

@@ -1,5 +1,5 @@
 /*
- * smplsim.h -- C ABI of libsmplsim_b200.so, the B200-native batched SMPL-humanoid stepper.
+ * smplsim.h -- C ABI of libsmplsim_b200.so, the H100-native (sm_90a) batched SMPL-humanoid stepper.
  *
  * The reference (ZhengyiLuo/SMPLSim) has no FFI: its "operator API" for this path is the
  * Python protocol of smpl_sim/envs (SURVEY.md section 8b).  Each entry point below names

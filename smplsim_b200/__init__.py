@@ -1,4 +1,4 @@
-"""smplsim_b200 -- B200-native batched SMPL-humanoid physics stepper.
+"""smplsim_b200 -- H100-native (sm_90a) batched SMPL-humanoid physics stepper.
 
 Drop-in for the hot path of ZhengyiLuo/SMPLSim (``HumanoidEnv.step`` =
 15 x [PD torque + mj_step] + obs / reward / reset flags).  See DESIGN.md.

@@ -13,8 +13,8 @@ _LIB = None
 
 # -ftz / -prec-div / -prec-sqrt: denormals flushed, division and square root at 2 ulp (MUFU + one Newton step instead of the IEEE
 # sequences with their slow paths and denormal guards).  FMA contraction and everything else stay as in the default mode; the parity
-# tolerances (1e-4 against the fp64 oracle) are met with a wide margin, and the step kernel is 6 % faster (DESIGN.md 6).
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-ftz=true", "-prec-div=false", "-prec-sqrt=false",
+# tolerances (1e-4 against the fp64 oracle) are met with a wide margin, and the step kernel is faster (fewer instructions on its dependent chains).
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-ftz=true", "-prec-div=false", "-prec-sqrt=false",
               "-shared", "-Xcompiler", "-fPIC"]
 
 
@@ -25,7 +25,7 @@ def sources():
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """nvcc-compile the library in-tree for sm_100a (cross-compiles without a GPU)."""
+    """nvcc-compile the library in-tree for sm_90a (H100; cross-compiles without a GPU)."""
     newest = max(os.path.getmtime(s) for s in sources())
     if force or not os.path.exists(SO_PATH) or os.path.getmtime(SO_PATH) < newest:
         nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
@@ -56,10 +56,9 @@ _SYMBOLS = {
     "smplsim_warps_per_block": (C.c_int, [C.c_void_p]),
     "smplsim_kernel_version": (C.c_int, [C.c_void_p]),
     "smplsim_schedule_steps": (C.c_int, [C.c_void_p]),
-    "smplsim_records_in_tmem": (C.c_int, [C.c_void_p]),
 }
 # the entry points include/smplsim.h declares (checked by tests/test_abi.py)
-_INTROSPECTION = ("smplsim_smem_bytes_per_env", "smplsim_warps_per_block", "smplsim_kernel_version", "smplsim_schedule_steps", "smplsim_records_in_tmem")
+_INTROSPECTION = ("smplsim_smem_bytes_per_env", "smplsim_warps_per_block", "smplsim_kernel_version", "smplsim_schedule_steps")
 HEADER_SYMBOLS = [s for s in _SYMBOLS if s not in _INTROSPECTION]
 
 

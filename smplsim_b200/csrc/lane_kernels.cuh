@@ -5,14 +5,12 @@
 //   post_physics_step mj_kinematics, self obs v1/v2, task obs, reward  smpl_sim/envs/humanoid_env.py:388-403,455-469,565-688
 //   reset             Default / Fall / MoCap                           smpl_sim/envs/humanoid_env.py:471-512
 //
-// Mapping (driven by the round-1 profile, profiles/r1_k_step3_final.md: 4.8 of 32 lanes active, 15.9 KB of shared memory
-// per env -> two waves at 4 096 envs):
+// Mapping (a warp per env kept only ~5 of 32 lanes busy and needed ~16 KB of shared memory per env):
 //   * an env is stepped by LM_LPE = 8 lanes; a lane walks a kinematic chain, one body per sweep step (host list schedule in
 //     LHdr::sched).  Along a chain the sweep state (articulated inertia 21 + bias force 6 inward; pose / velocity /
 //     acceleration outward) is handed from step to step IN REGISTERS; only tree junctions use shared-memory mailboxes;
 //   * per-body results a lane produces in one sweep and consumes itself in a later one (joint factors K = U/D, c = u/D, bias
-//     force) are lane-private "records": they live in Blackwell tensor memory (tcgen05.st / tcgen05.ld, 256 columns per
-//     lane, indexed by the warp-uniform sweep step) -- or in shared memory when the kernel is built with RECT = 0;
+//     force) are lane-private "records", kept per body in the env's shared-memory rows (RECW words a body);
 //   * four fused sweeps per substep instead of seven passes:
 //       S1 outward: stable-PD acceleration (factors of the previous substep) -> torque, kinematics, velocities, bias forces,
 //                   rigid inertias, floor contacts and joint-limit rows
@@ -20,7 +18,8 @@
 //       S3 outward: accelerations, residuals of the constraint rows (working-set test)
 //       [S2'/S3' : active-set Newton iterations, S2' only over the chains that carry rows; row-space exact line search]
 //       S4 inward : semi-implicit Euler of the body's own dofs, then the stable-PD factors (M + h Kd) for the next substep
-//   * everything else per env (~7.9 KB) stays in shared memory so that 28 envs (7 warps) live on one SM: 4 096 envs = one wave.
+//   * everything else per env stays in shared memory too (SMPL: 10.1 KB an env with the records), so that an H100 SM (227 KB
+//     per CTA) holds 16 envs (4 warps) of the table-plus-rows layout; 4 096 envs are two waves over 132 SMs.
 // The mathematics (ABA in world-aligned spatial coordinates about the root origin, MuJoCo's soft-constraint rows as an
 // active-set problem solved by ABA passes) is that of round 1's warp_kernels.cuh; DESIGN.md section 2.
 #pragma once
@@ -42,16 +41,16 @@
 #define L_ST_SELF_CONTACT 32 // SMPLSIM_STATUS_SELF_CONTACT: a geom pair MuJoCo would collide touches (not simulated)
 
 // ------------------------------------------------------------------ compile-time sizes / per-env shared-memory layout (words)
-template <int NB_, int NV_, int NG_, int NS_, int NMBI_, int NMBO_, int NCS_, int NLS_, int RECT_, int SELFCOL_ = 0>
+template <int NB_, int NV_, int NG_, int NS_, int NMBI_, int NMBO_, int NCS_, int NLS_, int SELFCOL_ = 0>
 struct LCfg {
   static constexpr int NB = NB_, NV = NV_, NQ = NV_ + 1, NU = NV_ - 6, NG = NG_, NS = NS_, NMBI = NMBI_, NMBO = NMBO_, NCS = NCS_, NLS = NLS_;
-  static constexpr int RECT = RECT_, SELFCOL = SELFCOL_, LPE = LM_LPE, EPW = 32 / LM_LPE;   // SELFCOL: geom-geom (two-body) rows compiled in
+  static constexpr int SELFCOL = SELFCOL_, LPE = LM_LPE, EPW = 32 / LM_LPE;   // SELFCOL: geom-geom (two-body) rows compiled in
   static constexpr int BODYW = 24, MBIW = 28, MBOW = 32, CONW = 24, LIMW = 8, RECW = 28, ROOTW = 44;
   static constexpr int r4(int n) { return (n + 3) & ~3; }
   static constexpr int qpos = 0, qvel = qpos + r4(NQ), qacc = qvel + r4(NV), act = qacc + r4(NV), tau = act + r4(NU), qstar = tau + r4(NU),
                        body = qstar + r4(NV), mbi = body + BODYW * NB, mbo = mbi + MBIW * NMBI, root = mbo + MBOW * NMBO, con = root + ROOTW,
                        lim = con + CONW * NCS, pfl = lim + LIMW * NLS, PFLW = r4((NS + 3) / 4), misc = pfl + PFLW, tsk = misc + 8,
-                       rec = tsk + 12, total_ = rec + (RECT ? 0 : RECW * NB);
+                       rec = tsk + 12, total_ = rec + RECW * NB;
   static constexpr int total = total_ | 4;   // env stride: a multiple of 4 words (float4 rows) but not of 8 (bank spread)
   // staging of the final kinematics / observation row: aliases the mailboxes, the root's 6 x 6 system and the contact list (dead by then).  When
   // the observation row does not fit beside the xquat rows (SMPL-X) it is written straight to global memory instead.
@@ -86,7 +85,6 @@ struct LCfg {
 #define LBR_X 9
 #define LBR_R10 12
 #define LBR_CI 22
-#define LBR_C2 23   // c of the third hinge (tensor-memory records: K, c0, c1 in columns 0..19, pb in 20..25; no column group is shared)
 // contact entry: [info | cpos 3 | t1 3 | D | aref 4 | phi 4 | r 4 | rs 4]; info: bit0 present, bits1-4 working set, bits 8-15 geom, 16-23 slot
 #define LCE_INFO 0
 #define LCE_CP 1
@@ -116,7 +114,6 @@ struct LLane {
   bool live;
   bool bar;        // CTA barriers are legal here (every warp of the CTA makes this call); false inside warp-divergent redo paths
   int env;
-  unsigned tm;     // tensor-memory address of this warp's record block (RECT = 1)
   float* gscr;     // overflow contact entries of this env (global scratch)
   float* gbody;    // body quaternion (4) + spatial velocity about the root origin (6) of the current forward pass [10 nb] (self-collision; NULL: off)
   int* gpfl;       // working set per contact slot carried across launches (handle-internal scratch, r4(NS / 4) words per env)
@@ -180,82 +177,26 @@ __device__ __forceinline__ V3 l_pyr_dir(const LHdr& H, V3 n, V3 t1, V3 t2, int k
   return n + sg * t;
 }
 
-// ------------------------------------------------------------------ lane records: [K 18 | c 3 | - | pb 6] per (lane, step)
-#ifndef SMPLSIM_EMU
-#define L_TM_LD4(a, r) asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];" : "=r"((r)[0]), "=r"((r)[1]), "=r"((r)[2]), "=r"((r)[3]) : "r"(a))
-#define L_TM_LD8(a, r) asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];" : "=r"((r)[0]), "=r"((r)[1]), "=r"((r)[2]), "=r"((r)[3]), "=r"((r)[4]), "=r"((r)[5]), "=r"((r)[6]), "=r"((r)[7]) : "r"(a))
-#define L_TM_LD16(a, r) asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];" \
-  : "=r"((r)[0]), "=r"((r)[1]), "=r"((r)[2]), "=r"((r)[3]), "=r"((r)[4]), "=r"((r)[5]), "=r"((r)[6]), "=r"((r)[7]), "=r"((r)[8]), "=r"((r)[9]), "=r"((r)[10]), "=r"((r)[11]), "=r"((r)[12]), "=r"((r)[13]), "=r"((r)[14]), "=r"((r)[15]) : "r"(a))
-#define L_TM_ST4(a, r) asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"((r)[0]), "r"((r)[1]), "r"((r)[2]), "r"((r)[3]) : "memory")
-#define L_TM_ST8(a, r) asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(a), "r"((r)[0]), "r"((r)[1]), "r"((r)[2]), "r"((r)[3]), "r"((r)[4]), "r"((r)[5]), "r"((r)[6]), "r"((r)[7]) : "memory")
-#define L_TM_ST16(a, r) asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" \
-  ::"r"(a), "r"((r)[0]), "r"((r)[1]), "r"((r)[2]), "r"((r)[3]), "r"((r)[4]), "r"((r)[5]), "r"((r)[6]), "r"((r)[7]), "r"((r)[8]), "r"((r)[9]), "r"((r)[10]), "r"((r)[11]), "r"((r)[12]), "r"((r)[13]), "r"((r)[14]), "r"((r)[15]) : "memory")
-#define L_TM_WAIT_LD() asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory")
-#define L_TM_WAIT_ST() asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory")
-#else
-static inline uint32_t* emu_tm(unsigned a) {
-  int tid = emu::cur().tid, q = (tid >> 5) & 3;
-  if ((int)(a >> 16) != 32 * q) { fprintf(stderr, "emu: tensor-memory lane field %u of warp %d (quarter %d)\n", a >> 16, tid >> 5, q); abort(); }
-  int col = a & 0xffff;
-  if (col < 0 || col > 512) { fprintf(stderr, "emu: tensor-memory column %d\n", col); abort(); }
-  return emu::g_cta->tmem + (size_t)(32 * q + (tid & 31)) * 512 + col;
-}
-#define L_TM_LDN(a, r, n) do { uint32_t* p_ = emu_tm(a); if (((a) & 0xffff) + (n) > 512) { fprintf(stderr, "emu: tensor-memory overrun\n"); abort(); } for (int i_ = 0; i_ < (n); i_++) (r)[i_] = p_[i_]; } while (0)
-#define L_TM_STN(a, r, n) do { uint32_t* p_ = emu_tm(a); if (((a) & 0xffff) + (n) > 512) { fprintf(stderr, "emu: tensor-memory overrun\n"); abort(); } for (int i_ = 0; i_ < (n); i_++) p_[i_] = (r)[i_]; } while (0)
-#define L_TM_LD4(a, r) L_TM_LDN(a, r, 4)
-#define L_TM_LD8(a, r) L_TM_LDN(a, r, 8)
-#define L_TM_LD16(a, r) L_TM_LDN(a, r, 16)
-#define L_TM_ST4(a, r) L_TM_STN(a, r, 4)
-#define L_TM_ST8(a, r) L_TM_STN(a, r, 8)
-#define L_TM_ST16(a, r) L_TM_STN(a, r, 16)
-#define L_TM_WAIT_LD() do { } while (0)
-#define L_TM_WAIT_ST() do { } while (0)
+// ------------------------------------------------------------------ lane records: [K 18 | c 3 | - | pb 6] per body
+#ifdef SMPLSIM_EMU
 static inline unsigned __float_as_uint(float f) { return emu_bits(f); }
 static inline int __float_as_int(float f) { return (int)emu_bits(f); }
 static inline float __int_as_float(int i) { return emu_float((unsigned)i); }
 static inline float __uint_as_float(unsigned u) { return emu_float(u); }
 #endif
 
-// K (3 x 6) and c (3) of the body this lane runs at step t.  Tensor-memory accesses are warp collectives: every lane of the
-// warp must reach them (callers keep them outside lane-divergent code); `keep` lanes write back what is there.
+// K (3 x 6) and c (3) of body b (b < 0: a lane without a body this step reads body 0's record and ignores it)
 template <class C>
-__device__ __forceinline__ void l_rec_ld_Kc(const unsigned tm, float* sm, int t, int b, float* K, float* c) {
-  if (C::RECT) {
-    unsigned r[20], a = tm + (unsigned)(C::RECW * t);
-    L_TM_LD16(a, r);
-    L_TM_LD4(a + 16u, r + 16);
-    c[2] = (b >= 0) ? sm[C::body + C::BODYW * b + LBR_C2] : 0.f;
-    L_TM_WAIT_LD();
-#pragma unroll
-    for (int i = 0; i < 18; i++) K[i] = __uint_as_float(r[i]);
-    c[0] = __uint_as_float(r[18]); c[1] = __uint_as_float(r[19]);
-  } else {
-    const float4* p = (const float4*)(sm + C::rec + C::RECW * (b < 0 ? 0 : b));
-    float4 v0 = p[0], v1 = p[1], v2 = p[2], v3 = p[3], v4 = p[4], v5 = p[5];
-    K[0] = v0.x; K[1] = v0.y; K[2] = v0.z; K[3] = v0.w; K[4] = v1.x; K[5] = v1.y; K[6] = v1.z; K[7] = v1.w;
-    K[8] = v2.x; K[9] = v2.y; K[10] = v2.z; K[11] = v2.w; K[12] = v3.x; K[13] = v3.y; K[14] = v3.z; K[15] = v3.w;
-    K[16] = v4.x; K[17] = v4.y; c[0] = v4.z; c[1] = v4.w; c[2] = v5.x;
-  }
+__device__ __forceinline__ void l_rec_ld_Kc(float* sm, int b, float* K, float* c) {
+  const float4* p = (const float4*)(sm + C::rec + C::RECW * (b < 0 ? 0 : b));
+  float4 v0 = p[0], v1 = p[1], v2 = p[2], v3 = p[3], v4 = p[4], v5 = p[5];
+  K[0] = v0.x; K[1] = v0.y; K[2] = v0.z; K[3] = v0.w; K[4] = v1.x; K[5] = v1.y; K[6] = v1.z; K[7] = v1.w;
+  K[8] = v2.x; K[9] = v2.y; K[10] = v2.z; K[11] = v2.w; K[12] = v3.x; K[13] = v3.y; K[14] = v3.z; K[15] = v3.w;
+  K[16] = v4.x; K[17] = v4.y; c[0] = v4.z; c[1] = v4.w; c[2] = v5.x;
 }
-// Stores are not waited for here: the sweeps end with one tcgen05.wait::st (a record is read again in a later sweep only).
 template <class C>
-__device__ __forceinline__ void l_rec_st_Kc(const unsigned tm, float* sm, int t, int b, const float* K, const float* c, bool wr, bool preload) {
-  if (C::RECT) {
-    unsigned r[20], a = tm + (unsigned)(C::RECW * t);
-    if (preload) {   // some lanes keep their record (clean chains of a re-sweep): read - select - write
-      L_TM_LD16(a, r);
-      L_TM_LD4(a + 16u, r + 16);
-      L_TM_WAIT_LD();
-    }
-    if (wr || !preload) {   // without a preload the lanes that do not write hold nothing worth keeping: no per-lane select, the registers of K go out as they are
-#pragma unroll
-      for (int i = 0; i < 18; i++) r[i] = __float_as_uint(K[i]);
-      r[18] = __float_as_uint(c[0]); r[19] = __float_as_uint(c[1]);
-    }
-    if (wr && b >= 0) sm[C::body + C::BODYW * b + LBR_C2] = c[2];
-    L_TM_ST16(a, r);
-    L_TM_ST4(a + 16u, r + 16);
-  } else if (wr && b >= 0) {
+__device__ __forceinline__ void l_rec_st_Kc(float* sm, int b, const float* K, const float* c, bool wr) {
+  if (wr && b >= 0) {
     float4* p = (float4*)(sm + C::rec + C::RECW * b);
     p[0] = make_float4(K[0], K[1], K[2], K[3]); p[1] = make_float4(K[4], K[5], K[6], K[7]);
     p[2] = make_float4(K[8], K[9], K[10], K[11]); p[3] = make_float4(K[12], K[13], K[14], K[15]);
@@ -264,35 +205,13 @@ __device__ __forceinline__ void l_rec_st_Kc(const unsigned tm, float* sm, int t,
   }
 }
 template <class C>
-__device__ __forceinline__ S6 l_rec_ld_pb(const unsigned tm, float* sm, int t, int b) {
-  float q[6];
-  if (C::RECT) {
-    unsigned r[8], a = tm + (unsigned)(C::RECW * t + 20);
-    L_TM_LD8(a, r);
-    L_TM_WAIT_LD();
-#pragma unroll
-    for (int i = 0; i < 6; i++) q[i] = __uint_as_float(r[i]);
-  } else {
-    const float* p = sm + C::rec + C::RECW * (b < 0 ? 0 : b) + 22;
-#pragma unroll
-    for (int i = 0; i < 6; i++) q[i] = p[i];
-  }
-  return s6(v3(q[0], q[1], q[2]), v3(q[3], q[4], q[5]));
+__device__ __forceinline__ S6 l_rec_ld_pb(float* sm, int b) {
+  const float* p = sm + C::rec + C::RECW * (b < 0 ? 0 : b) + 22;
+  return s6(v3(p[0], p[1], p[2]), v3(p[3], p[4], p[5]));
 }
 template <class C>
-__device__ __forceinline__ void l_rec_st_pb(const unsigned tm, const bool keep, float* sm, int t, int b, S6 pb, bool wr) {
-  if (C::RECT) {
-    unsigned r[8], a = tm + (unsigned)(C::RECW * t + 20);
-    if (keep) {   // partial re-forward (mj_checkAcc path): the other envs of the warp keep their pb
-      L_TM_LD8(a, r);
-      L_TM_WAIT_LD();
-    }
-    if (wr) {
-      r[0] = __float_as_uint(pb.a.x); r[1] = __float_as_uint(pb.a.y); r[2] = __float_as_uint(pb.a.z);
-      r[3] = __float_as_uint(pb.l.x); r[4] = __float_as_uint(pb.l.y); r[5] = __float_as_uint(pb.l.z);
-    }
-    L_TM_ST8(a, r);
-  } else if (wr && b >= 0) {
+__device__ __forceinline__ void l_rec_st_pb(float* sm, int b, S6 pb, bool wr) {
+  if (wr && b >= 0) {
     float* p = sm + C::rec + C::RECW * b + 22;
     st3(p, pb.a); st3(p + 3, pb.l);
   }
@@ -581,7 +500,6 @@ __device__ __noinline__ LRootOut l_root_out(const float* ms, float* sm, const LL
   const LHdr& H = l_hdr<C>(ms);
   const LBody& lb = l_bodies(ms)[0];
   LRootOut R; R.ncon = 0; R.npresent = 0; R.gbits = 0ull;
-  const unsigned tm = w.tm;
   const bool actv = w.live && w.li == 0;
   S6 pbv = s6(v3(0.f, 0.f, 0.f), v3(0.f, 0.f, 0.f));
   int alloc = 0;
@@ -621,7 +539,7 @@ __device__ __noinline__ LRootOut l_root_out(const float* ms, float* sm, const LL
       }
     }
   }
-  if (flags & LF_VEL) l_rec_st_pb<C>(tm, !w.bar, sm, 0, 0, pbv, actv);
+  if (flags & LF_VEL) l_rec_st_pb<C>(sm, 0, pbv, actv);
   R.ncon = __shfl_sync(L_FULL, alloc, w.gbase);
   __syncwarp();
   return R;
@@ -632,9 +550,8 @@ __device__ __noinline__ LFkOut l_sweep_out(const float* ms, float* sm, const LLa
   const LHdr& H = l_hdr<C>(ms);
   const LBody* MB = l_bodies(ms);
   const LGeom* MG = l_geoms(ms);
-  const unsigned tm = w.tm;   // lane fields the loop uses, copied out of the LLane in memory: the tensor-memory statements clobber memory, every w.x after one is a reload from the stack
   const int li = w.li, T = H.T;
-  const bool live = w.live, keep = !w.bar;
+  const bool live = w.live;
   const float hh = H.h;
   const float h0 = dot(ld3(H.plane_n), ld3(sm + C::qpos) - ld3(H.plane_pos));
   LRootOut R0 = l_root_out<C>(ms, sm, w, flags, h0);
@@ -650,7 +567,7 @@ __device__ __noinline__ LFkOut l_sweep_out(const float* ms, float* sm, const LLa
     const int b = H.sched[t][li];
     const bool actv = live && b >= 0;
     float K[18], kc[3];
-    if (flags & LF_GOUT) l_rec_ld_Kc<C>(tm, sm, t, b, K, kc);
+    if (flags & LF_GOUT) l_rec_ld_Kc<C>(sm, b, K, kc);
     S6 pbv = s6(v3(0.f, 0.f, 0.f), v3(0.f, 0.f, 0.f));
     float* br = sm + C::body + C::BODYW * (actv ? b : 0);
     int alloc = 0, nlr = 0;   // contact entries / limit rows this lane wants
@@ -779,10 +696,9 @@ __device__ __noinline__ LFkOut l_sweep_out(const float* ms, float* sm, const LLa
         npresent += lcnt;
       }
     }
-    if (flags & LF_VEL) l_rec_st_pb<C>(tm, keep, sm, t, b, pbv, actv);
+    if (flags & LF_VEL) l_rec_st_pb<C>(sm, b, pbv, actv);
     __syncwarp();
   }
-  if (C::RECT && (flags & LF_VEL)) L_TM_WAIT_ST();   // pb is read by the inward sweep that follows
   LFkOut o;
   if (flags & LF_COLLIDE) {
     if (w.live && w.li == 0) { ((int*)sm)[C::misc + LMI_NCON] = ncon; ((int*)sm)[C::misc + LMI_NLIM] = min(nlim, C::NLS); ((int*)sm)[C::misc + LMI_NSELF] = 0; }
@@ -1023,8 +939,7 @@ template <class C, bool SPD>
 __device__ __noinline__ bool l_root_in(const float* ms, float* sm, const LLane& w, bool need, int flags) {
   const LHdr& H = l_hdr<C>(ms);
   const LBody& lb = l_bodies(ms)[0];
-  const unsigned tm = w.tm;
-  S6 p = l_rec_ld_pb<C>(tm, sm, 0, 0);
+  S6 p = l_rec_ld_pb<C>(sm, 0);
   bool dirty = false;
   float* rt = sm + C::root;
   if (need && w.li == 0) {
@@ -1119,7 +1034,6 @@ __device__ __noinline__ void l_sweep_in(const float* ms, float* sm, const LLane&
   const LHdr& H = l_hdr<C>(ms);
   const LBody* MB = l_bodies(ms);
   LSolveLane st = st_;
-  const unsigned tm = w.tm;   // lane fields the loop uses, copied out of the LLane in memory: the tensor-memory statements clobber memory, every w.x after one is a reload from the stack
   const int li = w.li;
   const float hh = H.h;
   float cA[21];
@@ -1137,8 +1051,8 @@ __device__ __noinline__ void l_sweep_in(const float* ms, float* sm, const LLane&
     const bool actv = run && b >= 0;
     const bool need = actv && (!resweep || ((st.rc_bits >> t) & 1u));
     if (resweep && !__any_sync(L_FULL, need)) continue;
-    S6 p = l_rec_ld_pb<C>(tm, sm, t, b);
-    float K[18], kc[3];   // written by the lanes that need the body; the others store back what the record holds (or nothing that is read)
+    S6 p = l_rec_ld_pb<C>(sm, b);
+    float K[18], kc[3];   // written by the lanes that need the body; the others leave the record as it is
     if (need) {
       const LBody& lb = MB[b];
       float* br = sm + C::body + C::BODYW * b;
@@ -1204,7 +1118,7 @@ __device__ __noinline__ void l_sweep_in(const float* ms, float* sm, const LLane&
       if (lb.in_mbox >= 0) l_mbi_put(sm + C::mbi + C::MBIW * lb.in_mbox, A, p, dirty);
       if (!spd && !resweep && dirty) st.dirty_bits |= 1u << t;
     }
-    l_rec_st_Kc<C>(tm, sm, t, b, K, kc, need, resweep);
+    l_rec_st_Kc<C>(sm, b, K, kc, need);
     __syncwarp();
   }
   {   // the root body closes the sweep
@@ -1214,7 +1128,6 @@ __device__ __noinline__ void l_sweep_in(const float* ms, float* sm, const LLane&
     if (!resweep || __any_sync(L_FULL, need0)) d0 = l_root_in<C, SPD>(ms, sm, w, need0, flags);
     if (!spd && !resweep && d0 && li == 0) st.dirty_bits |= 1u;
   }
-  if (C::RECT) L_TM_WAIT_ST();   // the records of this sweep are read by the next one
   st_ = st;
 }
 
@@ -1249,7 +1162,6 @@ __device__ __noinline__ bool l_sweep_acc(const float* ms, float* sm, const LLane
   bool same = true;
   float* qout = sm + (to_qstar ? C::qstar : C::qacc);
   const bool stepbar = (H.align & 16) && w.bar;
-  const unsigned tm = w.tm;   // lane fields the loop uses, copied out of the LLane in memory: the tensor-memory statements clobber memory, every w.x after one is a reload from the stack
   const int li = w.li, T = H.T;
   if (stepbar) __syncthreads();
   l_root_acc<C>(ms, sm, w, run, qout, &same);
@@ -1258,7 +1170,7 @@ __device__ __noinline__ bool l_sweep_acc(const float* ms, float* sm, const LLane
     const int b = H.sched[t][li];
     const bool actv = run && b >= 0;
     float K[18], kc[3];
-    l_rec_ld_Kc<C>(tm, sm, t, b, K, kc);
+    l_rec_ld_Kc<C>(sm, b, K, kc);
     if (actv) {
       const LBody& lb = MB[b];
       const float* br = sm + C::body + C::BODYW * b;
@@ -2037,12 +1949,12 @@ extern __shared__ float4 l_smem4[];
 #define L_SMEM ((float*)l_smem4)
 #endif
 
-// CTA prologue: stage the constant table, carve the env rows, claim tensor memory.  Shared memory: [table | 4 words | env rows]
+// CTA prologue: stage the constant table, carve the env rows.  Shared memory: [table | 4 words | env rows]
 template <class C>
 __device__ __forceinline__ float* l_setup(const float* __restrict__ gimg, int img_bytes, LLane& w, const float*& ms, int n, const LMap& map, float* gscr, float* gsens, int* gpfl, float* gbody = nullptr) {
   float* smem = L_SMEM;
   if (map.blk_img) gimg += (size_t)map.blk_img[blockIdx.x] * (size_t)(img_bytes / 4);   // this CTA's body shape
-  unsigned* slot = (unsigned*)(smem + img_bytes / 4);   // [0] tensor-memory base, [2..3] mbarrier of the table copy
+  unsigned* slot = (unsigned*)(smem + img_bytes / 4);   // [2..3] mbarrier of the table copy
 #ifndef SMPLSIM_EMU
   {
     // the constant table arrives as ONE bulk asynchronous copy (TMA engine, cp.async.bulk -> UBLKCP) signalled on an mbarrier: one thread
@@ -2062,22 +1974,8 @@ __device__ __forceinline__ float* l_setup(const float* __restrict__ gimg, int im
 #endif
   ms = smem;
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5, wpb = blockDim.x >> 5;
-  unsigned tbase = 0u;
-#ifndef SMPLSIM_EMU
-  if (C::RECT) {
-    if (wib == 0) {
-      unsigned sa = (unsigned)__cvta_generic_to_shared(slot);
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(sa) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  }
-#else
-  if (threadIdx.x == 0) *slot = 0u;
-#endif
   __syncthreads();
 #ifndef SMPLSIM_EMU
-  if (C::RECT) asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
   {   // one thread starts the copy; every thread waits for the table (phase 0 of the mbarrier)
     const unsigned mb = (unsigned)__cvta_generic_to_shared(slot + 2), dst = (unsigned)__cvta_generic_to_shared(smem);
     if (threadIdx.x == 0) {
@@ -2091,7 +1989,6 @@ __device__ __forceinline__ float* l_setup(const float* __restrict__ gimg, int im
     }
   }
 #endif
-  if (C::RECT) tbase = *slot;
   const int sub = lane / LM_LPE;
   w.lane = lane; w.li = lane % LM_LPE; w.gbase = sub * LM_LPE;
   w.gmask = ((1u << LM_LPE) - 1u) << (sub * LM_LPE);
@@ -2099,26 +1996,11 @@ __device__ __forceinline__ float* l_setup(const float* __restrict__ gimg, int im
   if (map.slot_env) w.env = map.slot_env[w.env];
   w.live = w.env >= 0 && w.env < n;
   w.bar = true;
-  // tensor memory: a warp reaches the 32 lanes of its quarter (warp id mod 4); warps 4.. take the upper 256 columns
-  w.tm = tbase + ((unsigned)((wib & 3) * 32) << 16) + (unsigned)((wib >> 2) * 256);
   w.gscr = gscr + (size_t)(w.live ? w.env : 0) * (size_t)(C::CONW * (C::NS - C::NCS));
   w.gbody = gbody ? gbody + (size_t)(w.live ? w.env : 0) * (size_t)(10 * C::NB) : nullptr;
   w.gpfl = gpfl ? gpfl + (size_t)(w.live ? w.env : 0) * (size_t)C::PFLW : nullptr;
   w.gsens = gsens ? gsens + (size_t)(w.live ? w.env : 0) * (size_t)(6 * C::NB) : nullptr;
   return smem + img_bytes / 4 + 4 + (size_t)(wib * C::EPW + sub) * C::total;
-}
-template <class C>
-__device__ __forceinline__ void l_teardown(const float* ms) {
-#ifndef SMPLSIM_EMU
-  if (C::RECT) {
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if ((threadIdx.x >> 5) == 0) {
-      unsigned tb = *(const unsigned*)(ms + ((const LHdr*)ms)->bytes / 4);
-      asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tb) : "memory");
-    }
-  }
-#endif
 }
 
 // stable PD, stale inertia (quirk Q1): rebuild the (M + h Kd) factors of the state of the last forward pass for the current
@@ -2197,7 +2079,6 @@ __global__ void __launch_bounds__(256, 1) k_step5(const float* __restrict__ gimg
   l_copy_out<C>(a.st.qacc_warm + eo * H.nv, sm + C::qacc, H.nv, w);
   if (w.live && w.gpfl) for (int i = w.li; i < (H.nslot + 3) / 4; i += LM_LPE) w.gpfl[i] = ((const int*)sm)[C::pfl + i];
   if (a.mode == 0) l_task_io<C>(sm, w, a.st, true);
-  l_teardown<C>(ms);
 }
 
 template <class C>
@@ -2273,7 +2154,6 @@ __global__ void __launch_bounds__(256, 1) k_reset5(const float* __restrict__ gim
   l_copy_out<C>(a.st.qacc_warm + eo * H.nv, sm + C::qacc, H.nv, w);
   if (w.live && w.gpfl) for (int i = w.li; i < (H.nslot + 3) / 4; i += LM_LPE) w.gpfl[i] = ((const int*)sm)[C::pfl + i];
   l_task_io<C>(sm, w, a.st, true);
-  l_teardown<C>(ms);
 }
 
 // mujoco.mj_kinematics (humanoid_env.py:389) / poselib global_transformation on caller-supplied qpos rows
@@ -2291,5 +2171,4 @@ __global__ void __launch_bounds__(256, 1) k_kin5(const float* __restrict__ gimg,
     for (int b = w.li; b < H.nb; b += LM_LPE) st3(a.xpos + (eo * H.nb + b) * 3, ld3(sm + C::body + C::BODYW * b + LBR_X) + root);
     l_copy<C>(a.xquat + eo * H.nb * 4, sm + C::xq, 4 * H.nb, w);
   }
-  l_teardown<C>(ms);
 }

@@ -18,9 +18,9 @@
 #endif
 
 // model classes the kernels are instantiated for: <bodies, dofs, geoms, contact slots, in-mailboxes, out-mailboxes, contact
-// entries in shared memory, limit rows, records in tensor memory, geom-geom rows compiled in>
-#define L_SMPL(RECT, SC) LCfg<24, 75, 24, 64, 5, 2, 20, 16, RECT, SC>
-#define L_SMPLX(RECT, SC) LCfg<52, 159, 52, 128, 13, 4, 14, 16, RECT, SC>   // sized so that 16 envs (4 warps) fit one SM
+// entries in shared memory, limit rows, geom-geom rows compiled in>
+#define L_SMPL(SC) LCfg<24, 75, 24, 64, 5, 2, 20, 16, SC>
+#define L_SMPLX(SC) LCfg<52, 159, 52, 128, 13, 4, 14, 16, SC>
 
 struct SmplsimHandle {
   LaneImage img;
@@ -29,9 +29,8 @@ struct SmplsimHandle {
   float* gsens = nullptr;  // body velocities of the last forward pass (obs v2 / aux)
   int* gpfl = nullptr;     // working set per contact slot, carried from call to call (solver warm start only)
   float* gbody = nullptr;  // body pose / velocity of the current forward pass (self-collision narrow phase)
-  int num_envs = 0, device = 0, nsm = 148, max_smem = 0;
+  int num_envs = 0, device = 0, nsm = 132, max_smem = 0;
   int cls = 0;             // 1 SMPL class, 2 SMPL-X class
-  int rect = 1;            // lane records in tensor memory (1) or shared memory (0)
   int selfcol = 0;         // cfg.env.self_collision: kernels with the geom-geom rows compiled in
   int wpb = 0;             // warps per CTA
   size_t smem = 0, env_words = 0;
@@ -76,7 +75,6 @@ static long count_blocks(const SmplsimHandle* h, long per) {
 // warps per CTA: fewest waves over the SMs first, then the fewest warps (an SM issues faster for few resident warps)
 template <class C>
 static int pick_wpb(SmplsimHandle* h) {
-  const LHdr& H = *h->img.hdr();
   int best = 0;
   long best_waves = 1L << 60;
   int forced = 0;
@@ -84,7 +82,6 @@ static int pick_wpb(SmplsimHandle* h) {
   for (int wpb = 1; wpb <= 8; wpb++) {
     if (forced && wpb != forced) continue;
     if (cta_smem<C>(h, wpb) > (size_t)h->max_smem) continue;
-    if (C::RECT && C::RECW * H.T > (wpb > 4 ? 256 : 512)) continue;
     long per = (long)wpb * C::EPW, blocks = count_blocks(h, per), waves = (blocks + h->nsm - 1) / h->nsm;
     if (waves < best_waves) { best_waves = waves; best = wpb; }
   }
@@ -113,18 +110,14 @@ static void run_kin(SmplsimHandle* h, const LKinArgs& a, cudaStream_t st) {
   int wpb = h->wpb, per = wpb * C::EPW;
   L_LAUNCH(k_kin5<C>, h->nblocks ? h->nblocks : (a.n + per - 1) / per, 32 * wpb, h->smem, st, h->dimg, h->img.hdr()->bytes, a);
 }
-// dispatch over (model class, record placement, self-collision)
+// dispatch over (model class, self-collision)
 #define L_DISPATCH(h, CALL)                                                   \
   do {                                                                        \
-    switch (((h)->cls << 2) | ((h)->rect << 1) | (h)->selfcol) {              \
-      case (1 << 2) | 0: { typedef L_SMPL(0, 0) C_; CALL; } break;            \
-      case (1 << 2) | 1: { typedef L_SMPL(0, 1) C_; CALL; } break;            \
-      case (1 << 2) | 2: { typedef L_SMPL(1, 0) C_; CALL; } break;            \
-      case (1 << 2) | 3: { typedef L_SMPL(1, 1) C_; CALL; } break;            \
-      case (2 << 2) | 0: { typedef L_SMPLX(0, 0) C_; CALL; } break;           \
-      case (2 << 2) | 1: { typedef L_SMPLX(0, 1) C_; CALL; } break;           \
-      case (2 << 2) | 2: { typedef L_SMPLX(1, 0) C_; CALL; } break;           \
-      default: { typedef L_SMPLX(1, 1) C_; CALL; } break;                     \
+    switch (((h)->cls << 1) | (h)->selfcol) {                                 \
+      case (1 << 1) | 0: { typedef L_SMPL(0) C_; CALL; } break;               \
+      case (1 << 1) | 1: { typedef L_SMPL(1) C_; CALL; } break;               \
+      case (2 << 1) | 0: { typedef L_SMPLX(0) C_; CALL; } break;              \
+      default: { typedef L_SMPLX(1) C_; CALL; } break;                        \
     }                                                                         \
   } while (0)
 
@@ -174,7 +167,7 @@ static int create_impl(const SmplsimModelDesc* s, int nmodels, const int32_t* en
   }
   h->nmodels = nmodels;
   if (env_model && nmodels > 1) h->env_model.assign(env_model, env_model + num_envs);
-  typedef L_SMPL(0, 0) CS; typedef L_SMPLX(0, 0) CX;
+  typedef L_SMPL(0) CS; typedef L_SMPLX(0) CX;
   if (H.nb == CS::NB && H.nv == CS::NV && H.ng <= CS::NG && H.nslot <= CS::NS && H.nmbi <= CS::NMBI && H.nmbo <= CS::NMBO) h->cls = 1;
   else if (H.nb == CX::NB && H.nv == CX::NV && H.ng <= CX::NG && H.nslot <= CX::NS && H.nmbi <= CX::NMBI && H.nmbo <= CX::NMBO) h->cls = 2;
   else {
@@ -191,10 +184,9 @@ static int create_impl(const SmplsimModelDesc* s, int nmodels, const int32_t* en
   if (e == cudaSuccess) e = cudaDeviceGetAttribute(&h->nsm, cudaDevAttrMultiProcessorCount, cuda_device);
 #endif
   if (e != cudaSuccess) { delete h; return fail(SMPLSIM_ECUDA, std::string("smplsim_create: ") + cudaGetErrorString(e)); }
-  if (const char* r = std::getenv("SMPLSIM_REC")) h->rect = (std::string(r) == "smem") ? 0 : 1;
   int ok = 0;
   L_DISPATCH(h, ok = pick_wpb<C_>(h));
-  if (ok <= 0) { delete h; return fail(SMPLSIM_EUNSUPPORTED, "per-env rows exceed shared memory / tensor memory"); }
+  if (ok <= 0) { delete h; return fail(SMPLSIM_EUNSUPPORTED, "per-env rows exceed shared memory"); }
   size_t gs = 0;
   L_DISPATCH(h, gs = (size_t)C_::CONW * (C_::NS - C_::NCS));
   e = cudaMalloc(&h->dimg, (size_t)H.bytes * nmodels);
@@ -229,8 +221,8 @@ static int create_impl(const SmplsimModelDesc* s, int nmodels, const int32_t* en
   if (e == cudaSuccess && cfg->self_collision) e = cudaMalloc(&h->gbody, (size_t)10 * H.nb * num_envs * 4);
   if (e != cudaSuccess) { free_handle(h); return fail(SMPLSIM_ECUDA, std::string("smplsim_create: ") + cudaGetErrorString(e)); }
   if (std::getenv("SMPLSIM_DEBUG"))
-    fprintf(stderr, "smplsim_create: class %d, %d bodies, schedule %d steps, mailboxes %d in / %d out, %d geom pairs, table %d B, %zu B per env, %d warps per CTA, %zu B shared memory per CTA, records in %s, self-collision %d\n",
-            h->cls, H.nb, H.T, H.nmbi, H.nmbo, H.npair, H.bytes, h->env_words * 4, h->wpb, h->smem, h->rect ? "tensor memory" : "shared memory", h->selfcol);
+    fprintf(stderr, "smplsim_create: class %d, %d bodies, schedule %d steps, mailboxes %d in / %d out, %d geom pairs, table %d B, %zu B per env, %d warps per CTA, %zu B shared memory per CTA, self-collision %d\n",
+            h->cls, H.nb, H.T, H.nmbi, H.nmbo, H.npair, H.bytes, h->env_words * 4, h->wpb, h->smem, h->selfcol);
   *out = h;
   return SMPLSIM_OK;
 }
@@ -257,8 +249,6 @@ extern "C" int smplsim_warps_per_block(const SmplsimHandle* h) { return h ? h->w
 /* 5: lane-chain kernels (lane_kernels.cuh) */
 extern "C" int smplsim_kernel_version(const SmplsimHandle* h) { return h ? 5 : SMPLSIM_EINVAL; }
 extern "C" int smplsim_schedule_steps(const SmplsimHandle* h) { return h ? h->img.hdr()->T : SMPLSIM_EINVAL; }
-/* 1: lane records in tensor memory, 0: in shared memory (SMPLSIM_REC=smem) */
-extern "C" int smplsim_records_in_tmem(const SmplsimHandle* h) { return h ? h->rect : SMPLSIM_EINVAL; }
 
 static bool state_ok(const SmplsimState* st) {
   return st && st->qpos && st->qvel && st->qpos_fwd && st->qvel_fwd && st->qacc_warm && st->task_target && st->task_change_step &&

@@ -33,7 +33,6 @@ void launch(dim3 grid, dim3 block, size_t smem, const std::function<void()>& bod
   c.warp.resize((nt + 31) / 32);
   c.bdim = block; c.gdim = grid;
   c.smem = (char*)aligned_alloc(128, ((smem + 127) / 128 + 1) * 128);
-  c.tmem = (uint32_t*)calloc(128 * 512, 4);
   c.body = body;
   for (int i = 0; i < nt; i++) c.th[i].stack = (char*)malloc(kStack);
   Cta* prev = g_cta;
@@ -80,6 +79,5 @@ void launch(dim3 grid, dim3 block, size_t smem, const std::function<void()>& bod
   g_cta = prev;
   for (int i = 0; i < nt; i++) free(c.th[i].stack);
   free(c.smem);
-  free(c.tmem);
 }
 }  // namespace emu

@@ -5,7 +5,7 @@
 // the very kernel source against the oracle on a machine without a GPU.  Every CUDA thread of a CTA is a ucontext
 // coroutine; warp collectives (__shfl_sync, __ballot_sync, __syncwarp, ...) and __syncthreads are rendezvous points of the
 // cooperative scheduler, so mis-synchronised code deadlocks here (reported) instead of silently racing.  Shared memory is
-// one heap block per CTA, tensor memory (tcgen05 ld/st used as lane-private scratch) a 128-lane x 512-column array.
+// one heap block per CTA.
 // Nothing under smplsim_b200/ includes or links this.
 #pragma once
 #include <math.h>
@@ -88,7 +88,6 @@ struct Cta {
   int or_acc[2];
   dim3 bidx, bdim, gdim;
   char* smem;
-  uint32_t* tmem;   // [128][512]
   std::function<void()> body;
   ucontext_t sched;
   int cur;

@@ -165,7 +165,8 @@ def gen_obs(model_name, nb, nu, seed, B=48):
         gu_rew.append(HG.height_reward(np.array([[tar_h[i]]]), xpos[i:i + 1, 0])[0])
     out.update(tar_speed=tar_speed, tar_pos=tar_pos, prev_root=prev_root, tar_h=tar_h, speed_obs=np.array(sp_obs),
                reach_obs=np.array(rc_obs), speed_rew=np.array(sp_rew), reach_rew=np.array(rc_rew), getup_rew=np.array(gu_rew))
-    np.savez_compressed(os.path.join(HERE, f"obs_{model_name}.npz"), **out)
+    # the first 40 of the B states are stored (same random stream as before): each fixture stays below 1 MB
+    np.savez_compressed(os.path.join(HERE, f"obs_{model_name}.npz"), **{k: v[:40] for k, v in out.items()})
     print(f"obs_{model_name}.npz: v1 {out['v1_u0h1'].shape} v2 {out['v2_u0h1'].shape}; "
           f"K-7a sum v2 = {out['v2_u0h1'][0].sum() - out['v2_u0h1'][0][-6 * nb:].sum():.4f}")
 
