@@ -10,7 +10,7 @@
 //     LHdr::sched).  Along a chain the sweep state (articulated inertia 21 + bias force 6 inward; pose / velocity /
 //     acceleration outward) is handed from step to step IN REGISTERS; only tree junctions use shared-memory mailboxes;
 //   * per-body results a lane produces in one sweep and consumes itself in a later one (joint factors K = U/D, c = u/D, bias
-//     force) are lane-private "records", kept per body in the env's shared-memory rows (RECW words a body);
+//     force) are lane-private "records", kept per body in the env's global scratch (RECW words a body, L2-resident);
 //   * four fused sweeps per substep instead of seven passes:
 //       S1 outward: stable-PD acceleration (factors of the previous substep) -> torque, kinematics, velocities, bias forces,
 //                   rigid inertias, floor contacts and joint-limit rows
@@ -18,8 +18,8 @@
 //       S3 outward: accelerations, residuals of the constraint rows (working-set test)
 //       [S2'/S3' : active-set Newton iterations, S2' only over the chains that carry rows; row-space exact line search]
 //       S4 inward : semi-implicit Euler of the body's own dofs, then the stable-PD factors (M + h Kd) for the next substep
-//   * everything else per env stays in shared memory too (SMPL: 10.1 KB an env with the records), so that an H100 SM (227 KB
-//     per CTA) holds 16 envs (4 warps) of the table-plus-rows layout; 4 096 envs are two waves over 132 SMs.
+//   * everything else per env stays in shared memory (SMPL: 6.7 KB an env), so that an H100 SM (227 KB per CTA) holds 32 envs
+//     (8 warps) of the table-plus-rows layout; 4 096 envs are one wave over 132 SMs.
 // The mathematics (ABA in world-aligned spatial coordinates about the root origin, MuJoCo's soft-constraint rows as an
 // active-set problem solved by ABA passes) is that of round 1's warp_kernels.cuh; DESIGN.md section 2.
 #pragma once
@@ -47,11 +47,14 @@ struct LCfg {
   static constexpr int SELFCOL = SELFCOL_, LPE = LM_LPE, EPW = 32 / LM_LPE;   // SELFCOL: geom-geom (two-body) rows compiled in
   static constexpr int BODYW = 24, MBIW = 28, MBOW = 32, CONW = 24, LIMW = 8, RECW = 28, ROOTW = 44;
   static constexpr int r4(int n) { return (n + 3) & ~3; }
-  static constexpr int qpos = 0, qvel = qpos + r4(NQ), qacc = qvel + r4(NV), act = qacc + r4(NV), tau = act + r4(NU), qstar = tau + r4(NU),
-                       body = qstar + r4(NV), mbi = body + BODYW * NB, mbo = mbi + MBIW * NMBI, root = mbo + MBOW * NMBO, con = root + ROOTW,
+  static constexpr int qpos = 0, qvel = qpos + r4(NQ), qacc = qvel + r4(NV), act = qacc + r4(NV), tau = act + r4(NU),
+                       body = tau + r4(NU), mbi = body + BODYW * NB, mbo = mbi + MBIW * NMBI, root = mbo + MBOW * NMBO, con = root + ROOTW,
                        lim = con + CONW * NCS, pfl = lim + LIMW * NLS, PFLW = r4((NS + 3) / 4), misc = pfl + PFLW, tsk = misc + 8,
-                       rec = tsk + 12, total_ = rec + RECW * NB;
+                       total_ = tsk + 12;
   static constexpr int total = total_ | 4;   // env stride: a multiple of 4 words (float4 rows) but not of 8 (bank spread)
+  // per-env global scratch (L2-resident): the lane records, the line search's trial accelerations (qstar) and the contact entries
+  // past NCS.  Keeping the records and qstar out of shared memory is what lets 32 SMPL envs (8 warps) and the table share one SM.
+  static constexpr int grec = 0, gqstar = grec + RECW * NB, gcon = gqstar + r4(NV), GSCRW = gcon + CONW * (NS - NCS);
   // staging of the final kinematics / observation row: aliases the mailboxes, the root's 6 x 6 system and the contact list (dead by then).  When
   // the observation row does not fit beside the xquat rows (SMPL-X) it is written straight to global memory instead.
   static constexpr int OBSW = 4 * ((NB * 18 + 16 + 3) / 4);
@@ -114,7 +117,7 @@ struct LLane {
   bool live;
   bool bar;        // CTA barriers are legal here (every warp of the CTA makes this call); false inside warp-divergent redo paths
   int env;
-  float* gscr;     // overflow contact entries of this env (global scratch)
+  float* gscr;     // this env's global scratch: lane records, qstar, overflow contact entries (LCfg::GSCRW words)
   float* gbody;    // body quaternion (4) + spatial velocity about the root origin (6) of the current forward pass [10 nb] (self-collision; NULL: off)
   int* gpfl;       // working set per contact slot carried across launches (handle-internal scratch, r4(NS / 4) words per env)
   float* gsens;    // framelinvel / frameangvel of the last forward pass [6 nb] of this env (global scratch; NULL: not wanted)
@@ -187,17 +190,17 @@ static inline float __uint_as_float(unsigned u) { return emu_float(u); }
 
 // K (3 x 6) and c (3) of body b (b < 0: a lane without a body this step reads body 0's record and ignores it)
 template <class C>
-__device__ __forceinline__ void l_rec_ld_Kc(float* sm, int b, float* K, float* c) {
-  const float4* p = (const float4*)(sm + C::rec + C::RECW * (b < 0 ? 0 : b));
+__device__ __forceinline__ void l_rec_ld_Kc(const LLane& w, int b, float* K, float* c) {
+  const float4* p = (const float4*)(w.gscr + C::grec + C::RECW * (b < 0 ? 0 : b));
   float4 v0 = p[0], v1 = p[1], v2 = p[2], v3 = p[3], v4 = p[4], v5 = p[5];
   K[0] = v0.x; K[1] = v0.y; K[2] = v0.z; K[3] = v0.w; K[4] = v1.x; K[5] = v1.y; K[6] = v1.z; K[7] = v1.w;
   K[8] = v2.x; K[9] = v2.y; K[10] = v2.z; K[11] = v2.w; K[12] = v3.x; K[13] = v3.y; K[14] = v3.z; K[15] = v3.w;
   K[16] = v4.x; K[17] = v4.y; c[0] = v4.z; c[1] = v4.w; c[2] = v5.x;
 }
 template <class C>
-__device__ __forceinline__ void l_rec_st_Kc(float* sm, int b, const float* K, const float* c, bool wr) {
+__device__ __forceinline__ void l_rec_st_Kc(const LLane& w, int b, const float* K, const float* c, bool wr) {
   if (wr && b >= 0) {
-    float4* p = (float4*)(sm + C::rec + C::RECW * b);
+    float4* p = (float4*)(w.gscr + C::grec + C::RECW * b);
     p[0] = make_float4(K[0], K[1], K[2], K[3]); p[1] = make_float4(K[4], K[5], K[6], K[7]);
     p[2] = make_float4(K[8], K[9], K[10], K[11]); p[3] = make_float4(K[12], K[13], K[14], K[15]);
     p[4] = make_float4(K[16], K[17], c[0], c[1]);
@@ -205,14 +208,14 @@ __device__ __forceinline__ void l_rec_st_Kc(float* sm, int b, const float* K, co
   }
 }
 template <class C>
-__device__ __forceinline__ S6 l_rec_ld_pb(float* sm, int b) {
-  const float* p = sm + C::rec + C::RECW * (b < 0 ? 0 : b) + 22;
+__device__ __forceinline__ S6 l_rec_ld_pb(const LLane& w, int b) {
+  const float* p = w.gscr + C::grec + C::RECW * (b < 0 ? 0 : b) + 22;
   return s6(v3(p[0], p[1], p[2]), v3(p[3], p[4], p[5]));
 }
 template <class C>
-__device__ __forceinline__ void l_rec_st_pb(float* sm, int b, S6 pb, bool wr) {
+__device__ __forceinline__ void l_rec_st_pb(const LLane& w, int b, S6 pb, bool wr) {
   if (wr && b >= 0) {
-    float* p = sm + C::rec + C::RECW * b + 22;
+    float* p = w.gscr + C::grec + C::RECW * b + 22;
     st3(p, pb.a); st3(p + 3, pb.l);
   }
 }
@@ -220,7 +223,7 @@ __device__ __forceinline__ void l_rec_st_pb(float* sm, int b, S6 pb, bool wr) {
 // contact entry c: the first NCS live in shared memory, the rest in this env's global scratch
 template <class C>
 __device__ __forceinline__ float* l_centry(float* sm, const LLane& w, int c) {
-  return c < C::NCS ? sm + C::con + C::CONW * c : w.gscr + (size_t)C::CONW * (c - C::NCS);
+  return c < C::NCS ? sm + C::con + C::CONW * c : w.gscr + C::gcon + (size_t)C::CONW * (c - C::NCS);
 }
 
 // S of hinge k of body row br (axis in world coordinates, moment about the root origin)
@@ -356,7 +359,7 @@ template <class C>
 __device__ __forceinline__ bool l_rows_eval(const LHdr& H, float* sm, const LLane& w, int cb, int cn, S6 a) {
   bool same = true;
   for (int c = cb; c < cb + cn; c++) {
-    float* ce = (c < C::NCS) ? nullptr : w.gscr + (size_t)C::CONW * (c - C::NCS);
+    float* ce = (c < C::NCS) ? nullptr : w.gscr + C::gcon + (size_t)C::CONW * (c - C::NCS);
     float e[12];
     if (c < C::NCS) l_ld12(sm + C::con + C::CONW * c, e);
     else for (int j = 0; j < 12; j++) e[j] = ce[j];
@@ -480,13 +483,13 @@ __device__ __forceinline__ int l_narrow(const LHdr& H, const LGeom& G, int g, co
 #endif
     const int c = cb + cnt;
     if (c < C::NCS) l_st12(sm + C::con + C::CONW * c, e);
-    else { float* ce = w.gscr + (size_t)C::CONW * (c - C::NCS); for (int j = 0; j < 12; j++) ce[j] = e[j]; }
+    else { float* ce = w.gscr + C::gcon + (size_t)C::CONW * (c - C::NCS); for (int j = 0; j < 12; j++) ce[j] = e[j]; }
     cnt++;
   }
   for (int i = cnt; i < alloc; i++) {
     const int c = cb + i;
     if (c < C::NCS) ((int*)(sm + C::con + C::CONW * c))[LCE_INFO] = 0;
-    else ((int*)(w.gscr + (size_t)C::CONW * (c - C::NCS)))[LCE_INFO] = 0;
+    else ((int*)(w.gscr + C::gcon + (size_t)C::CONW * (c - C::NCS)))[LCE_INFO] = 0;
   }
   return cnt;
 }
@@ -539,7 +542,7 @@ __device__ __noinline__ LRootOut l_root_out(const float* ms, float* sm, const LL
       }
     }
   }
-  if (flags & LF_VEL) l_rec_st_pb<C>(sm, 0, pbv, actv);
+  if (flags & LF_VEL) l_rec_st_pb<C>(w, 0, pbv, actv);
   R.ncon = __shfl_sync(L_FULL, alloc, w.gbase);
   __syncwarp();
   return R;
@@ -567,7 +570,7 @@ __device__ __noinline__ LFkOut l_sweep_out(const float* ms, float* sm, const LLa
     const int b = H.sched[t][li];
     const bool actv = live && b >= 0;
     float K[18], kc[3];
-    if (flags & LF_GOUT) l_rec_ld_Kc<C>(sm, b, K, kc);
+    if (flags & LF_GOUT) l_rec_ld_Kc<C>(w, b, K, kc);
     S6 pbv = s6(v3(0.f, 0.f, 0.f), v3(0.f, 0.f, 0.f));
     float* br = sm + C::body + C::BODYW * (actv ? b : 0);
     int alloc = 0, nlr = 0;   // contact entries / limit rows this lane wants
@@ -696,7 +699,7 @@ __device__ __noinline__ LFkOut l_sweep_out(const float* ms, float* sm, const LLa
         npresent += lcnt;
       }
     }
-    if (flags & LF_VEL) l_rec_st_pb<C>(sm, b, pbv, actv);
+    if (flags & LF_VEL) l_rec_st_pb<C>(w, b, pbv, actv);
     __syncwarp();
   }
   LFkOut o;
@@ -731,7 +734,7 @@ __device__ __forceinline__ void l_fold_contacts(const LHdr& H, float* sm, const 
   for (int c = cb; c < cb + cn; c++) {
     float e[12];
     if (c < C::NCS) l_ld12(sm + C::con + C::CONW * c, e);
-    else { const float* ce = w.gscr + (size_t)C::CONW * (c - C::NCS); for (int j = 0; j < 12; j++) e[j] = ce[j]; }
+    else { const float* ce = w.gscr + C::gcon + (size_t)C::CONW * (c - C::NCS); for (int j = 0; j < 12; j++) e[j] = ce[j]; }
     const int info = __float_as_int(e[0]);
     if (!(info & 1) || !(info & 30)) continue;
     V3 cpt = v3(e[1], e[2], e[3]), t1 = v3(e[4], e[5], e[6]);
@@ -939,7 +942,7 @@ template <class C, bool SPD>
 __device__ __noinline__ bool l_root_in(const float* ms, float* sm, const LLane& w, bool need, int flags) {
   const LHdr& H = l_hdr<C>(ms);
   const LBody& lb = l_bodies(ms)[0];
-  S6 p = l_rec_ld_pb<C>(sm, 0);
+  S6 p = l_rec_ld_pb<C>(w, 0);
   bool dirty = false;
   float* rt = sm + C::root;
   if (need && w.li == 0) {
@@ -1051,7 +1054,7 @@ __device__ __noinline__ void l_sweep_in(const float* ms, float* sm, const LLane&
     const bool actv = run && b >= 0;
     const bool need = actv && (!resweep || ((st.rc_bits >> t) & 1u));
     if (resweep && !__any_sync(L_FULL, need)) continue;
-    S6 p = l_rec_ld_pb<C>(sm, b);
+    S6 p = l_rec_ld_pb<C>(w, b);
     float K[18], kc[3];   // written by the lanes that need the body; the others leave the record as it is
     if (need) {
       const LBody& lb = MB[b];
@@ -1118,7 +1121,7 @@ __device__ __noinline__ void l_sweep_in(const float* ms, float* sm, const LLane&
       if (lb.in_mbox >= 0) l_mbi_put(sm + C::mbi + C::MBIW * lb.in_mbox, A, p, dirty);
       if (!spd && !resweep && dirty) st.dirty_bits |= 1u << t;
     }
-    l_rec_st_Kc<C>(sm, b, K, kc, need);
+    l_rec_st_Kc<C>(w, b, K, kc, need);
     __syncwarp();
   }
   {   // the root body closes the sweep
@@ -1160,7 +1163,7 @@ __device__ __noinline__ bool l_sweep_acc(const float* ms, float* sm, const LLane
   const LBody* MB = l_bodies(ms);
   S6 ca = s6(v3(0.f, 0.f, 0.f), v3(0.f, 0.f, 0.f));
   bool same = true;
-  float* qout = sm + (to_qstar ? C::qstar : C::qacc);
+  float* qout = to_qstar ? w.gscr + C::gqstar : sm + C::qacc;
   const bool stepbar = (H.align & 16) && w.bar;
   const int li = w.li, T = H.T;
   if (stepbar) __syncthreads();
@@ -1170,7 +1173,7 @@ __device__ __noinline__ bool l_sweep_acc(const float* ms, float* sm, const LLane
     const int b = H.sched[t][li];
     const bool actv = run && b >= 0;
     float K[18], kc[3];
-    l_rec_ld_Kc<C>(sm, b, K, kc);
+    l_rec_ld_Kc<C>(w, b, K, kc);
     if (actv) {
       const LBody& lb = MB[b];
       const float* br = sm + C::body + C::BODYW * b;
@@ -1509,10 +1512,10 @@ __device__ __noinline__ int l_solve(const float* ms, float* sm, const LLane& w, 
       bool step = lsrch && (al > 0.f);
       if (lsrch && !step) { run = false; iters = it; }
       l_rows<C>(sm, w, step, 2, al, o4);
-      if (step) for (int d = w.li; d < H.nv; d += LM_LPE) sm[C::qacc + d] = fmaf(al, sm[C::qstar + d] - sm[C::qacc + d], sm[C::qacc + d]);
+      if (step) for (int d = w.li; d < H.nv; d += LM_LPE) sm[C::qacc + d] = fmaf(al, w.gscr[C::gqstar + d] - sm[C::qacc + d], sm[C::qacc + d]);
     }
     if (fin) {
-      for (int d = w.li; d < H.nv; d += LM_LPE) sm[C::qacc + d] = sm[C::qstar + d];
+      for (int d = w.li; d < H.nv; d += LM_LPE) sm[C::qacc + d] = w.gscr[C::gqstar + d];
       run = false; iters = it;
     }
     __syncwarp();
@@ -1746,7 +1749,7 @@ struct LStepArgs {
   float* reward;
   uint8_t* terminated;
   uint8_t* truncated;
-  float* gscr;       // [n, (NS - NCS) * CONW] overflow contact entries
+  float* gscr;       // [n, GSCRW] lane records, qstar, overflow contact entries
   float* gsens;      // [n, 6 nb] or NULL
   float* gbody;      // [n, 10 nb] or NULL (self-collision)
   int* gpfl;         // [n, r4(NS / 4)] working set per contact slot
@@ -1996,7 +1999,7 @@ __device__ __forceinline__ float* l_setup(const float* __restrict__ gimg, int im
   if (map.slot_env) w.env = map.slot_env[w.env];
   w.live = w.env >= 0 && w.env < n;
   w.bar = true;
-  w.gscr = gscr + (size_t)(w.live ? w.env : 0) * (size_t)(C::CONW * (C::NS - C::NCS));
+  w.gscr = gscr + (size_t)(w.live ? w.env : 0) * (size_t)C::GSCRW;
   w.gbody = gbody ? gbody + (size_t)(w.live ? w.env : 0) * (size_t)(10 * C::NB) : nullptr;
   w.gpfl = gpfl ? gpfl + (size_t)(w.live ? w.env : 0) * (size_t)C::PFLW : nullptr;
   w.gsens = gsens ? gsens + (size_t)(w.live ? w.env : 0) * (size_t)(6 * C::NB) : nullptr;

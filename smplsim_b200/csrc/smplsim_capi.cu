@@ -19,13 +19,13 @@
 
 // model classes the kernels are instantiated for: <bodies, dofs, geoms, contact slots, in-mailboxes, out-mailboxes, contact
 // entries in shared memory, limit rows, geom-geom rows compiled in>
-#define L_SMPL(SC) LCfg<24, 75, 24, 64, 5, 2, 20, 16, SC>
+#define L_SMPL(SC) LCfg<24, 75, 24, 64, 5, 2, 15, 16, SC>
 #define L_SMPLX(SC) LCfg<52, 159, 52, 128, 13, 4, 14, 16, SC>
 
 struct SmplsimHandle {
   LaneImage img;
   float* dimg = nullptr;   // device copy of the table
-  float* gscr = nullptr;   // overflow contact entries
+  float* gscr = nullptr;   // per-env global scratch: lane records, qstar, overflow contact entries
   float* gsens = nullptr;  // body velocities of the last forward pass (obs v2 / aux)
   int* gpfl = nullptr;     // working set per contact slot, carried from call to call (solver warm start only)
   float* gbody = nullptr;  // body pose / velocity of the current forward pass (self-collision narrow phase)
@@ -188,7 +188,7 @@ static int create_impl(const SmplsimModelDesc* s, int nmodels, const int32_t* en
   L_DISPATCH(h, ok = pick_wpb<C_>(h));
   if (ok <= 0) { delete h; return fail(SMPLSIM_EUNSUPPORTED, "per-env rows exceed shared memory"); }
   size_t gs = 0;
-  L_DISPATCH(h, gs = (size_t)C_::CONW * (C_::NS - C_::NCS));
+  L_DISPATCH(h, gs = (size_t)C_::GSCRW);
   e = cudaMalloc(&h->dimg, (size_t)H.bytes * nmodels);
   if (e == cudaSuccess) e = cudaMemcpy(h->dimg, h->img.bytes.data(), H.bytes, cudaMemcpyHostToDevice);
   for (int k = 1; k < nmodels && e == cudaSuccess; k++) e = cudaMemcpy((char*)h->dimg + (size_t)H.bytes * k, more[k - 1].bytes.data(), H.bytes, cudaMemcpyHostToDevice);
