@@ -136,6 +136,13 @@ typedef struct SmplsimState {
   float* pid_integral;      /* [N,nu] SimplePID._integral   (control_mode simple_pid only, else may be NULL); like the reference's
                              *        controller object it is NOT cleared by reset */
   float* pid_last_error;    /* [N,nu] SimplePID._last_error ; NaN = None (first call: d_error = 0) */
+  const float* xfrc_applied; /* [N,nbody,6] or NULL: mj_data.xfrc_applied of the robot bodies (row 0 = root), read only.  Per body a
+                              * world-frame force (fx fy fz) acting at the body's centre of mass and a world-frame torque (tx ty tz),
+                              * as mj_xfrcAccumulate: qfrc_applied = Jp(xipos)^T f + Jr^T t.  It enters qfrc_smooth (hence qacc_smooth,
+                              * the constraint solve and qacc), NOT qfrc_bias: the stable-PD controller never sees it directly.
+                              * smplsim_step / smplsim_mj_step hold it constant over every substep of the call; smplsim_reset ignores
+                              * it.  An env that auto-resets (mj_checkPos/Vel/Acc -> mj_resetData, which zeroes xfrc_applied) runs the
+                              * rest of the call without it; the caller's array is never written. */
 } SmplsimState;
 
 /* Side outputs of the last forward pass / kinematics (any pointer may be NULL). */
@@ -159,7 +166,7 @@ typedef struct SmplsimAux {
 typedef struct SmplsimHandle SmplsimHandle;
 
 const char* smplsim_last_error(void);
-int smplsim_version(void);   /* 110 = this header (100: before pid_* state and aux.status) */
+int smplsim_version(void);   /* 210 = this header (200: before SmplsimState.xfrc_applied; 100: before pid_* state and aux.status) */
 
 /* MjModel.from_xml_string + MjData + setup_humanoid_properties/setup_controller
  * (base_env.py:139-142, humanoid_env.py:262-323). */

@@ -30,7 +30,7 @@ class SmplsimStateC(C.Structure):
         ("qpos", C.c_void_p), ("qvel", C.c_void_p), ("qpos_fwd", C.c_void_p), ("qvel_fwd", C.c_void_p),
         ("qacc_warm", C.c_void_p), ("task_target", C.c_void_p), ("task_change_step", C.c_void_p),
         ("progress", C.c_void_p), ("recovery", C.c_void_p), ("rng_counter", C.c_void_p),
-        ("pid_integral", C.c_void_p), ("pid_last_error", C.c_void_p),
+        ("pid_integral", C.c_void_p), ("pid_last_error", C.c_void_p), ("xfrc_applied", C.c_void_p),
     ]
 
 

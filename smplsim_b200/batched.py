@@ -105,6 +105,7 @@ class HumanoidBatchB200:
                                                          self.contact_mask, self.qacc, self.ctrl, self.solver_iter, self.status)])
         if not with_aux:        # throughput runs: skip the side outputs (NULL pointers), keep the 1-byte status
             self._aux = SmplsimAuxC(status=self.status.data_ptr())
+        self._xfrc = None           # mj_data.xfrc_applied (None: no external wrench; see xfrc_applied)
         self.gpu_launches = 0
 
     def __del__(self):
@@ -166,6 +167,7 @@ class HumanoidBatchB200:
             a = torch.clamp(a, -1.0, 1.0)      # action_space Box(-1,1) (humanoid_env.py:180-184; agent.py:153-161)
         a = a.contiguous()
         assert a.shape == (self.num_envs, self.num_actions)
+        self._set_xfrc()
         self._check(self._L().smplsim_step(self._h, C.byref(self._state), _ptr(a), _ptr(self.obs_buf), _ptr(self.rew_buf),
                                            _ptr(self.terminate_buf), _ptr(self.truncate_buf), C.byref(self._aux), self._stream()))
         self.gpu_launches += 1
@@ -173,10 +175,45 @@ class HumanoidBatchB200:
         self._keep_a = a
         return self.obs_buf, self.rew_buf, self.terminate_buf, self.truncate_buf
 
+    # ------------------------------------------------------------------ external body wrenches (mj_data.xfrc_applied)
+    @property
+    def xfrc_applied(self) -> Optional[torch.Tensor]:
+        """External wrench per robot body and env: None (none, the default) or a caller-owned contiguous float32 tensor
+        ``[num_envs, nbody, 6]`` on this batch's device, indexed like ``xpos`` (row 0 = root / Pelvis).  Each row is a world-frame force
+        ``(fx, fy, fz)`` acting at the body's centre of mass and a world-frame torque ``(tx, ty, tz)``, as MuJoCo's
+        ``mj_data.xfrc_applied``.  ``step`` and ``mj_step`` read it on every call and hold it constant over all substeps of the call; it
+        enters the dynamics (qfrc_smooth) but not the bias forces the stable-PD controller reads.  ``reset`` ignores it.  An env that
+        auto-resets on a bad state inside a call runs the rest of that call without it (mj_resetData zeroes xfrc_applied); the tensor
+        itself is never written.  Assign None to clear it."""
+        return self._xfrc
+
+    @xfrc_applied.setter
+    def xfrc_applied(self, t: Optional[torch.Tensor]):
+        if t is not None:
+            shape = (self.num_envs, self.model.nbody, 6)
+            if not isinstance(t, torch.Tensor):
+                raise ValueError(f"xfrc_applied must be a torch.Tensor of shape {shape} or None, got {type(t).__name__}")
+            if tuple(t.shape) != shape:
+                raise ValueError(f"xfrc_applied must have shape {shape} (envs, robot bodies, force + torque), got {tuple(t.shape)}")
+            if t.dtype != torch.float32:
+                raise ValueError(f"xfrc_applied must be float32, got {t.dtype}")
+            dv = self.device
+            if t.device.type != dv.type or (dv.index is not None and t.device.index != dv.index):
+                raise ValueError(f"xfrc_applied must live on {dv}, got {t.device}")
+            if not t.is_contiguous():
+                raise ValueError("xfrc_applied must be contiguous")
+        self._xfrc = t
+
+    def _set_xfrc(self):
+        """The wrench pointer of this call (NULL: none); the tensor is kept referenced until the next call."""
+        self._state.xfrc_applied = None if self._xfrc is None else self._xfrc.data_ptr()
+        self._keep_xfrc = self._xfrc
+
     # ------------------------------------------------------------------ raw physics / kinematics (parity + tools)
     def mj_step(self, ctrl: torch.Tensor, nsub: int = 1):
         """data.ctrl[:] = ctrl; mujoco.mj_step x nsub."""
         c = ctrl.to(self.device, torch.float32).contiguous()
+        self._set_xfrc()
         self._check(self._L().smplsim_mj_step(self._h, C.byref(self._state), _ptr(c), int(nsub), C.byref(self._aux), self._stream()))
         self.gpu_launches += 1
         self._keep_a = c

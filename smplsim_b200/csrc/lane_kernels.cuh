@@ -41,10 +41,12 @@
 #define L_ST_SELF_CONTACT 32 // SMPLSIM_STATUS_SELF_CONTACT: a geom pair MuJoCo would collide touches (not simulated)
 
 // ------------------------------------------------------------------ compile-time sizes / per-env shared-memory layout (words)
-template <int NB_, int NV_, int NG_, int NS_, int NMBI_, int NMBO_, int NCS_, int NLS_, int SELFCOL_ = 0>
+template <int NB_, int NV_, int NG_, int NS_, int NMBI_, int NMBO_, int NCS_, int NLS_, int SELFCOL_ = 0, int XFRC_ = 0>
 struct LCfg {
   static constexpr int NB = NB_, NV = NV_, NQ = NV_ + 1, NU = NV_ - 6, NG = NG_, NS = NS_, NMBI = NMBI_, NMBO = NMBO_, NCS = NCS_, NLS = NLS_;
   static constexpr int SELFCOL = SELFCOL_, LPE = LM_LPE, EPW = 32 / LM_LPE;   // SELFCOL: geom-geom (two-body) rows compiled in
+  static constexpr int XFRC = XFRC_;   // external body wrenches (SmplsimState.xfrc_applied) compiled in; same layout as without
+  typedef LCfg<NB_, NV_, NG_, NS_, NMBI_, NMBO_, NCS_, NLS_, SELFCOL_, 1> WithXfrc;
   static constexpr int BODYW = 24, MBIW = 28, MBOW = 32, CONW = 24, LIMW = 8, RECW = 28, ROOTW = 44;
   static constexpr int r4(int n) { return (n + 3) & ~3; }
   static constexpr int qpos = 0, qvel = qpos + r4(NQ), qacc = qvel + r4(NV), act = qacc + r4(NV), tau = act + r4(NU),
@@ -68,6 +70,7 @@ struct LCfg {
 #define LMI_DISP 2   // root displacement x, y accumulated over the substeps of this call (words 2, 3)
 #define LMI_NSELF 4  // geom-geom contacts of this substep (two list entries each, starting at LMI_SELF0)
 #define LMI_SELF0 5
+#define LMI_XFRC 6    // (XFRC instances) words 6, 7: this env's xfrc_applied rows for the rest of the call (8-byte pointer; NULL: none / cleared)
 #define L_MAXSELF 4   // simultaneous geom-geom contacts simulated per env (16 two-body rows, two per lane); more are dropped with L_ST_ROWS_DROPPED
 #define L_SELFQ (L_MAXSELF / 2)   // two-body rows per lane: lane li owns rows li, li + 8, ...
 #define LCE_SELF 64   // info bit: entry A of a geom-geom contact (entry B follows: [0 | n 3 | b1 | b2 | - - | lam 4 | part1 4 | part2 4 | r0 4])
@@ -812,6 +815,20 @@ __device__ __forceinline__ void l_self_wrench(const LHdr& H, float* sm, const LL
     p.l = p.l - f; p.a = p.a - cross(cp, f);
   }
 }
+// (XFRC) bias force of body b -= its external wrench (SmplsimState.xfrc_applied row b: force f at the centre of mass, torque t, world
+// axes), about the root origin [t + r x f ; f] with r = (m r) / m from the body's rigid-inertia row (massless body: r = 0).  Called by
+// the constraint-side inward sweeps only (first sweep, re-sweeps, Woodbury probes): the bias forces S1 stores in the records and the
+// stable-PD system (the SPD instances, S4) stay without it, as qfrc_bias does in MuJoCo (quirk Q1 reads qfrc_bias).
+template <class C>
+__device__ __forceinline__ void l_xfrc_wrench(const float* sm, int b, const float* r10, S6& p) {
+  const float* xf = *(const float* const*)(sm + C::misc + LMI_XFRC);
+  if (!xf) return;
+  const float* x = xf + 6 * b;
+  const V3 f = v3(__ldg(x), __ldg(x + 1), __ldg(x + 2)), t = v3(__ldg(x + 3), __ldg(x + 4), __ldg(x + 5));
+  const float im = r10[0] > 0.f ? 1.0f / r10[0] : 0.f;
+  const V3 r = im * v3(r10[1], r10[2], r10[3]);
+  p.l = p.l - f; p.a = p.a - (t + cross(r, f));
+}
 // partial row values x_k . a_b of the geom-geom rows that touch body b (part1 for b1, part2 for b2)
 template <class C>
 __device__ __forceinline__ void l_self_part(const LHdr& H, float* sm, const LLane& w, int b, S6 a) {
@@ -956,6 +973,7 @@ __device__ __noinline__ bool l_root_in(const float* ms, float* sm, const LLane& 
       dirty = dirty || cn > 0;
       l_fold_contacts<C>(H, sm, w, ci & 255, cn, A, p);
       if (C::SELFCOL && ((const int*)sm)[C::misc + LMI_NSELF]) { l_self_wrench<C>(H, sm, w, 0, p); dirty = dirty || l_self_touches<C>(sm, w, 0); }
+      if (C::XFRC) l_xfrc_wrench<C>(sm, 0, r10, p);
     }
     if (SPD && (flags & LI_INTEGRATE)) {
       float* qpos = sm + C::qpos; float* qvel = sm + C::qvel; const float* qacc = sm + C::qacc;
@@ -1075,6 +1093,7 @@ __device__ __noinline__ void l_sweep_in(const float* ms, float* sm, const LLane&
         dirty = dirty || cn > 0 || ln > 0;
         l_fold_contacts<C>(H, sm, w, cb, cn, A, p);
         if (C::SELFCOL && ((const int*)sm)[C::misc + LMI_NSELF]) { l_self_wrench<C>(H, sm, w, b, p); dirty = dirty || l_self_touches<C>(sm, w, b); }
+        if (C::XFRC) l_xfrc_wrench<C>(sm, b, r10, p);
         for (int e = lbs; e < lbs + ln; e++) {   // joint-limit rows of this body that sit in the working set
           const float4* l4 = (const float4*)(sm + C::lim + C::LIMW * e);
           float4 u = l4[0], v = l4[1];
@@ -1548,9 +1567,19 @@ __device__ __noinline__ int l_solve(const float* ms, float* sm, const LLane& w, 
   return iters;
 }
 
+// the state rows the kernels read and write: SmplsimState without its trailing xfrc_applied, which k_step5 takes as a parameter of its
+// own.  The kernels keep a copy of their argument struct on the stack (parts of it are passed by reference), so it keeps the size it had
+// before the wrench existed.
+struct LState {
+  float *qpos, *qvel, *qpos_fwd, *qvel_fwd, *qacc_warm, *task_target;
+  int32_t *task_change_step, *progress, *recovery;
+  uint32_t* rng_counter;
+  float *pid_integral, *pid_last_error;
+};
+
 // ------------------------------------------------------------------ elementwise controllers (pd / torque / simple_pid), controllers.py:6-47,186-349
 template <class C>
-__device__ __noinline__ void l_torque_elem(const float* ms, float* sm, const LLane& w, const SmplsimState& sta) {
+__device__ __noinline__ void l_torque_elem(const float* ms, float* sm, const LLane& w, const LState& sta) {
   const LHdr& H = l_hdr<C>(ms);
   const LBody* MB = l_bodies(ms);
   const int mode = H.cfg.control_mode;
@@ -1645,6 +1674,7 @@ __device__ __noinline__ int l_check(const float* ms, float* sm, const LLane& w, 
     for (int i = w.li; i < H.nv; i += LM_LPE) { sm[C::qvel + i] = 0.f; sm[C::qacc + i] = 0.f; }
 #pragma unroll 1
     for (int i = w.li; i < H.nu; i += LM_LPE) sm[C::tau + i] = 0.f;
+    if (C::XFRC && w.li == 0) *(const float**)(sm + C::misc + LMI_XFRC) = nullptr;   // mj_resetData zeroes xfrc_applied: gone for the rest of the call
   }
   __syncwarp();
   return bits;
@@ -1675,7 +1705,7 @@ struct LFwd { unsigned long long mask; int iters; int status; };
 // Entry condition in stable-PD (stale) mode: records hold the (M + h Kd) factors of the last forward pass for the state in
 // qpos / qvel and the action in act (prologue of the kernels: l_spd_prologue).
 template <class C>
-__device__ __noinline__ void l_substeps(const float* ms, float* sm, const LLane& w, int nsub, int raw, LFwd* fo, const SmplsimState& sta,
+__device__ __noinline__ void l_substeps(const float* ms, float* sm, const LLane& w, int nsub, int raw, LFwd* fo, const LState& sta,
                                         bool write_fwd, bool prep_last, LSolveLane& st) {
   const LHdr& H = l_hdr<C>(ms);
   const bool spd = (H.cfg.control_mode == SMPLSIM_CTRL_UHC_PD) && !raw, stale = H.cfg.spd_stale != 0;
@@ -1742,7 +1772,7 @@ __device__ __noinline__ void l_substeps(const float* ms, float* sm, const LLane&
 // Both NULL: one table, slot == env.
 struct LMap { const int* slot_env; const int* blk_img; };
 struct LStepArgs {
-  SmplsimState st;
+  LState st;
   SmplsimAux aux;
   const float* action;
   float* obs;
@@ -1757,7 +1787,7 @@ struct LStepArgs {
   int n, nsub, mode;
 };
 struct LResetArgs {
-  SmplsimState st;
+  LState st;
   SmplsimAux aux;
   const uint8_t* mask;
   const float* qpos0;
@@ -1798,7 +1828,7 @@ __device__ __forceinline__ void l_copy_out(float* __restrict__ dst, const float*
 }
 
 template <class C>
-__device__ __noinline__ void l_task_io(float* sm, const LLane& w, const SmplsimState& st, bool store) {
+__device__ __noinline__ void l_task_io(float* sm, const LLane& w, const LState& st, bool store) {
   if (store) __syncwarp();
   if (w.live && w.li == 0) {
     float* t = sm + C::tsk;
@@ -2009,7 +2039,7 @@ __device__ __forceinline__ float* l_setup(const float* __restrict__ gimg, int im
 // stable PD, stale inertia (quirk Q1): rebuild the (M + h Kd) factors of the state of the last forward pass for the current
 // state / action.  On entry qpos / qvel / act hold the current state; qpos_fwd / qvel_fwd come from HBM.
 template <class C>
-__device__ __noinline__ void l_spd_prologue(const float* ms, float* sm, const LLane& w, const SmplsimState& sta, LSolveLane& st) {
+__device__ __noinline__ void l_spd_prologue(const float* ms, float* sm, const LLane& w, const LState& sta, LSolveLane& st) {
   const LHdr& H = l_hdr<C>(ms);
   size_t eo = w.live ? (size_t)w.env : 0;
   l_copy_in<C>(sm + C::qpos, sta.qpos_fwd + eo * (H.nv + 1), H.nv + 1, w);
@@ -2023,7 +2053,7 @@ __device__ __noinline__ void l_spd_prologue(const float* ms, float* sm, const LL
 }
 
 template <class C>
-__global__ void __launch_bounds__(256, 1) k_step5(const float* __restrict__ gimg, int img_bytes, LStepArgs a) {
+__global__ void __launch_bounds__(256, 1) k_step5(const float* __restrict__ gimg, int img_bytes, LStepArgs a, const float* __restrict__ xfrc) {
   const float* ms; LLane w;
   float* sm = l_setup<C>(gimg, img_bytes, w, ms, a.n, a.map, a.gscr, a.gsens, a.gpfl, a.gbody);
   const LHdr& H = l_hdr<C>(ms);
@@ -2045,6 +2075,7 @@ __global__ void __launch_bounds__(256, 1) k_step5(const float* __restrict__ gimg
     int* ti = (int*)(sm + C::tsk);
     if (H.cfg.task != SMPLSIM_TASK_NONE && ti[L_TSK_CURT] >= ti[L_TSK_CHANGE]) l_reset_task<C>(H, sm, w.env);
   }
+  if (C::XFRC && w.live && w.li == 0) *(const float**)(sm + C::misc + LMI_XFRC) = xfrc ? xfrc + eo * 6 * H.nb : nullptr;   // read after the sweeps' __syncwarp
   __syncwarp();
   LFwd fo; fo.mask = 0ull; fo.iters = 0; fo.status = 0;
   l_substeps<C>(ms, sm, w, a.nsub, a.mode, &fo, a.st, true, false, st);

@@ -74,6 +74,10 @@ class HumanoidEnvB200(_EnvBase):
         self.dtype = np.float32
         self._b = self._make_batch(cfg, device)
         m = self._b.model
+        # mj_data.xfrc_applied: one persistent array in MuJoCo indexing (row 0 = world, no effect), so that
+        # env.mj_data.xfrc_applied[body_id] = (fx, fy, fz, tx, ty, tz) works as it does on an MjData
+        self._xfrc_applied = np.zeros((m.nbody + 1, 6))
+        self._xfrc_dev = None
         self.control_mode = e.control_mode
         self.max_episode_length = e.episode_length
         self.self_obs_v = e.self_obs_v
@@ -123,8 +127,20 @@ class HumanoidEnvB200(_EnvBase):
         self.cur_t = 0
         return obs, {"critic_state": obs}
 
+    def _upload_xfrc(self):
+        """mj_data.xfrc_applied -> the batch's wrench tensor before a step: an all-zero array is no wrench (None)."""
+        x = self._xfrc_applied[1:]
+        if not np.any(x):
+            self._b.xfrc_applied = None
+            return
+        if self._xfrc_dev is None:
+            self._xfrc_dev = torch.zeros(1, self._b.model.nbody, 6, dtype=torch.float32, device=self._b.device)
+        self._xfrc_dev.copy_(torch.as_tensor(x, dtype=torch.float32)[None])
+        self._b.xfrc_applied = self._xfrc_dev
+
     def step(self, action):
         a = torch.as_tensor(np.asarray(action, dtype=np.float32)[None, : self.dof_size])
+        self._upload_xfrc()
         obs, rew, term, trunc = self._b.step(a)
         obs = obs.cpu().numpy()[0].astype(self.dtype)
         self.cur_t = int(self._b.progress_buf[0].item())
@@ -150,7 +166,8 @@ class HumanoidEnvB200(_EnvBase):
         return SimpleNamespace(qpos=b.qpos[0].cpu().numpy().astype(np.float64), qvel=b.qvel[0].cpu().numpy().astype(np.float64),
                                ctrl=b.ctrl[0].cpu().numpy().astype(np.float64), qacc=b.qacc[0].cpu().numpy().astype(np.float64),
                                xpos=np.concatenate([z3, b.xpos[0].cpu().numpy()]), xquat=np.concatenate([z4, b.xquat[0].cpu().numpy()]),
-                               sensordata=sens, contact=_Contacts(int(b.contact_mask[0].item())))
+                               sensordata=sens, contact=_Contacts(int(b.contact_mask[0].item())),
+                               xfrc_applied=self._xfrc_applied)
 
     @property
     def mj_model(self):
