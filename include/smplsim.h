@@ -161,12 +161,23 @@ typedef struct SmplsimAux {
                          *       (the contact is not simulated, the state differs from the reference from here on).
                          *       As in mj_step (mj_checkPos/Vel/Acc + mj_resetData) a NaN or |x| > 1e10 auto-resets that env's
                          *       data to qpos0 / zero velocity and the call carries on -- a device fault never traps. */
+  float* contact_wrench; /* [N,nbody,6] or NULL: per robot body (rows as xpos / xfrc_applied, row 0 = root) the wrench the contacts of
+                          * the last forward pass (the pass contact_mask, qacc and solver_iter describe: last substep, before integration)
+                          * apply to it: [0:3] world-frame force, [3:6] world-frame torque of those forces about the body's centre of mass
+                          * (xipos) -- the convention of xfrc_applied.  So sum_b Jp_b(xipos_b)^T F_b + Jr_b^T t_b is the contact part of
+                          * qfrc_constraint (all of it but the joint-limit rows).  A floor contact on a geom of body b adds
+                          * F = sum_k f_k (n +- mu t_k) of its four pyramid rows at the contact point; a geom-geom contact adds +F to the
+                          * body of geom2 and -F to the body of geom1.  A body without contact force reads exact zeros.  smplsim_reset
+                          * zeroes the rows of the envs it resets (its mj_forward runs no constraint solve) and leaves the others.
+                          * [MJ-upstream] mj_contactForce summed per body; MuJoCo's cfrc_ext holds the same wrench (without
+                          * xfrc_applied) in com-based form about the root subtree COM, rotation first -- not checked against a wheel. */
 } SmplsimAux;
 
 typedef struct SmplsimHandle SmplsimHandle;
 
 const char* smplsim_last_error(void);
-int smplsim_version(void);   /* 210 = this header (200: before SmplsimState.xfrc_applied; 100: before pid_* state and aux.status) */
+int smplsim_version(void);   /* 220 = this header (210: before SmplsimAux.contact_wrench; 200: before SmplsimState.xfrc_applied;
+                              * 100: before pid_* state and aux.status) */
 
 /* MjModel.from_xml_string + MjData + setup_humanoid_properties/setup_controller
  * (base_env.py:139-142, humanoid_env.py:262-323). */

@@ -38,6 +38,7 @@ class SmplsimAuxC(C.Structure):
     _fields_ = [
         ("xpos", C.c_void_p), ("xquat", C.c_void_p), ("body_linvel", C.c_void_p), ("body_angvel", C.c_void_p),
         ("contact_mask", C.c_void_p), ("qacc", C.c_void_p), ("ctrl", C.c_void_p), ("solver_iter", C.c_void_p), ("status", C.c_void_p),
+        ("contact_wrench", C.c_void_p),
     ]
 
 

@@ -31,9 +31,18 @@ class HumanoidBatchB200:
 
     def __init__(self, cfg: Any, num_envs: Optional[int] = None, device: str = "cuda:0", seed: Optional[int] = None,
                  model: Optional[ModelDesc] = None, rank: int = 0, with_aux: bool = True,
-                 models: Optional[Sequence[ModelDesc]] = None, env_model: Optional[Sequence[int]] = None):
+                 models: Optional[Sequence[ModelDesc]] = None, env_model: Optional[Sequence[int]] = None,
+                 contact_wrench: bool = False):
         """``models`` + ``env_model`` ([num_envs] indices into models): per-env body shapes in one batch -- what one SMPL_Robot per
-        env process gives the reference (humanoid_env.py:219-250).  Same tree / joints / geom layout in every model."""
+        env process gives the reference (humanoid_env.py:219-250).  Same tree / joints / geom layout in every model.
+
+        ``contact_wrench=True`` allocates ``self.contact_wrench`` ``[num_envs, nbody, 6]`` float32 on the device (also with
+        ``with_aux=False``), which ``step`` / ``mj_step`` fill with the per-body contact wrench of the last forward pass (last substep,
+        before integration; the pass ``contact_mask`` and ``qacc`` describe): rows indexed like ``xpos`` (row 0 = root / Pelvis),
+        ``[..., 0:3]`` the world-frame force the floor and geom-geom contacts apply to the body, ``[..., 3:6]`` the torque of those forces
+        about the body's centre of mass -- the convention of ``xfrc_applied``.  ``contact_wrench[..., :3]`` is the layout of Isaac's
+        ``net_contact_force`` ([N, nbody, 3]).  Bodies without contact force read exact zeros; ``reset`` zeroes the rows of the envs it
+        resets.  False (the default): ``self.contact_wrench`` is None and the kernels skip it."""
         self._require_device(device)
         self.cfg = cfg
         e = cfg.env
@@ -105,6 +114,9 @@ class HumanoidBatchB200:
                                                          self.contact_mask, self.qacc, self.ctrl, self.solver_iter, self.status)])
         if not with_aux:        # throughput runs: skip the side outputs (NULL pointers), keep the 1-byte status
             self._aux = SmplsimAuxC(status=self.status.data_ptr())
+        self.contact_wrench = torch.zeros(N, m.nbody, 6, **f32) if contact_wrench else None   # per-body contact wrench (see above)
+        if self.contact_wrench is not None:
+            self._aux.contact_wrench = self.contact_wrench.data_ptr()
         self._xfrc = None           # mj_data.xfrc_applied (None: no external wrench; see xfrc_applied)
         self.gpu_launches = 0
 

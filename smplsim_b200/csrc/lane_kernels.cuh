@@ -1576,6 +1576,14 @@ struct LState {
   uint32_t* rng_counter;
   float *pid_integral, *pid_last_error;
 };
+// the side outputs likewise: SmplsimAux without its trailing contact_wrench, which k_step5 and k_reset5 take as a parameter of their own
+struct LAux {
+  float *xpos, *xquat, *body_linvel, *body_angvel;
+  uint64_t* contact_mask;
+  float *qacc, *ctrl;
+  int32_t* solver_iter;
+  uint8_t* status;
+};
 
 // ------------------------------------------------------------------ elementwise controllers (pd / torque / simple_pid), controllers.py:6-47,186-349
 template <class C>
@@ -1773,7 +1781,7 @@ __device__ __noinline__ void l_substeps(const float* ms, float* sm, const LLane&
 struct LMap { const int* slot_env; const int* blk_img; };
 struct LStepArgs {
   LState st;
-  SmplsimAux aux;
+  LAux aux;
   const float* action;
   float* obs;
   float* reward;
@@ -1788,7 +1796,7 @@ struct LStepArgs {
 };
 struct LResetArgs {
   LState st;
-  SmplsimAux aux;
+  LAux aux;
   const uint8_t* mask;
   const float* qpos0;
   const float* qvel0;
@@ -1919,8 +1927,75 @@ __device__ __noinline__ void l_write_obs(const float* ms, float* sm, const LLane
   __syncwarp();
 }
 
+// Per-body contact wrench of the last forward pass (SmplsimAux.contact_wrench): row b = [F ; t], the world-frame force the floor and
+// geom-geom contacts apply to body b and its torque about the body's centre of mass (xipos), the convention of xfrc_applied.  Read from
+// the contact list the last solve left, before the final kinematics sweep aliases it as staging.  The contact points and the body's
+// (m r) row are both relative to the root origin of that forward pass, so the lever arm is cp - (m r) / m.  Lane li owns bodies
+// li, li + 8, ...: each sums its own contacts (body row cinfo) and then the geom-geom entries in list order -- no atomics, bit-reproducible.
+// Row forces f with M qacc - qfrc_smooth = J^T f at the qacc the solve returned:
+//   * exits at a point whose row signs equal the working set (first pass, or a trial point taken as it is): -D rs on the set for the
+//     floor rows, the Woodbury multipliers (LSB_LAM) for the geom-geom rows;
+//   * exits after line-search steps (stopped at al = 0, or at the iteration cap): phi, which the row passes keep at the iterate.
 template <class C>
-__device__ __noinline__ void l_write_aux(const float* ms, float* sm, const LLane& w, const SmplsimAux& aux, const LFwd& fo) {
+__device__ __noinline__ void l_contact_wrench(const float* ms, float* sm, const LLane& w, int iters, float* out) {
+  const LHdr& H = l_hdr<C>(ms);
+  const int ncon = ((const int*)sm)[C::misc + LMI_NCON], nlim = ((const int*)sm)[C::misc + LMI_NLIM];
+  bool same = true;
+  if (w.live) {
+    for (int c = w.li; c < ncon; c += LM_LPE) {
+      const float* ce = l_centry<C>(sm, w, c);
+      const int info = ((const int*)ce)[LCE_INFO];
+      if (!(info & 1)) continue;
+      int nf = 0;
+#pragma unroll
+      for (int k = 0; k < 4; k++) if (ce[LCE_RS + k] < 0.f) nf |= 2 << k;
+      same = same && nf == (info & 30);
+    }
+    for (int e = w.li; e < nlim; e += LM_LPE) {
+      const float* le = sm + C::lim + C::LIMW * e;
+      same = same && (le[LLE_RS] < 0.f ? 1 : 0) == (((const int*)le)[LLE_FLAG] & 1);
+    }
+  }
+  const bool take = l_gall(same, w) && iters < L_SOLVER_MAXITER;
+  if (!w.live) return;
+  const V3 n0 = ld3(H.plane_n), z = v3(0.f, 0.f, 0.f);
+  const int nself = C::SELFCOL ? ((const int*)sm)[C::misc + LMI_NSELF] : 0, s0 = ((const int*)sm)[C::misc + LMI_SELF0];
+  for (int b = w.li; b < H.nb; b += LM_LPE) {
+    float r10[10];
+    const int ci = l_ld_r10(sm + C::body + C::BODYW * b, r10), cb = ci & 255, cn = (ci >> 8) & 255;
+    const V3 rc = (r10[0] > 0.f ? 1.0f / r10[0] : 0.f) * v3(r10[1], r10[2], r10[3]);
+    V3 f = z, t = z;
+    for (int c = cb; c < cb + cn; c++) {   // floor contacts of body b
+      const float* ce = l_centry<C>(sm, w, c);
+      const int info = ((const int*)ce)[LCE_INFO];
+      if (!(info & 1)) continue;
+      const V3 t1 = ld3(ce + LCE_T1), t2 = cross(n0, t1);
+      V3 fc = z;
+#pragma unroll
+      for (int k = 0; k < 4; k++) {
+        const float fk = take ? ((info & (2 << k)) ? -ce[LCE_D] * ce[LCE_RS + k] : 0.f) : ce[LCE_PHI + k];
+        fc = fc + fk * l_pyr_dir(H, n0, t1, t2, k);
+      }
+      f = f + fc; t = t + cross(ld3(ce + LCE_CP) - rc, fc);
+    }
+    for (int s = 0; s < nself; s++) {      // geom-geom contacts: + on the body of geom2, - on the body of geom1
+      const float* ea = l_centry<C>(sm, w, s0 + 2 * s); const float* eb = l_centry<C>(sm, w, s0 + 2 * s + 1);
+      const int b1 = ((const int*)eb)[LSB_B1], b2 = ((const int*)eb)[LSB_B2];
+      if (b != b1 && b != b2) continue;
+      const V3 n = ld3(eb + LSB_N), t1 = ld3(ea + LCE_T1), t2 = cross(n, t1);
+      V3 fc = z;
+#pragma unroll
+      for (int k = 0; k < 4; k++) fc = fc + (take ? eb[LSB_LAM + k] : ea[LCE_PHI + k]) * l_pyr_dir(H, n, t1, t2, k);
+      if (b == b1) fc = -1.0f * fc;
+      f = f + fc; t = t + cross(ld3(ea + LCE_CP) - rc, fc);
+    }
+    float* o = out + ((size_t)w.env * H.nb + b) * 6;
+    st3(o, f); st3(o + 3, t);
+  }
+}
+
+template <class C>
+__device__ __noinline__ void l_write_aux(const float* ms, float* sm, const LLane& w, const LAux& aux, const LFwd& fo) {
   const LHdr& H = l_hdr<C>(ms);
   if (!w.live) return;
   V3 root = ld3(sm + C::qpos);
@@ -2053,7 +2128,8 @@ __device__ __noinline__ void l_spd_prologue(const float* ms, float* sm, const LL
 }
 
 template <class C>
-__global__ void __launch_bounds__(256, 1) k_step5(const float* __restrict__ gimg, int img_bytes, LStepArgs a, const float* __restrict__ xfrc) {
+__global__ void __launch_bounds__(256, 1) k_step5(const float* __restrict__ gimg, int img_bytes, LStepArgs a, const float* __restrict__ xfrc,
+                                                         float* __restrict__ cwrench) {
   const float* ms; LLane w;
   float* sm = l_setup<C>(gimg, img_bytes, w, ms, a.n, a.map, a.gscr, a.gsens, a.gpfl, a.gbody);
   const LHdr& H = l_hdr<C>(ms);
@@ -2079,6 +2155,7 @@ __global__ void __launch_bounds__(256, 1) k_step5(const float* __restrict__ gimg
   __syncwarp();
   LFwd fo; fo.mask = 0ull; fo.iters = 0; fo.status = 0;
   l_substeps<C>(ms, sm, w, a.nsub, a.mode, &fo, a.st, true, false, st);
+  if (cwrench) l_contact_wrench<C>(ms, sm, w, fo.iters, cwrench);   // before the sweep below reuses the contact list
   l_sweep_out<C>(ms, sm, w, LF_FK | LF_XQUAT, false);
   if (H.npair > 0 && !H.cfg.self_collision && a.aux.status && l_self_contact<C>(ms, sm, w)) fo.status |= L_ST_SELF_CONTACT;   // detected, not simulated
   if (a.mode == 0) {
@@ -2188,6 +2265,13 @@ __global__ void __launch_bounds__(256, 1) k_reset5(const float* __restrict__ gim
   l_copy_out<C>(a.st.qacc_warm + eo * H.nv, sm + C::qacc, H.nv, w);
   if (w.live && w.gpfl) for (int i = w.li; i < (H.nslot + 3) / 4; i += LM_LPE) w.gpfl[i] = ((const int*)sm)[C::pfl + i];
   l_task_io<C>(sm, w, a.st, true);
+}
+
+// aux.contact_wrench of the envs smplsim_reset resets (mask NULL: all): zeros, since the reset's mj_forward runs no constraint solve.
+// A launch of its own after k_reset5, only when the caller passes the output, so that k_reset5 compiles as it does without it.
+__global__ void k_zero_wrench(float* __restrict__ cw, const uint8_t* __restrict__ mask, int n, int row) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < (long)n * row && (!mask || mask[i / row])) cw[i] = 0.f;
 }
 
 // mujoco.mj_kinematics (humanoid_env.py:389) / poselib global_transformation on caller-supplied qpos rows

@@ -58,7 +58,7 @@ struct DeviceGuard {   // every entry point runs on the handle's device and rest
 };
 
 extern "C" const char* smplsim_last_error(void) { return g_err.c_str(); }
-extern "C" int smplsim_version(void) { return 210; }   // 210: SmplsimState.xfrc_applied; 200: lane-chain kernels (ABI structs of 110)
+extern "C" int smplsim_version(void) { return 220; }   // 220: SmplsimAux.contact_wrench; 210: SmplsimState.xfrc_applied; 200: lane-chain kernels (ABI structs of 110)
 
 template <class C>
 static size_t cta_smem(const SmplsimHandle* h, int wpb) { return (size_t)h->img.hdr()->bytes + 16 + (size_t)wpb * C::EPW * C::total * 4; }
@@ -98,17 +98,22 @@ static int pick_wpb(SmplsimHandle* h) {
 }
 
 // step and mj_step: the instance with the external-wrench code compiled in only when the caller passes xfrc_applied (same layout,
-// shared memory and CTA size; without a wrench the kernel is the one without that code)
+// shared memory and CTA size; without a wrench the kernel is the one without that code).  The contact wrench output is a run-time
+// argument of every instance (NULL: not written).
 template <class C>
-static void run_step(SmplsimHandle* h, const LStepArgs& a, const float* xfrc, cudaStream_t st) {
+static void run_step(SmplsimHandle* h, const LStepArgs& a, const float* xfrc, float* cwrench, cudaStream_t st) {
   int wpb = h->wpb, per = wpb * C::EPW, grid = h->nblocks ? h->nblocks : (a.n + per - 1) / per;
-  if (xfrc) L_LAUNCH(k_step5<typename C::WithXfrc>, grid, 32 * wpb, h->smem, st, h->dimg, h->img.hdr()->bytes, a, xfrc);
-  else L_LAUNCH(k_step5<C>, grid, 32 * wpb, h->smem, st, h->dimg, h->img.hdr()->bytes, a, nullptr);
+  if (xfrc) L_LAUNCH(k_step5<typename C::WithXfrc>, grid, 32 * wpb, h->smem, st, h->dimg, h->img.hdr()->bytes, a, xfrc, cwrench);
+  else L_LAUNCH(k_step5<C>, grid, 32 * wpb, h->smem, st, h->dimg, h->img.hdr()->bytes, a, nullptr, cwrench);
 }
 template <class C>
-static void run_reset(SmplsimHandle* h, const LResetArgs& a, cudaStream_t st) {
+static void run_reset(SmplsimHandle* h, const LResetArgs& a, float* cwrench, cudaStream_t st) {
   int wpb = h->wpb, per = wpb * C::EPW;
   L_LAUNCH(k_reset5<C>, h->nblocks ? h->nblocks : (a.n + per - 1) / per, 32 * wpb, h->smem, st, h->dimg, h->img.hdr()->bytes, a);
+  if (cwrench) {
+    const int row = 6 * h->img.hdr()->nb;
+    L_LAUNCH(k_zero_wrench, (int)(((long)a.n * row + 255) / 256), 256, 0, st, cwrench, a.mask, a.n, row);
+  }
 }
 template <class C>
 static void run_kin(SmplsimHandle* h, const LKinArgs& a, cudaStream_t st) {
@@ -261,6 +266,14 @@ static LState lane_state(const SmplsimState* st) {   // the rows before xfrc_app
   std::memcpy(&s, st, sizeof s);
   return s;
 }
+static LAux lane_aux(const SmplsimAux* aux) {   // the rows before contact_wrench, in the same order (all NULL without aux)
+  static_assert(sizeof(LAux) == offsetof(SmplsimAux, contact_wrench), "LAux must mirror SmplsimAux up to contact_wrench");
+  LAux x;
+  std::memset(&x, 0, sizeof x);
+  if (aux) std::memcpy(&x, aux, sizeof x);
+  return x;
+}
+static float* aux_wrench(const SmplsimAux* aux) { return aux ? aux->contact_wrench : nullptr; }
 static bool state_ok(const SmplsimState* st) {
   return st && st->qpos && st->qvel && st->qpos_fwd && st->qvel_fwd && st->qacc_warm && st->task_target && st->task_change_step &&
          st->progress && st->recovery && st->rng_counter;
@@ -276,11 +289,11 @@ extern "C" int smplsim_step(SmplsimHandle* h, const SmplsimState* st, const floa
     return fail(SMPLSIM_EINVAL, "smplsim_step: control_mode simple_pid needs state.pid_integral / pid_last_error");
   DeviceGuard guard(h->device);
   LStepArgs a; std::memset(&a, 0, sizeof a);
-  a.st = lane_state(st); if (aux) a.aux = *aux;
+  a.st = lane_state(st); a.aux = lane_aux(aux);
   a.action = action_dev; a.obs = obs_dev; a.reward = reward_dev; a.terminated = terminated_dev; a.truncated = truncated_dev;
   a.gscr = h->gscr; a.gpfl = h->gpfl; a.gbody = h->gbody; a.n = h->num_envs; a.nsub = h->img.hdr()->cfg.nsubsteps; a.mode = 0; a.map = h->map();
   a.gsens = want_sens(h, aux) ? h->gsens : nullptr;
-  L_DISPATCH(h, run_step<C_>(h, a, st->xfrc_applied, (cudaStream_t)stream));
+  L_DISPATCH(h, run_step<C_>(h, a, st->xfrc_applied, aux_wrench(aux), (cudaStream_t)stream));
   CUDA_TRY(cudaGetLastError());
   return SMPLSIM_OK;
 }
@@ -289,10 +302,10 @@ extern "C" int smplsim_mj_step(SmplsimHandle* h, const SmplsimState* st, const f
   if (!h || !state_ok(st) || !ctrl_dev || nsub < 1) return fail(SMPLSIM_EINVAL, "smplsim_mj_step: bad argument");
   DeviceGuard guard(h->device);
   LStepArgs a; std::memset(&a, 0, sizeof a);
-  a.st = lane_state(st); if (aux) a.aux = *aux;
+  a.st = lane_state(st); a.aux = lane_aux(aux);
   a.action = ctrl_dev; a.gscr = h->gscr; a.gpfl = h->gpfl; a.gbody = h->gbody; a.n = h->num_envs; a.nsub = nsub; a.mode = 1; a.map = h->map();
   a.gsens = want_sens(h, aux) ? h->gsens : nullptr;
-  L_DISPATCH(h, run_step<C_>(h, a, st->xfrc_applied, (cudaStream_t)stream));
+  L_DISPATCH(h, run_step<C_>(h, a, st->xfrc_applied, aux_wrench(aux), (cudaStream_t)stream));
   CUDA_TRY(cudaGetLastError());
   return SMPLSIM_OK;
 }
@@ -307,10 +320,10 @@ extern "C" int smplsim_reset(SmplsimHandle* h, const SmplsimState* st, const uin
   if (mode == SMPLSIM_INIT_MOCAP && (!qpos0_dev || !qvel0_dev)) return fail(SMPLSIM_EINVAL, "smplsim_reset: MoCap init needs qpos0/qvel0");
   DeviceGuard guard(h->device);
   LResetArgs a; std::memset(&a, 0, sizeof a);
-  a.st = lane_state(st); if (aux) a.aux = *aux;
+  a.st = lane_state(st); a.aux = lane_aux(aux);
   a.mask = mask_dev; a.qpos0 = qpos0_dev; a.qvel0 = qvel0_dev; a.obs = obs_dev; a.gscr = h->gscr; a.gpfl = h->gpfl; a.gbody = h->gbody; a.n = h->num_envs; a.init_mode = mode; a.map = h->map();
   a.gsens = want_sens(h, aux) ? h->gsens : nullptr;
-  L_DISPATCH(h, run_reset<C_>(h, a, (cudaStream_t)stream));
+  L_DISPATCH(h, run_reset<C_>(h, a, aux_wrench(aux), (cudaStream_t)stream));
   CUDA_TRY(cudaGetLastError());
   return SMPLSIM_OK;
 }
