@@ -176,7 +176,7 @@ typedef struct SmplsimAux {
 typedef struct SmplsimHandle SmplsimHandle;
 
 const char* smplsim_last_error(void);
-int smplsim_version(void);   /* 220 = this header (210: before SmplsimAux.contact_wrench; 200: before SmplsimState.xfrc_applied;
+int smplsim_version(void);   /* 230 = this header (220: before smplsim_inverse; 210: before SmplsimAux.contact_wrench; 200: before SmplsimState.xfrc_applied;
                               * 100: before pid_* state and aux.status) */
 
 /* MjModel.from_xml_string + MjData + setup_humanoid_properties/setup_controller
@@ -217,6 +217,20 @@ int smplsim_mj_step(SmplsimHandle* h, const SmplsimState* st, const float* ctrl_
  * (poselib/skeleton/skeleton3d.py:389-408): qpos[N,nq] -> xpos[N,nbody,3], xquat[N,nbody,4]. */
 int smplsim_kinematics(SmplsimHandle* h, const float* qpos_dev, float* xpos_dev, float* xquat_dev, int n,
                        void* cuda_stream);
+
+/* mujoco.mj_inverse on n caller rows: qpos[n,nq], qvel[n,nv], qacc[n,nv] -> qfrc_inverse[n,nv];
+ * contact_wrench[n,nbody,6] or NULL (same layout / convention as SmplsimAux.contact_wrench).
+ * qfrc_inverse = M(qpos) qacc + qfrc_bias(qpos, qvel) - J^T f, f_r = -D_r min(0, J_r qacc - aref_r) over the floor-contact pyramid rows
+ * and joint-limit rows that mj_forward at (qpos, qvel) builds; M includes the armature.  Conventions of qfrc_bias / qvel: root dofs
+ * [0:3] world-frame force, [3:6] torque about the root body's axes.  If qacc is what the forward pass produced from ctrl (and
+ * xfrc_applied), qfrc_inverse = [0_6 ; ctrl] + J_b^T xfrc.  The inverse takes no xfrc_applied, never auto-resets and writes no
+ * per-env state (a later smplsim_step is unaffected); a row with non-finite inputs gets unspecified values in that row only.
+ * Joint-limit rows past the kernels' cap are dropped, as in smplsim_step.  Single-shape handle: any n >= 0 (launched in pieces of at
+ * most num_envs rows on the stream).  Per-env shapes: n == num_envs, row i uses env i's shape.  A handle with self_collision = 1:
+ * SMPLSIM_EUNSUPPORTED (no geom-geom rows in the inverse).
+ * [MJ-upstream] mj_inverse with mjENBL_INVDISCRETE off (engine_inverse.c); not checked against a MuJoCo wheel. */
+int smplsim_inverse(SmplsimHandle* h, const float* qpos_dev, const float* qvel_dev, const float* qacc_dev,
+                    float* qfrc_inverse_dev, float* contact_wrench_dev, int n, void* cuda_stream);
 
 /* compute_humanoid_self_obs_v1 / _v2 (humanoid_env.py:565-688) on caller-supplied body states:
  * qvel[N,nv] (v1), xpos, xquat, linvel, angvel [N,nbody,*] -> obs[N,self_obs_dim]. */

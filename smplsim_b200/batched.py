@@ -239,6 +239,35 @@ class HumanoidBatchB200:
         self.gpu_launches += 1
         return xpos, xquat
 
+    def inverse(self, qpos: torch.Tensor, qvel: torch.Tensor, qacc: torch.Tensor, contact_wrench: bool = False):
+        """mujoco.mj_inverse on caller rows: ``qfrc_inverse [n, nv]`` (and ``contact_wrench [n, nbody, 6]`` when asked), the generalized
+        force that produces ``qacc`` at ``(qpos, qvel)``: ``M qacc + qfrc_bias - J^T f`` with the soft-constraint forces
+        ``f = -D min(0, J qacc - aref)`` of the floor contacts and joint limits.  ``qfrc_inverse[:, 0:6]`` is the root residual (world-frame
+        force, torque about the root body's axes), ``[:, 6:]`` the joint torques.  ``contact_wrench`` uses the convention of
+        ``self.contact_wrench``.  Float32 tensors on this batch's device, ``[n, nq]`` / ``[n, nv]`` / ``[n, nv]``; any n on a one-shape
+        batch, n == num_envs with per-env shapes (row i uses env i's shape).  Reads no env state and changes none; ``xfrc_applied``
+        is not taken.  Not available with ``cfg.env.self_collision``."""
+        m = self.model
+        rows = []
+        for name, t, w in (("qpos", qpos, m.nq), ("qvel", qvel, m.nv), ("qacc", qacc, m.nv)):
+            if not isinstance(t, torch.Tensor):
+                raise ValueError(f"{name} must be a torch.Tensor, got {type(t).__name__}")
+            if t.dim() != 2 or t.shape[1] != w or t.shape[0] != qpos.shape[0]:
+                raise ValueError(f"{name} must have shape [n, {w}] with the same n as qpos, got {tuple(t.shape)}")
+            if t.dtype != torch.float32:
+                raise ValueError(f"{name} must be float32, got {t.dtype}")
+            dv = self.device
+            if t.device.type != dv.type or (dv.index is not None and t.device.index != dv.index):
+                raise ValueError(f"{name} must live on {dv}, got {t.device}")
+            rows.append(t.contiguous())
+        q, v, a = rows
+        n = q.shape[0]
+        out = torch.empty(n, m.nv, dtype=torch.float32, device=self.device)
+        cw = torch.empty(n, m.nbody, 6, dtype=torch.float32, device=self.device) if contact_wrench else None
+        self._check(self._L().smplsim_inverse(self._h, _ptr(q), _ptr(v), _ptr(a), _ptr(out), _ptr(cw), n, self._stream()))
+        self.gpu_launches += 1
+        return (out, cw) if contact_wrench else out
+
     def self_obs(self, version: int, xpos, xquat, qvel=None, linvel=None, angvel=None):
         def prep(t):
             return None if t is None else t.to(self.device, torch.float32).contiguous()

@@ -2290,3 +2290,163 @@ __global__ void __launch_bounds__(256, 1) k_kin5(const float* __restrict__ gimg,
     l_copy<C>(a.xquat + eo * H.nb * 4, sm + C::xq, 4 * H.nb, w);
   }
 }
+
+// ------------------------------------------------------------------ inverse dynamics (mujoco.mj_inverse, mjENBL_INVDISCRETE off)
+// qfrc_inverse = M qacc + qfrc_bias - J^T f with f_r = -D_r min(0, J_r qacc - aref_r) over the floor-contact pyramid rows and the
+// joint-limit rows of the forward pass at (qpos, qvel).  With pyramidal cones every row's soft-constraint force is explicit in qacc, so
+// there is no solve: S1 (kinematics, velocities, bias forces pb, rows with aref / D), one outward sweep of the body accelerations of the
+// given qacc (+ the row residuals), one inward RNE force sweep.  The working-set bits of the rows are set to rs < 0, so the rows carry
+// -D rs on the set, as after a solve that ends on a point whose sign pattern matches its set (l_contact_wrench's "take" branch).
+// [MJ-upstream] engine_inverse.c; not checked against a MuJoCo wheel.
+
+// outward: body accelerations a_b = a_parent + sum_k qacc_k S_k of the given qacc (the ABA's a, without the bias accelerations pb
+// carries), residuals rs = J a - aref of the body's rows, and the body's net inertial force I_b a_b + pb_b into its record's pb slot
+template <class C>
+__device__ __noinline__ void l_inv_acc(const float* ms, float* sm, const LLane& w) {
+  const LHdr& H = l_hdr<C>(ms);
+  const LBody* MB = l_bodies(ms);
+  const float* qa = sm + C::qacc;
+  const bool stepbar = (H.align & 16) && w.bar;
+  const int li = w.li, T = H.T;
+  S6 ca = s6(v3(0.f, 0.f, 0.f), v3(0.f, 0.f, 0.f));
+  if (stepbar) __syncthreads();
+  if (w.live && li == 0) {   // root: the inverse of l_root_acc's map, a = [sum_k qacc[3 + k] c_k ; qacc[0:3]]
+    const float* br = sm + C::body;
+    const V3 c0 = ld3(br + LBR_AX), c1 = ld3(br + LBR_AX + 3), c2 = ld3(br + LBR_AX + 6);
+    const S6 a = s6(qa[3] * c0 + qa[4] * c1 + qa[5] * c2, ld3(qa));
+    l_mbo_put_acc(sm + C::mbo + C::MBOW * MB[0].out_mbox, a);
+    float r10[10];
+    const int ci = l_ld_r10(br, r10);
+    l_rows_eval<C>(H, sm, w, ci & 255, (ci >> 8) & 255, a);
+    l_rec_st_pb<C>(w, 0, rb_mul(r10, a) + l_rec_ld_pb<C>(w, 0), true);
+  }
+  __syncwarp();
+  for (int t = 1; t < T; t++) {
+    if (stepbar) __syncthreads();
+    const int b = H.sched[t][li];
+    if (w.live && b >= 0) {
+      const LBody& lb = MB[b];
+      const float* br = sm + C::body + C::BODYW * b;
+      if (!(lb.flags & LB_CARRY_OUT)) ca = l_mbo_get_acc(sm + C::mbo + C::MBOW * lb.pmbox);
+      const LAxes AX = l_ld_axes(br);
+      S6 a = ca;
+#pragma unroll
+      for (int k = 0; k < 3; k++) {
+        const V3 ax = l_axis(AX, k);
+        a = a + qa[lb.dofadr + k] * s6(ax, cross(AX.x, ax));
+      }
+      ca = a;
+      if (lb.out_mbox >= 0) l_mbo_put_acc(sm + C::mbo + C::MBOW * lb.out_mbox, a);
+      float r10[10];
+      const int ci = l_ld_r10(br, r10), cb = ci & 255, cn = (ci >> 8) & 255, lbs = (ci >> 16) & 255, ln = (ci >> 24) & 255;
+      if (cn) l_rows_eval<C>(H, sm, w, cb, cn, a);
+      for (int e = lbs; e < lbs + ln; e++) {
+        float* le = sm + C::lim + C::LIMW * e;
+        le[LLE_RS] = le[LLE_SG] * qa[((const int*)le)[LLE_DOF]] - le[LLE_AREF];
+      }
+      l_rec_st_pb<C>(w, b, rb_mul(r10, a) + l_rec_ld_pb<C>(w, b), true);
+    }
+    __syncwarp();
+  }
+}
+
+// wrench about the root origin of the floor-contact rows [cb, cb + cn): -D rs on the working set, sum over rows of f_k [cp x d_k ; d_k]
+template <class C>
+__device__ __forceinline__ S6 l_inv_rows(const LHdr& H, float* sm, const LLane& w, int cb, int cn) {
+  const V3 n = ld3(H.plane_n);
+  S6 f = s6(v3(0.f, 0.f, 0.f), v3(0.f, 0.f, 0.f));
+  for (int c = cb; c < cb + cn; c++) {
+    const float* ce = l_centry<C>(sm, w, c);
+    const int info = ((const int*)ce)[LCE_INFO];
+    if (!(info & 1)) continue;
+    const V3 t1 = ld3(ce + LCE_T1), t2 = cross(n, t1);
+    V3 fc = v3(0.f, 0.f, 0.f);
+#pragma unroll
+    for (int k = 0; k < 4; k++) if (info & (2 << k)) fc = fc + (-ce[LCE_D] * ce[LCE_RS + k]) * l_pyr_dir(H, n, t1, t2, k);
+    f.l = f.l + fc; f.a = f.a + cross(ld3(ce + LCE_CP), fc);
+  }
+  return f;
+}
+
+// inward: F_b = (I_b a_b + pb_b) - contact wrench + the subtrees of the children (in registers along a chain, through the in-mailboxes'
+// bias-force words at junctions); tau_k = S_k^T F + armature_k qacc_k - sg f_lim per hinge, the root's six on lane 0.  The result goes to
+// the qvel row of shared memory (dead after S1), which the kernel then copies out.
+template <class C>
+__device__ __noinline__ void l_inv_force(const float* ms, float* sm, const LLane& w) {
+  const LHdr& H = l_hdr<C>(ms);
+  const LBody* MB = l_bodies(ms);
+  const float* qa = sm + C::qacc;
+  float* out = sm + C::qvel;
+  const bool stepbar = (H.align & 16) && w.bar;
+  const int li = w.li;
+  S6 cF = s6(v3(0.f, 0.f, 0.f), v3(0.f, 0.f, 0.f));
+  for (int t = H.T - 1; t >= 1; t--) {
+    if (stepbar) __syncthreads();
+    const int b = H.sched[t][li];
+    if (w.live && b >= 0) {
+      const LBody& lb = MB[b];
+      const float* br = sm + C::body + C::BODYW * b;
+      const int ci = ((const int*)br)[LBR_CI], lbs = (ci >> 16) & 255, ln = (ci >> 24) & 255;
+      S6 F = l_rec_ld_pb<C>(w, b) - l_inv_rows<C>(H, sm, w, ci & 255, (ci >> 8) & 255);
+      if (lb.flags & LB_CARRY_IN) F = F + cF;
+      for (int j = 0; j < lb.nmb; j++) F = F + ld6(sm + C::mbi + C::MBIW * lb.mb[j] + 21);
+      float lf[3] = {0.f, 0.f, 0.f};   // sg f of the joint-limit rows on the working set
+      for (int e = lbs; e < lbs + ln; e++) {
+        const float* le = sm + C::lim + C::LIMW * e;
+        if (!(((const int*)le)[LLE_FLAG] & 1)) continue;
+        const int k = ((const int*)le)[LLE_DOF] - lb.dofadr;
+        const float f = le[LLE_SG] * (-le[LLE_D] * le[LLE_RS]);
+#pragma unroll
+        for (int kk = 0; kk < 3; kk++) if (kk == k) lf[kk] += f;
+      }
+      const LAxes AX = l_ld_axes(br);
+#pragma unroll
+      for (int k = 0; k < 3; k++) {
+        const V3 ax = l_axis(AX, k);
+        const int d = lb.dofadr + k;
+        out[d] = dot6(s6(ax, cross(AX.x, ax)), F) + lb.arm[k] * qa[d] - lf[k];
+      }
+      cF = F;
+      if (lb.in_mbox >= 0) st6(sm + C::mbi + C::MBIW * lb.in_mbox + 21, F);   // the pA words of the in-mailbox
+    }
+    __syncwarp();
+  }
+  if (stepbar) __syncthreads();
+  if (w.live && li == 0) {   // root: free joint S = [0 R ; I 0], armature as l_root_in adds it
+    const LBody& lb = MB[0];
+    const float* br = sm + C::body;
+    const int ci = ((const int*)br)[LBR_CI];
+    S6 F = l_rec_ld_pb<C>(w, 0) - l_inv_rows<C>(H, sm, w, ci & 255, (ci >> 8) & 255);
+    for (int j = 0; j < lb.nmb; j++) F = F + ld6(sm + C::mbi + C::MBIW * lb.mb[j] + 21);
+    const V3 c0 = ld3(br + LBR_AX), c1 = ld3(br + LBR_AX + 3), c2 = ld3(br + LBR_AX + 6);
+    out[0] = F.l.x + H.rarm[0] * qa[0]; out[1] = F.l.y + H.rarm[1] * qa[1]; out[2] = F.l.z + H.rarm[2] * qa[2];
+    out[3] = dot(c0, F.a) + H.rarm[3] * qa[3]; out[4] = dot(c1, F.a) + H.rarm[4] * qa[4]; out[5] = dot(c2, F.a) + H.rarm[5] * qa[5];
+  }
+  __syncwarp();
+}
+
+// mujoco.mj_inverse on caller rows (qpos, qvel, qacc) -> qfrc_inverse (and, cwrench != NULL, the per-body wrench of the row forces).
+// Uses the handle's per-env scratch (lane records, overflow contact entries) of the rows it runs; writes neither the working-set memory
+// (gpfl) nor the sensor rows (gsens), so the stepper cannot tell that it ran.
+struct LInvArgs { const float* qpos; const float* qvel; const float* qacc; float* qfrc; float* cwrench; float* gscr; LMap map; int n; };
+template <class C>
+__global__ void __launch_bounds__(256, 1) k_inverse5(const float* __restrict__ gimg, int img_bytes, LInvArgs a) {
+  const float* ms; LLane w;
+  float* sm = l_setup<C>(gimg, img_bytes, w, ms, a.n, a.map, a.gscr, nullptr, nullptr);
+  const LHdr& H = l_hdr<C>(ms);
+  const size_t eo = w.live ? (size_t)w.env : 0;
+  if (w.live && w.li == 0) { ((int*)sm)[C::misc + LMI_NSELF] = 0; ((int*)sm)[C::misc + LMI_NCON] = 0; ((int*)sm)[C::misc + LMI_NLIM] = 0; }
+  if (w.live) for (int i = w.li; i < (H.nslot + 3) / 4; i += LM_LPE) ((int*)sm)[C::pfl + i] = 0;
+  l_copy_in<C>(sm + C::qpos, a.qpos + eo * (H.nv + 1), H.nv + 1, w);
+  l_copy_in<C>(sm + C::qvel, a.qvel + eo * H.nv, H.nv, w);
+  l_copy_in<C>(sm + C::qacc, a.qacc + eo * H.nv, H.nv, w);
+  __syncwarp();
+  l_sweep_out<C>(ms, sm, w, LF_FK | LF_VEL | LF_COLLIDE, false);
+  l_inv_acc<C>(ms, sm, w);
+  float o4[5];
+  l_rows<C>(sm, w, w.live, 0, 0.f, o4);   // working set := (rs < 0) of every row (its phi / r bookkeeping is not read here)
+  __syncwarp();
+  l_inv_force<C>(ms, sm, w);
+  if (a.cwrench) l_contact_wrench<C>(ms, sm, w, 0, a.cwrench);
+  l_copy_out<C>(a.qfrc + eo * H.nv, sm + C::qvel, H.nv, w);
+}

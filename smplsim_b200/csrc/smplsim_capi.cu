@@ -6,6 +6,7 @@
 #include <cstddef>
 #include <cstdio>
 #include <cstdlib>
+#include <algorithm>
 #include <cstring>
 #include <string>
 #include <vector>
@@ -58,7 +59,7 @@ struct DeviceGuard {   // every entry point runs on the handle's device and rest
 };
 
 extern "C" const char* smplsim_last_error(void) { return g_err.c_str(); }
-extern "C" int smplsim_version(void) { return 220; }   // 220: SmplsimAux.contact_wrench; 210: SmplsimState.xfrc_applied; 200: lane-chain kernels (ABI structs of 110)
+extern "C" int smplsim_version(void) { return 230; }   // 230: smplsim_inverse; 220: SmplsimAux.contact_wrench; 210: SmplsimState.xfrc_applied; 200: lane-chain kernels (ABI structs of 110)
 
 template <class C>
 static size_t cta_smem(const SmplsimHandle* h, int wpb) { return (size_t)h->img.hdr()->bytes + 16 + (size_t)wpb * C::EPW * C::total * 4; }
@@ -94,6 +95,8 @@ static int pick_wpb(SmplsimHandle* h) {
   if (cudaFuncSetAttribute(k_step5<typename C::WithXfrc>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem) != cudaSuccess) return -1;
   if (cudaFuncSetAttribute(k_reset5<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem) != cudaSuccess) return -1;
   if (cudaFuncSetAttribute(k_kin5<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem) != cudaSuccess) return -1;
+  if constexpr (!C::SELFCOL)
+    if (cudaFuncSetAttribute(k_inverse5<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem) != cudaSuccess) return -1;
   return best;
 }
 
@@ -119,6 +122,26 @@ template <class C>
 static void run_kin(SmplsimHandle* h, const LKinArgs& a, cudaStream_t st) {
   int wpb = h->wpb, per = wpb * C::EPW;
   L_LAUNCH(k_kin5<C>, h->nblocks ? h->nblocks : (a.n + per - 1) / per, 32 * wpb, h->smem, st, h->dimg, h->img.hdr()->bytes, a);
+}
+// inverse dynamics: instances without the geom-geom rows only (smplsim_inverse refuses self-collision handles).  One shape: launches of
+// at most num_envs rows (the handle's scratch rows), in order on the caller's stream; per-env shapes: n == num_envs, one launch.
+template <class C>
+static void run_inverse(SmplsimHandle* h, const LInvArgs& a, cudaStream_t st) {
+  if constexpr (!C::SELFCOL) {
+    const LHdr& H = *h->img.hdr();
+    const int wpb = h->wpb, per = wpb * C::EPW;
+    if (h->nblocks) {
+      L_LAUNCH(k_inverse5<C>, h->nblocks, 32 * wpb, h->smem, st, h->dimg, H.bytes, a);
+      return;
+    }
+    for (int r0 = 0; r0 < a.n; r0 += h->num_envs) {
+      LInvArgs c = a;
+      c.n = std::min(h->num_envs, a.n - r0);
+      c.qpos += (size_t)r0 * (H.nv + 1); c.qvel += (size_t)r0 * H.nv; c.qacc += (size_t)r0 * H.nv; c.qfrc += (size_t)r0 * H.nv;
+      if (c.cwrench) c.cwrench += (size_t)r0 * H.nb * 6;
+      L_LAUNCH(k_inverse5<C>, (c.n + per - 1) / per, 32 * wpb, h->smem, st, h->dimg, H.bytes, c);
+    }
+  }
 }
 // dispatch over (model class, self-collision)
 #define L_DISPATCH(h, CALL)                                                   \
@@ -335,6 +358,23 @@ extern "C" int smplsim_kinematics(SmplsimHandle* h, const float* qpos_dev, float
   if (h->nblocks && n != h->num_envs) return fail(SMPLSIM_EINVAL, "smplsim_kinematics: with per-env body shapes n must be the handle's num_envs (row i uses env i's shape)");
   LKinArgs a; a.qpos = qpos_dev; a.xpos = xpos_dev; a.xquat = xquat_dev; a.n = n; a.map = h->map();
   L_DISPATCH(h, run_kin<C_>(h, a, (cudaStream_t)stream));
+  CUDA_TRY(cudaGetLastError());
+  return SMPLSIM_OK;
+}
+
+extern "C" int smplsim_inverse(SmplsimHandle* h, const float* qpos_dev, const float* qvel_dev, const float* qacc_dev, float* qfrc_inverse_dev,
+                               float* contact_wrench_dev, int n, void* stream) {
+  if (!h || n < 0) return fail(SMPLSIM_EINVAL, "smplsim_inverse: null handle or n < 0");
+  if (h->selfcol)
+    return fail(SMPLSIM_EUNSUPPORTED, "smplsim_inverse: the inverse does not build geom-geom contacts (handle created with self_collision = 1)");
+  if (n == 0) return SMPLSIM_OK;   // nothing is read: empty tensors may come as NULL
+  if (!qpos_dev || !qvel_dev || !qacc_dev || !qfrc_inverse_dev) return fail(SMPLSIM_EINVAL, "smplsim_inverse: null argument");
+  if (h->nblocks && n != h->num_envs) return fail(SMPLSIM_EINVAL, "smplsim_inverse: with per-env body shapes n must be the handle's num_envs (row i uses env i's shape)");
+  DeviceGuard guard(h->device);
+  LInvArgs a; std::memset(&a, 0, sizeof a);
+  a.qpos = qpos_dev; a.qvel = qvel_dev; a.qacc = qacc_dev; a.qfrc = qfrc_inverse_dev; a.cwrench = contact_wrench_dev; a.gscr = h->gscr; a.n = n;
+  a.map = h->map();
+  L_DISPATCH(h, run_inverse<C_>(h, a, (cudaStream_t)stream));
   CUDA_TRY(cudaGetLastError());
   return SMPLSIM_OK;
 }

@@ -131,6 +131,20 @@ class MotionLibB200:
                     dof_vel=outs["dof_vel"], xpos=xpos, xquat=xquat, body_vel=bv, body_ang_vel=bav, qpos=outs["qpos"], qvel=outs["qvel"],
                     motion_aa=outs.get("motion_aa"), motion_bodies=self._motion_bodies[ids.long()], frame_idx=frame)
 
+    def inverse_dynamics(self, contact_wrench: bool = False):
+        """``env.inverse`` over every frame of the library: ``qfrc_inverse [total_frames, nv]`` (and ``contact_wrench [total_frames,
+        nbody, 6]``), indexed like the tables.  ``qfrc_inverse[:, 0:6]`` is the root residual force of each frame.  ``qacc`` is the
+        forward difference of ``qvel`` over the clip's ``motion_dt``; a clip's last frame repeats its previous difference (a one-frame clip
+        gets zero), so nothing is differenced across clips."""
+        qpos, qvel = self.tables["qpos"], self.tables["qvel"]
+        idx = torch.arange(qvel.shape[0], device=qvel.device)
+        clip = torch.searchsorted(self.length_starts.long(), idx, right=True) - 1
+        start, last = self.length_starts.long()[clip], (self.length_starts.long() + self._motion_num_frames.long() - 1)[clip]
+        hi = torch.where(idx < last, idx + 1, idx)
+        lo = torch.maximum(hi - 1, start)
+        qacc = (qvel[hi] - qvel[lo]) / self._motion_dt[clip][:, None]
+        return self.env.inverse(qpos, qvel, qacc, contact_wrench=contact_wrench)
+
     # ------------------------------------------------------------------ sampling (motion_lib_base.py:231-312), on the device
     def _uniform(self):
         K = self._num_unique_motions
