@@ -176,7 +176,7 @@ typedef struct SmplsimAux {
 typedef struct SmplsimHandle SmplsimHandle;
 
 const char* smplsim_last_error(void);
-int smplsim_version(void);   /* 230 = this header (220: before smplsim_inverse; 210: before SmplsimAux.contact_wrench; 200: before SmplsimState.xfrc_applied;
+int smplsim_version(void);   /* 240 = this header (230: before smplsim_dynamics; 220: before smplsim_inverse; 210: before SmplsimAux.contact_wrench; 200: before SmplsimState.xfrc_applied;
                               * 100: before pid_* state and aux.status) */
 
 /* MjModel.from_xml_string + MjData + setup_humanoid_properties/setup_controller
@@ -231,6 +231,23 @@ int smplsim_kinematics(SmplsimHandle* h, const float* qpos_dev, float* xpos_dev,
  * [MJ-upstream] mj_inverse with mjENBL_INVDISCRETE off (engine_inverse.c); not checked against a MuJoCo wheel. */
 int smplsim_inverse(SmplsimHandle* h, const float* qpos_dev, const float* qvel_dev, const float* qacc_dev,
                     float* qfrc_inverse_dev, float* contact_wrench_dev, int n, void* cuda_stream);
+
+/* Mass matrix, bias forces and body Jacobians on n caller rows qpos[n,nq], qvel[n,nv] (each output NULL: skipped):
+ *   qM[n,nv,nv]          mujoco.mj_fullM(qM): the dense joint-space inertia, armature on the diagonal; exactly symmetric, exact zeros
+ *                        where neither dof is an ancestor of the other;
+ *   qfrc_bias[n,nv]      mj_rne at qacc = 0: Coriolis, centrifugal and gravity (no constraint rows, no armature term); qvel_dev may be
+ *                        NULL only when qfrc_bias_dev is NULL (qvel is then zero);
+ *   jac[n,njac,6,nv]     mujoco.mj_jacBody at each listed body's frame origin (xpos): rows 0-2 jacp (world-frame linear velocity of the
+ *                        point), rows 3-5 jacr (world-frame angular velocity); columns of dofs off the body's root path are 0.
+ * jac_body: host array of njac robot body indices (0 = root, repeats allowed, njac <= nbody).  Conventions of qvel / qfrc_bias: root
+ * dofs [0:3] world-frame translation / force, [3:6] rotation about / torque along the root body's axes c_k; a root rotation's jacp
+ * column is c_k x (p - root), a hinge's axis x (p - anchor).  Nothing here depends on contacts, so every handle kind is supported; no
+ * per-env state is read or written (a later smplsim_step is unaffected).  Single-shape handle: any n >= 0 (launched in pieces of at
+ * most num_envs rows on the stream).  Per-env shapes: n == num_envs, row i uses env i's shape.  SMPLSIM_EINVAL: a bad body index,
+ * njac > 0 with jac_dev NULL, qfrc_bias without qvel, or every output NULL with n > 0.
+ * [MJ-upstream] mj_fullM / mj_rne / mj_jacBody (engine_support.c, engine_core_smooth.c); not checked against a MuJoCo wheel. */
+int smplsim_dynamics(SmplsimHandle* h, const float* qpos_dev, const float* qvel_dev, int n, float* qM_dev, float* qfrc_bias_dev,
+                     const int32_t* jac_body, int njac, float* jac_dev, void* cuda_stream);
 
 /* compute_humanoid_self_obs_v1 / _v2 (humanoid_env.py:565-688) on caller-supplied body states:
  * qvel[N,nv] (v1), xpos, xquat, linvel, angvel [N,nbody,*] -> obs[N,self_obs_dim]. */

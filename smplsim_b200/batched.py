@@ -239,6 +239,24 @@ class HumanoidBatchB200:
         self.gpu_launches += 1
         return xpos, xquat
 
+    def _rows(self, args):
+        """Caller state rows (name, tensor, width) checked for shape [n, width] with the n of the first, float32 and this batch's device;
+        returned contiguous."""
+        rows = []
+        n = args[0][1].shape[0] if isinstance(args[0][1], torch.Tensor) else None
+        for name, t, w in args:
+            if not isinstance(t, torch.Tensor):
+                raise ValueError(f"{name} must be a torch.Tensor, got {type(t).__name__}")
+            if t.dim() != 2 or t.shape[1] != w or t.shape[0] != n:
+                raise ValueError(f"{name} must have shape [n, {w}] with the same n as qpos, got {tuple(t.shape)}")
+            if t.dtype != torch.float32:
+                raise ValueError(f"{name} must be float32, got {t.dtype}")
+            dv = self.device
+            if t.device.type != dv.type or (dv.index is not None and t.device.index != dv.index):
+                raise ValueError(f"{name} must live on {dv}, got {t.device}")
+            rows.append(t.contiguous())
+        return rows
+
     def inverse(self, qpos: torch.Tensor, qvel: torch.Tensor, qacc: torch.Tensor, contact_wrench: bool = False):
         """mujoco.mj_inverse on caller rows: ``qfrc_inverse [n, nv]`` (and ``contact_wrench [n, nbody, 6]`` when asked), the generalized
         force that produces ``qacc`` at ``(qpos, qvel)``: ``M qacc + qfrc_bias - J^T f`` with the soft-constraint forces
@@ -248,25 +266,59 @@ class HumanoidBatchB200:
         batch, n == num_envs with per-env shapes (row i uses env i's shape).  Reads no env state and changes none; ``xfrc_applied``
         is not taken.  Not available with ``cfg.env.self_collision``."""
         m = self.model
-        rows = []
-        for name, t, w in (("qpos", qpos, m.nq), ("qvel", qvel, m.nv), ("qacc", qacc, m.nv)):
-            if not isinstance(t, torch.Tensor):
-                raise ValueError(f"{name} must be a torch.Tensor, got {type(t).__name__}")
-            if t.dim() != 2 or t.shape[1] != w or t.shape[0] != qpos.shape[0]:
-                raise ValueError(f"{name} must have shape [n, {w}] with the same n as qpos, got {tuple(t.shape)}")
-            if t.dtype != torch.float32:
-                raise ValueError(f"{name} must be float32, got {t.dtype}")
-            dv = self.device
-            if t.device.type != dv.type or (dv.index is not None and t.device.index != dv.index):
-                raise ValueError(f"{name} must live on {dv}, got {t.device}")
-            rows.append(t.contiguous())
-        q, v, a = rows
+        q, v, a = self._rows((("qpos", qpos, m.nq), ("qvel", qvel, m.nv), ("qacc", qacc, m.nv)))
         n = q.shape[0]
         out = torch.empty(n, m.nv, dtype=torch.float32, device=self.device)
         cw = torch.empty(n, m.nbody, 6, dtype=torch.float32, device=self.device) if contact_wrench else None
         self._check(self._L().smplsim_inverse(self._h, _ptr(q), _ptr(v), _ptr(a), _ptr(out), _ptr(cw), n, self._stream()))
         self.gpu_launches += 1
         return (out, cw) if contact_wrench else out
+
+    def dynamics(self, qpos: torch.Tensor, qvel: Optional[torch.Tensor] = None, mass_matrix: bool = True, bias: bool = True,
+                 jac_bodies: Optional[Sequence] = None):
+        """Joint-space mass matrix, bias forces and body Jacobians at caller rows ``(qpos, qvel)``, as MuJoCo's ``mj_fullM(qM)``,
+        ``qfrc_bias`` and ``mj_jacBody``.  Returns a dict with the outputs asked for:
+
+        - ``qM`` ``[n, nv, nv]`` (``mass_matrix``): dense, armature on the diagonal, exactly symmetric;
+        - ``qfrc_bias`` ``[n, nv]`` (``bias``, needs ``qvel``): Coriolis, centrifugal and gravity forces (``mj_rne`` at qacc = 0);
+        - ``jacp`` / ``jacr`` ``[n, k, 3, nv]`` (``jac_bodies``: k robot body indices, 0 = root, or body names): the world-frame linear
+          velocity of each body's origin (``xpos``) and its angular velocity per unit qvel; both are views of one ``[n, k, 6, nv]`` tensor.
+
+        Root dofs follow the qvel convention: ``[0:3]`` world-frame translation, ``[3:6]`` rotation about the root body's axes.  Float32
+        tensors on this batch's device, ``[n, nq]`` / ``[n, nv]``; any n on a one-shape batch, n == num_envs with per-env shapes (row i
+        uses env i's shape).  Reads no env state and changes none; every handle kind (self-collision too) is supported."""
+        m = self.model
+        if bias and qvel is None:
+            raise ValueError("bias=True needs qvel")
+        args = (("qpos", qpos, m.nq),) + ((("qvel", qvel, m.nv),) if qvel is not None else ())
+        rows = self._rows(args)
+        q, v = rows[0], (rows[1] if qvel is not None else None)
+        bodies = []
+        for b in (jac_bodies if jac_bodies is not None else []):
+            if isinstance(b, str):
+                if b not in m.body_names:
+                    raise ValueError(f"unknown body name {b!r}")
+                b = list(m.body_names).index(b)
+            if isinstance(b, bool) or not isinstance(b, (int, np.integer)) or not 0 <= int(b) < m.nbody:
+                raise ValueError(f"jac_bodies entries must be body names or indices in [0, {m.nbody}), got {b!r}")
+            bodies.append(int(b))
+        n, f32 = q.shape[0], dict(dtype=torch.float32, device=self.device)
+        out = {}
+        if mass_matrix:
+            out["qM"] = torch.empty(n, m.nv, m.nv, **f32)
+        if bias:
+            out["qfrc_bias"] = torch.empty(n, m.nv, **f32)
+        jac = None
+        if jac_bodies is not None:
+            jac = torch.empty(n, len(bodies), 6, m.nv, **f32)
+            out["jacp"], out["jacr"] = jac[:, :, :3], jac[:, :, 3:]
+        if mass_matrix or bias or bodies:
+            jb = np.ascontiguousarray(np.asarray(bodies, dtype=np.int32))
+            self._check(self._L().smplsim_dynamics(self._h, _ptr(q), _ptr(v), n, _ptr(out.get("qM")), _ptr(out.get("qfrc_bias")),
+                                                   C.c_void_p(jb.ctypes.data) if bodies else None, len(bodies),
+                                                   _ptr(jac) if bodies else None, self._stream()))
+            self.gpu_launches += 1
+        return out
 
     def self_obs(self, version: int, xpos, xquat, qvel=None, linvel=None, angvel=None):
         def prep(t):

@@ -2450,3 +2450,153 @@ __global__ void __launch_bounds__(256, 1) k_inverse5(const float* __restrict__ g
   if (a.cwrench) l_contact_wrench<C>(ms, sm, w, 0, a.cwrench);
   l_copy_out<C>(a.qfrc + eo * H.nv, sm + C::qvel, H.nv, w);
 }
+
+// ------------------------------------------------------------------ mass matrix, bias forces, body Jacobians (mj_fullM(qM), qfrc_bias, mj_jacBody)
+// M by the composite-rigid-body algorithm.  The rigid inertias of the body rows are world-aligned about the root origin, so a body's
+// composite inertia Ic_b is the plain sum of its subtree's rows: one inward sweep, handed down a chain in registers and through the
+// in-mailboxes' IA words at junctions.  Then f_i = Ic_b S_i for each dof i of body b, and M[i, j] = M[j, i] = S_j . f_i for every dof
+// j on the path from i to the root (dofs are numbered parents first, so j <= i), plus the armature on the diagonal.
+// qfrc_bias is the inverse's RNE at qacc = 0 (no rows: S1 runs without LF_COLLIDE).  [MJ-upstream] engine_support.c (mj_fullM,
+// mj_jacBody), engine_core_smooth.c (mj_crb, mj_rne); not checked against a MuJoCo wheel.
+
+__device__ __forceinline__ int l_dof_body(int d) { return d < 6 ? 0 : (d - 6) / 3 + 1; }   // dofadr = 6 + 3 (b - 1) (lane_build checks it)
+__device__ __forceinline__ bool l_is_anc(const LBody& lb, int a) { return (lb.anc[a >> 5] >> (a & 31)) & 1u; }
+
+// motion subspace of dof d about the root origin: root translation [0 ; e_k], root rotation [c_k ; 0], hinge [a ; x_b x a]
+template <class C>
+__device__ __forceinline__ S6 l_dof_S(const float* sm, int d) {
+  const V3 z = v3(0.f, 0.f, 0.f);
+  if (d < 3) return s6(z, v3(d == 0 ? 1.f : 0.f, d == 1 ? 1.f : 0.f, d == 2 ? 1.f : 0.f));
+  if (d < 6) return s6(ld3(sm + C::body + LBR_AX + 3 * (d - 3)), z);
+  return l_hingeS(sm + C::body + C::BODYW * l_dof_body(d), (d - 6) % 3);
+}
+// where f_d = Ic S_d lives: when nv rows of 6 fit the env's contact-list, limit-row and working-set words (unused here: S1 runs without
+// LF_COLLIDE), there (SMPL); else the root's six in the root scratch and a hinge's in the K words of its body's lane record (SMPL-X).
+// The M writer reads f once per non-zero entry, so shared memory takes an L2 round trip off each of them.
+template <class C> __device__ __forceinline__ constexpr bool l_f_sm() { return 6 * C::NV <= C::misc - C::con; }
+template <class C>
+__device__ __forceinline__ float* l_dof_fp(float* sm, const LLane& w, int d) {
+  if (l_f_sm<C>()) return sm + C::con + 6 * d;
+  if (d < 6) return sm + C::root + 6 * d;
+  return w.gscr + C::grec + C::RECW * l_dof_body(d) + 6 * ((d - 6) % 3);
+}
+
+__device__ __forceinline__ void l_add10(float* I, const float* p) {
+#pragma unroll
+  for (int j = 0; j < 10; j++) I[j] += p[j];
+}
+
+// inward: composite inertias -> f of every dof (l_dof_fp)
+template <class C>
+__device__ __noinline__ void l_crb_in(const float* ms, float* sm, const LLane& w) {
+  const LHdr& H = l_hdr<C>(ms);
+  const LBody* MB = l_bodies(ms);
+  const bool stepbar = (H.align & 16) && w.bar;
+  const int li = w.li;
+  float cI[10];
+#pragma unroll
+  for (int j = 0; j < 10; j++) cI[j] = 0.f;
+  for (int t = H.T - 1; t >= 1; t--) {
+    if (stepbar) __syncthreads();
+    const int b = H.sched[t][li];
+    if (w.live && b >= 0) {
+      const LBody& lb = MB[b];
+      const float* br = sm + C::body + C::BODYW * b;
+      float I[10];
+      l_ld_r10(br, I);
+      if (lb.flags & LB_CARRY_IN) l_add10(I, cI);
+      for (int j = 0; j < lb.nmb; j++) l_add10(I, sm + C::mbi + C::MBIW * lb.mb[j]);
+      const LAxes AX = l_ld_axes(br);
+#pragma unroll
+      for (int k = 0; k < 3; k++) {
+        const V3 ax = l_axis(AX, k);
+        st6(l_dof_fp<C>(sm, w, lb.dofadr + k), rb_mul(I, s6(ax, cross(AX.x, ax))));
+      }
+#pragma unroll
+      for (int j = 0; j < 10; j++) cI[j] = I[j];
+      if (lb.in_mbox >= 0) {
+        float* mi = sm + C::mbi + C::MBIW * lb.in_mbox;   // the IA words of the in-mailbox
+#pragma unroll
+        for (int j = 0; j < 10; j++) mi[j] = I[j];
+      }
+    }
+    __syncwarp();
+  }
+  if (stepbar) __syncthreads();
+  if (w.live && li == 0) {
+    const LBody& lb = MB[0];
+    float I[10];
+    l_ld_r10(sm + C::body, I);
+    for (int j = 0; j < lb.nmb; j++) l_add10(I, sm + C::mbi + C::MBIW * lb.mb[j]);
+    for (int d = 0; d < 6; d++) st6(l_dof_fp<C>(sm, w, d), rb_mul(I, l_dof_S<C>(sm, d)));
+  }
+  __syncwarp();
+}
+
+// the dense [nv, nv] block, row by row, the env's lanes over the columns.  Both halves come from one expression, S_lo . f_hi, at one
+// site (two sites could contract the cross products into FMAs differently), so M is symmetric bit for bit.
+template <class C>
+__device__ __noinline__ void l_write_M(const float* ms, float* sm, const LLane& w, float* __restrict__ out) {
+  const LHdr& H = l_hdr<C>(ms);
+  const LBody* MB = l_bodies(ms);
+  if (!w.live) return;
+  const int nv = H.nv;
+  for (int r = 0; r < nv; r++) {
+    const int br = l_dof_body(r);
+    const float arm = r < 6 ? H.rarm[r] : MB[br].arm[(r - 6) % 3];
+    float* row = out + (size_t)r * nv;
+    for (int c = w.li; c < nv; c += LM_LPE) {
+      const int lo = min(r, c), hi = max(r, c);
+      float v = 0.f;
+      if (l_is_anc(MB[l_dof_body(hi)], l_dof_body(lo))) v = dot6(l_dof_S<C>(sm, lo), ld6(l_dof_fp<C>(sm, w, hi)));
+      row[c] = c == r ? v + arm : v;
+    }
+  }
+}
+
+// the [6, nv] block of body p: rows 0-2 jacp (velocity of the body origin), 3-5 jacr; the env's lanes over the columns
+template <class C>
+__device__ __noinline__ void l_write_jac(const float* ms, const float* sm, const LLane& w, int p, float* __restrict__ o) {
+  const LHdr& H = l_hdr<C>(ms);
+  const LBody& lb = l_bodies(ms)[p];
+  if (!w.live) return;
+  const int nv = H.nv;
+  const V3 xp = ld3(sm + C::body + C::BODYW * p + LBR_X);
+  for (int c = w.li; c < nv; c += LM_LPE) {
+    V3 jp = v3(0.f, 0.f, 0.f), jr = jp;
+    if (l_is_anc(lb, l_dof_body(c))) {
+      const S6 S = l_dof_S<C>(sm, c);
+      jp = S.l + cross(S.a, xp); jr = S.a;
+    }
+    o[c] = jp.x; o[nv + c] = jp.y; o[2 * nv + c] = jp.z; o[3 * nv + c] = jr.x; o[4 * nv + c] = jr.y; o[5 * nv + c] = jr.z;
+  }
+}
+
+// qM [n, nv, nv], qfrc_bias [n, nv], body Jacobians [n, njac, 6, nv] (each NULL: skipped) on caller rows (qpos, qvel; qvel NULL: zero,
+// only without bias).  Uses the handle's per-env scratch of the rows it runs (lane records); writes neither the working-set memory nor
+// the sensor rows, so the stepper cannot tell that it ran.
+struct LDynArgs { const float* qpos; const float* qvel; float* qM; float* bias; float* jac; float* gscr; LMap map; int n, njac; unsigned char jb[LM_MAXB]; };
+template <class C>
+__global__ void __launch_bounds__(256, 1) k_dyn5(const float* __restrict__ gimg, int img_bytes, LDynArgs a) {
+  const float* ms; LLane w;
+  float* sm = l_setup<C>(gimg, img_bytes, w, ms, a.n, a.map, a.gscr, nullptr, nullptr);
+  const LHdr& H = l_hdr<C>(ms);
+  const size_t eo = w.live ? (size_t)w.env : 0;
+  l_copy_in<C>(sm + C::qpos, a.qpos + eo * (H.nv + 1), H.nv + 1, w);
+  if (a.qvel) l_copy_in<C>(sm + C::qvel, a.qvel + eo * H.nv, H.nv, w);
+  else if (w.live) for (int i = w.li; i < H.nv; i += LM_LPE) sm[C::qvel + i] = 0.f;
+  if (w.live) for (int i = w.li; i < H.nv; i += LM_LPE) sm[C::qacc + i] = 0.f;
+  __syncwarp();
+  l_sweep_out<C>(ms, sm, w, LF_FK | LF_VEL, false);
+  if (a.qM) {
+    l_crb_in<C>(ms, sm, w);
+    l_write_M<C>(ms, sm, w, a.qM + eo * H.nv * H.nv);
+  }
+  if (a.jac)
+    for (int j = 0; j < a.njac; j++) l_write_jac<C>(ms, sm, w, a.jb[j], a.jac + (eo * a.njac + j) * 6 * H.nv);
+  if (a.bias) {
+    l_inv_acc<C>(ms, sm, w);
+    l_inv_force<C>(ms, sm, w);
+    l_copy_out<C>(a.bias + eo * H.nv, sm + C::qvel, H.nv, w);
+  }
+}

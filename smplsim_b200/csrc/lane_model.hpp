@@ -60,7 +60,7 @@ struct LBody {   // 72 words
   int ngeom, limited, in_mbox, out_mbox;       // limited: bit k = dof k has a range ; mailbox ids or -1
   int pmbox, nmb, step, lane;                  // pmbox: parent's outward mailbox (-1: carry)
   signed char mb[LM_MAXMB];                    // inward mailboxes of the children that do not arrive by carry
-  int pad1[2];
+  unsigned anc[2];                             // bit a (word a / 32): body a is this body or one of its ancestors
 };
 
 #define LM_BODY_OFF ((sizeof(LHdr) + 15) & ~(size_t)15)   // byte offset of the LBody array in the image (compile-time: the kernels add no header load)
@@ -101,6 +101,7 @@ static inline std::string lane_build(const SmplsimModelDesc* s, const SmplsimEnv
   for (int b = 1; b < nb; b++) {
     if (s->body_parent[b] < 0 || s->body_parent[b] >= b) return "bodies must be listed parent-first";
     if (s->body_dofnum[b] != 3) return "model class: exactly three hinges on every non-root body (SMPL family)";
+    if (s->body_dofadr[b] != 6 + 3 * (b - 1)) return "model class: dofs numbered in body order";
   }
   // ---- geom pairs that pass MuJoCo's filters (same body, filterparent, contype / conaffinity, <exclude>); capsule / sphere only
   std::vector<LPair> pairs;
@@ -173,6 +174,8 @@ static inline std::string lane_build(const SmplsimModelDesc* s, const SmplsimEnv
     for (int k = 0; k < 6; k++) L.inertia[k] = (float)s->body_inertia[6 * b + k];
     L.mass = (float)s->body_mass[b]; L.tiw0 = (float)s->body_invweight0[2 * b];
     L.parent = parent[b]; L.dofadr = s->body_dofadr[b]; L.step = step[b]; L.lane = lane[b];
+    L.anc[0] = L.anc[1] = 0u;
+    for (int a = b; a >= 0; a = parent[a]) L.anc[a >> 5] |= 1u << (a & 31);
     L.in_mbox = L.out_mbox = L.pmbox = -1; L.nmb = 0; L.geom0 = 0; L.ngeom = 0; L.limited = 0; L.flags = 0;
     memset(L.mb, -1, sizeof L.mb);
     if (b > 0) {

@@ -59,7 +59,7 @@ struct DeviceGuard {   // every entry point runs on the handle's device and rest
 };
 
 extern "C" const char* smplsim_last_error(void) { return g_err.c_str(); }
-extern "C" int smplsim_version(void) { return 230; }   // 230: smplsim_inverse; 220: SmplsimAux.contact_wrench; 210: SmplsimState.xfrc_applied; 200: lane-chain kernels (ABI structs of 110)
+extern "C" int smplsim_version(void) { return 240; }   // 240: smplsim_dynamics; 230: smplsim_inverse; 220: SmplsimAux.contact_wrench; 210: SmplsimState.xfrc_applied; 200: lane-chain kernels (ABI structs of 110)
 
 template <class C>
 static size_t cta_smem(const SmplsimHandle* h, int wpb) { return (size_t)h->img.hdr()->bytes + 16 + (size_t)wpb * C::EPW * C::total * 4; }
@@ -97,6 +97,7 @@ static int pick_wpb(SmplsimHandle* h) {
   if (cudaFuncSetAttribute(k_kin5<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem) != cudaSuccess) return -1;
   if constexpr (!C::SELFCOL)
     if (cudaFuncSetAttribute(k_inverse5<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem) != cudaSuccess) return -1;
+  if (cudaFuncSetAttribute(k_dyn5<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem) != cudaSuccess) return -1;
   return best;
 }
 
@@ -141,6 +142,26 @@ static void run_inverse(SmplsimHandle* h, const LInvArgs& a, cudaStream_t st) {
       if (c.cwrench) c.cwrench += (size_t)r0 * H.nb * 6;
       L_LAUNCH(k_inverse5<C>, (c.n + per - 1) / per, 32 * wpb, h->smem, st, h->dimg, H.bytes, c);
     }
+  }
+}
+// mass matrix / bias / Jacobians: every instance (no contact rows).  Chunked as the inverse.
+template <class C>
+static void run_dynamics(SmplsimHandle* h, const LDynArgs& a, cudaStream_t st) {
+  const LHdr& H = *h->img.hdr();
+  const int wpb = h->wpb, per = wpb * C::EPW;
+  if (h->nblocks) {
+    L_LAUNCH(k_dyn5<C>, h->nblocks, 32 * wpb, h->smem, st, h->dimg, H.bytes, a);
+    return;
+  }
+  for (int r0 = 0; r0 < a.n; r0 += h->num_envs) {
+    LDynArgs c = a;
+    c.n = std::min(h->num_envs, a.n - r0);
+    c.qpos += (size_t)r0 * (H.nv + 1);
+    if (c.qvel) c.qvel += (size_t)r0 * H.nv;
+    if (c.qM) c.qM += (size_t)r0 * H.nv * H.nv;
+    if (c.bias) c.bias += (size_t)r0 * H.nv;
+    if (c.jac) c.jac += (size_t)r0 * c.njac * 6 * H.nv;
+    L_LAUNCH(k_dyn5<C>, (c.n + per - 1) / per, 32 * wpb, h->smem, st, h->dimg, H.bytes, c);
   }
 }
 // dispatch over (model class, self-collision)
@@ -375,6 +396,31 @@ extern "C" int smplsim_inverse(SmplsimHandle* h, const float* qpos_dev, const fl
   a.qpos = qpos_dev; a.qvel = qvel_dev; a.qacc = qacc_dev; a.qfrc = qfrc_inverse_dev; a.cwrench = contact_wrench_dev; a.gscr = h->gscr; a.n = n;
   a.map = h->map();
   L_DISPATCH(h, run_inverse<C_>(h, a, (cudaStream_t)stream));
+  CUDA_TRY(cudaGetLastError());
+  return SMPLSIM_OK;
+}
+
+extern "C" int smplsim_dynamics(SmplsimHandle* h, const float* qpos_dev, const float* qvel_dev, int n, float* qM_dev, float* qfrc_bias_dev,
+                                const int32_t* jac_body, int njac, float* jac_dev, void* stream) {
+  if (!h || n < 0 || njac < 0) return fail(SMPLSIM_EINVAL, "smplsim_dynamics: null handle, n < 0 or njac < 0");
+  const LHdr& H = *h->img.hdr();
+  if (njac > H.nb) return fail(SMPLSIM_EINVAL, "smplsim_dynamics: njac > nbody");
+  if (njac > 0 && !jac_body) return fail(SMPLSIM_EINVAL, "smplsim_dynamics: njac > 0 needs jac_body");
+  for (int j = 0; j < njac; j++)
+    if (jac_body[j] < 0 || jac_body[j] >= H.nb) return fail(SMPLSIM_EINVAL, "smplsim_dynamics: jac_body entry out of range [0, nbody)");
+  if (qfrc_bias_dev && !qvel_dev) return fail(SMPLSIM_EINVAL, "smplsim_dynamics: qfrc_bias needs qvel");
+  if (n == 0) return SMPLSIM_OK;   // nothing is read: empty tensors may come as NULL
+  if (njac > 0 && !jac_dev) return fail(SMPLSIM_EINVAL, "smplsim_dynamics: njac > 0 needs jac_dev");
+  if (!qM_dev && !qfrc_bias_dev && !njac) return fail(SMPLSIM_EINVAL, "smplsim_dynamics: no output requested");
+  if (!qpos_dev) return fail(SMPLSIM_EINVAL, "smplsim_dynamics: null qpos");
+  if (h->nblocks && n != h->num_envs) return fail(SMPLSIM_EINVAL, "smplsim_dynamics: with per-env body shapes n must be the handle's num_envs (row i uses env i's shape)");
+  DeviceGuard guard(h->device);
+  LDynArgs a; std::memset(&a, 0, sizeof a);
+  a.qpos = qpos_dev; a.qvel = qvel_dev; a.qM = qM_dev; a.bias = qfrc_bias_dev; a.jac = njac ? jac_dev : nullptr; a.gscr = h->gscr; a.n = n;
+  a.njac = njac;
+  for (int j = 0; j < njac; j++) a.jb[j] = (unsigned char)jac_body[j];
+  a.map = h->map();
+  L_DISPATCH(h, run_dynamics<C_>(h, a, (cudaStream_t)stream));
   CUDA_TRY(cudaGetLastError());
   return SMPLSIM_OK;
 }

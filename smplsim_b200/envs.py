@@ -48,6 +48,60 @@ class _Contacts:
         self.geom1 = np.zeros_like(self.geom2)
 
 
+def _dof_tree(m):
+    """MuJoCo's ``dof_parentid``, ``dof_Madr`` and ``nM`` for the model: the compressed ``qM`` holds, for each dof i in turn,
+    ``M[i, i]`` followed by ``M[i, j]`` for each ancestor dof j, nearest first."""
+    par = np.full(m.nv, -1, dtype=np.int32)
+    for b in range(m.nbody):
+        d0, nd, p = int(m.body_dofadr[b]), int(m.body_dofnum[b]), int(m.body_parent[b])
+        par[d0] = -1 if p < 0 else int(m.body_dofadr[p] + m.body_dofnum[p] - 1)
+        par[d0 + 1:d0 + nd] = np.arange(d0, d0 + nd - 1)
+    adr = np.zeros(m.nv, dtype=np.int32)
+    n = 0
+    for i in range(m.nv):
+        adr[i] = n
+        j = i
+        while j >= 0:
+            n += 1
+            j = par[j]
+    return par, adr, n
+
+
+def _pairs(parentid):
+    """(i, j) in qM order: every dof i with itself and its ancestors."""
+    for i in range(len(parentid)):
+        j = i
+        while j >= 0:
+            yield i, j
+            j = parentid[j]
+
+
+def mj_fullM(model, dst, qM):
+    """``mujoco.mj_fullM``: expand the compressed ``qM`` (``model.dof_Madr`` layout) into the dense symmetric ``dst`` [nv, nv], in place."""
+    nv = model.nv
+    d = dst.reshape(nv * nv)
+    d[:] = 0.0
+    for k, (i, j) in enumerate(_pairs(model.dof_parentid)):
+        d[i * nv + j] = d[j * nv + i] = qM[k]
+
+
+class _MjData(SimpleNamespace):
+    """``mj_data`` view.  ``qM`` / ``qfrc_bias`` cost a kernel call, so they are evaluated on first read."""
+
+    @property
+    def qM(self):
+        return self._dyn()[0]
+
+    @property
+    def qfrc_bias(self):
+        return self._dyn()[1]
+
+    def _dyn(self):
+        if "_dyn_val" not in self.__dict__:
+            self._dyn_val = self._dyn_fn()
+        return self._dyn_val
+
+
 class HumanoidEnvB200(_EnvBase):
     metadata = {"render_modes": ["human", "rgb_array"], "render_fps": 30}
     TASK = None
@@ -92,6 +146,7 @@ class HumanoidEnvB200(_EnvBase):
         self.contact_bodies = list(e.contact_bodies)
         self.contact_bodies_ids = [m.geom_names.index(n) + 1 for n in self.contact_bodies]
         self.floor_idx = 0
+        self._dof_parentid, self._dof_Madr, self._nM = _dof_tree(m)
         self.jkp, self.jkd, self.torque_lim = m.act_kp.copy(), m.act_kd.copy(), m.act_torque_lim.copy()
         self._pd_action_scale, self._pd_action_offset = m.act_scale.copy(), m.act_offset.copy()
         self.observation_space = _Box(-np.inf * np.ones(self.get_obs_size(), dtype=np.float32),
@@ -160,10 +215,12 @@ class HumanoidEnvB200(_EnvBase):
     # ------------------------------------------------------------------ mj_data-style views (examples poke env.mj_data)
     @property
     def mj_data(self):
+        """``qM`` (compressed, ``mj_model.dof_Madr`` layout) and ``qfrc_bias`` are those of the last forward pass, at
+        ``(qpos_fwd, qvel_fwd)``, as on an MjData after ``mj_step``."""
         b = self._b
         sens = np.concatenate([b.body_linvel[0].cpu().numpy().ravel(), b.body_angvel[0].cpu().numpy().ravel()])
         z3, z4 = np.zeros((1, 3)), np.array([[1.0, 0, 0, 0]])
-        return SimpleNamespace(qpos=b.qpos[0].cpu().numpy().astype(np.float64), qvel=b.qvel[0].cpu().numpy().astype(np.float64),
+        return _MjData(_dyn_fn=self._fwd_dynamics, qpos=b.qpos[0].cpu().numpy().astype(np.float64), qvel=b.qvel[0].cpu().numpy().astype(np.float64),
                                ctrl=b.ctrl[0].cpu().numpy().astype(np.float64), qacc=b.qacc[0].cpu().numpy().astype(np.float64),
                                xpos=np.concatenate([z3, b.xpos[0].cpu().numpy()]), xquat=np.concatenate([z4, b.xquat[0].cpu().numpy()]),
                                sensordata=sens, contact=_Contacts(int(b.contact_mask[0].item())),
@@ -181,7 +238,43 @@ class HumanoidEnvB200(_EnvBase):
         return SimpleNamespace(nbody=m.nbody + 1, nq=m.nq, nv=m.nv, nu=m.nu, ngeom=len(m.geom_names) + 1, opt=SimpleNamespace(timestep=self.sim_timestep),
                                body=lambda i: SimpleNamespace(name=names[i], id=i), joint=lambda n: joints[n],
                                geom=lambda i: SimpleNamespace(name=(["floor"] + list(m.geom_names))[i], id=i),
-                               body_mass=np.concatenate([[0.0], np.asarray(m.body_mass)]))
+                               body_mass=np.concatenate([[0.0], np.asarray(m.body_mass)]),
+                               nM=self._nM, dof_Madr=self._dof_Madr.copy(), dof_parentid=self._dof_parentid.copy())
+
+    def _fwd_dynamics(self):
+        """(compressed qM, qfrc_bias) at the state of the last forward pass."""
+        b = self._b
+        out = b.dynamics(b.qpos_fwd, b.qvel_fwd)
+        M = out["qM"][0].cpu().numpy().astype(np.float64)
+        qM = np.array([M[i, j] for i, j in _pairs(self._dof_parentid)])
+        return qM, out["qfrc_bias"][0].cpu().numpy().astype(np.float64)
+
+    def get_body_jac_by_id(self, id, jacp=None, jacr=None):
+        """``mujoco.mj_jacBody`` at the current qpos for MuJoCo body id ``id`` (0 = world: zeros): the [3, nv] translational and
+        rotational Jacobians of the body's frame origin.  Fills ``jacp`` / ``jacr`` in place when given (any shape of 3 nv entries);
+        returns (jacp, jacr), new arrays where none were given."""
+        nv = self._b.model.nv
+        jp, jr = np.zeros((3, nv)), np.zeros((3, nv))
+        if id != 0:
+            out = self._b.dynamics(self._b.qpos, mass_matrix=False, bias=False, jac_bodies=[int(id) - 1])
+            jp, jr = (out[k][0, 0].cpu().numpy().astype(np.float64) for k in ("jacp", "jacr"))
+        if jacp is not None:
+            jacp.reshape(3 * nv)[:] = jp.ravel()
+        if jacr is not None:
+            jacr.reshape(3 * nv)[:] = jr.ravel()
+        return (jp if jacp is None else jacp), (jr if jacr is None else jacr)
+
+    def get_body_jacp_by_name(self, name, jacp=None, jacr=None):
+        """jacp [3, nv] of the named body (``jacr`` filled too when given)."""
+        return self.get_body_jac_by_id(self.mj_body_names.index(name), jacp=jacp, jacr=jacr)[0]
+
+    def get_body_xvelp(self, name):
+        """World-frame linear velocity of the named body's origin: jacp . qvel."""
+        return self.get_body_jacp_by_name(name).reshape(3, -1) @ self.get_qvel()
+
+    def get_body_xvelr(self, name):
+        """World-frame angular velocity of the named body: jacr . qvel."""
+        return self.get_body_jac_by_id(self.mj_body_names.index(name))[1].reshape(3, -1) @ self.get_qvel()
 
     def get_qpos(self):
         return self._b.qpos[0].cpu().numpy().astype(np.float64)
