@@ -125,6 +125,12 @@ struct LLane {
   int* gpfl;       // working set per contact slot carried across launches (handle-internal scratch, r4(NS / 4) words per env)
   float* gsens;    // framelinvel / frameangvel of the last forward pass [6 nb] of this env (global scratch; NULL: not wanted)
 };
+// The sweeps and the functions they call take the LLane by reference but work on a copy of it.  A reference parameter points into the
+// caller's stack frame, and ptxas cannot prove that the sweeps' stores (records, mailboxes, rows) miss it, so it reloads gscr / li /
+// gbase / gmask from the stack after every store: an LDL in front of each record access, often an L1 miss with 225 KB of shared
+// memory configured.  The copy stays in registers.  The self-collision instances keep the reference: they sit at the 255-register
+// cap, and the copy's live registers cost them more spills than the reloads it removes.
+#define L_LANE_BY_VALUE(C, w, ref) const LLane w##_copy = ref; const LLane& w = C::SELFCOL ? ref : w##_copy
 
 template <class C> __device__ __forceinline__ const LHdr& l_hdr(const float* ms) { return *(const LHdr*)ms; }
 __device__ __forceinline__ const LBody* l_bodies(const float* ms) { return (const LBody*)((const char*)ms + LM_BODY_OFF); }
@@ -189,37 +195,70 @@ static inline unsigned __float_as_uint(float f) { return emu_bits(f); }
 static inline int __float_as_int(float f) { return (int)emu_bits(f); }
 static inline float __int_as_float(int i) { return emu_float((unsigned)i); }
 static inline float __uint_as_float(unsigned u) { return emu_float(u); }
+template <class T> static inline T __ldca(const T* p) { return *p; }
+template <class T> static inline void __stwb(T* p, T v) { *p = v; }
+static inline float2 make_float2(float x, float y) { float2 r = {x, y}; return r; }
 #endif
 
-// K (3 x 6) and c (3) of body b (b < 0: a lane without a body this step reads body 0's record and ignores it)
+// The records are global memory: explicit global loads / stores (LDG / STG instead of generic LD / ST, which first test the address
+// for shared or local memory) with the default cache policy.  L2-only (__ldcg / __stcg) was measured slower on H100: cfg2 k_step5
+// 2.21 ms against 2.19 ms, and the self-collision step 8.0 ms against 7.7 ms.
+__device__ __forceinline__ float4 l_gld4(const float* p) { return __ldca((const float4*)p); }
+__device__ __forceinline__ float2 l_gld2(const float* p) { return __ldca((const float2*)p); }
+__device__ __forceinline__ float l_gld1(const float* p) { return __ldca(p); }
+__device__ __forceinline__ void l_gst4(float* p, float4 v) { __stwb((float4*)p, v); }
+__device__ __forceinline__ void l_gst2(float* p, float2 v) { __stwb((float2*)p, v); }
+__device__ __forceinline__ void l_gst1(float* p, float v) { __stwb(p, v); }
+
+// K (3 x 6) and c (3) of body b (b < 0: a lane without a body this step reads body 0's record and ignores it): 5 x 128 bits + 1 word
 template <class C>
 __device__ __forceinline__ void l_rec_ld_Kc(const LLane& w, int b, float* K, float* c) {
-  const float4* p = (const float4*)(w.gscr + C::grec + C::RECW * (b < 0 ? 0 : b));
-  float4 v0 = p[0], v1 = p[1], v2 = p[2], v3 = p[3], v4 = p[4], v5 = p[5];
+  const float* p = w.gscr + C::grec + C::RECW * (b < 0 ? 0 : b);
+  if constexpr (C::SELFCOL) {   // generic accesses: the self-collision step measured 2 % slower with the global ones (H100, 7.9 vs 7.7 ms)
+    const float4* q = (const float4*)p;
+    float4 v0 = q[0], v1 = q[1], v2 = q[2], v3 = q[3], v4 = q[4], v5 = q[5];
+    K[0] = v0.x; K[1] = v0.y; K[2] = v0.z; K[3] = v0.w; K[4] = v1.x; K[5] = v1.y; K[6] = v1.z; K[7] = v1.w;
+    K[8] = v2.x; K[9] = v2.y; K[10] = v2.z; K[11] = v2.w; K[12] = v3.x; K[13] = v3.y; K[14] = v3.z; K[15] = v3.w;
+    K[16] = v4.x; K[17] = v4.y; c[0] = v4.z; c[1] = v4.w; c[2] = v5.x;
+    return;
+  }
+  float4 v0 = l_gld4(p), v1 = l_gld4(p + 4), v2 = l_gld4(p + 8), v3 = l_gld4(p + 12), v4 = l_gld4(p + 16);
   K[0] = v0.x; K[1] = v0.y; K[2] = v0.z; K[3] = v0.w; K[4] = v1.x; K[5] = v1.y; K[6] = v1.z; K[7] = v1.w;
   K[8] = v2.x; K[9] = v2.y; K[10] = v2.z; K[11] = v2.w; K[12] = v3.x; K[13] = v3.y; K[14] = v3.z; K[15] = v3.w;
-  K[16] = v4.x; K[17] = v4.y; c[0] = v4.z; c[1] = v4.w; c[2] = v5.x;
+  K[16] = v4.x; K[17] = v4.y; c[0] = v4.z; c[1] = v4.w; c[2] = l_gld1(p + 20);
 }
 template <class C>
 __device__ __forceinline__ void l_rec_st_Kc(const LLane& w, int b, const float* K, const float* c, bool wr) {
   if (wr && b >= 0) {
-    float4* p = (float4*)(w.gscr + C::grec + C::RECW * b);
-    p[0] = make_float4(K[0], K[1], K[2], K[3]); p[1] = make_float4(K[4], K[5], K[6], K[7]);
-    p[2] = make_float4(K[8], K[9], K[10], K[11]); p[3] = make_float4(K[12], K[13], K[14], K[15]);
-    p[4] = make_float4(K[16], K[17], c[0], c[1]);
-    ((float*)p)[20] = c[2];
+    float* p = w.gscr + C::grec + C::RECW * b;
+    if constexpr (C::SELFCOL) {
+      float4* q = (float4*)p;
+      q[0] = make_float4(K[0], K[1], K[2], K[3]); q[1] = make_float4(K[4], K[5], K[6], K[7]);
+      q[2] = make_float4(K[8], K[9], K[10], K[11]); q[3] = make_float4(K[12], K[13], K[14], K[15]);
+      q[4] = make_float4(K[16], K[17], c[0], c[1]);
+      p[20] = c[2];
+      return;
+    }
+    l_gst4(p, make_float4(K[0], K[1], K[2], K[3])); l_gst4(p + 4, make_float4(K[4], K[5], K[6], K[7]));
+    l_gst4(p + 8, make_float4(K[8], K[9], K[10], K[11])); l_gst4(p + 12, make_float4(K[12], K[13], K[14], K[15]));
+    l_gst4(p + 16, make_float4(K[16], K[17], c[0], c[1]));
+    l_gst1(p + 20, c[2]);
   }
 }
+// pb at words 22..27: 8-byte aligned (records are 112 bytes, the scratch 16-byte aligned), so three 64-bit accesses
 template <class C>
 __device__ __forceinline__ S6 l_rec_ld_pb(const LLane& w, int b) {
   const float* p = w.gscr + C::grec + C::RECW * (b < 0 ? 0 : b) + 22;
-  return s6(v3(p[0], p[1], p[2]), v3(p[3], p[4], p[5]));
+  if constexpr (C::SELFCOL) return s6(v3(p[0], p[1], p[2]), v3(p[3], p[4], p[5]));
+  const float2 u = l_gld2(p), v = l_gld2(p + 2), x = l_gld2(p + 4);
+  return s6(v3(u.x, u.y, v.x), v3(v.y, x.x, x.y));
 }
 template <class C>
 __device__ __forceinline__ void l_rec_st_pb(const LLane& w, int b, S6 pb, bool wr) {
   if (wr && b >= 0) {
     float* p = w.gscr + C::grec + C::RECW * b + 22;
-    st3(p, pb.a); st3(p + 3, pb.l);
+    if constexpr (C::SELFCOL) { st3(p, pb.a); st3(p + 3, pb.l); return; }
+    l_gst2(p, make_float2(pb.a.x, pb.a.y)); l_gst2(p + 2, make_float2(pb.a.z, pb.l.x)); l_gst2(p + 4, make_float2(pb.l.y, pb.l.z));
   }
 }
 
@@ -502,7 +541,8 @@ __device__ __forceinline__ int l_narrow(const LHdr& H, const LGeom& G, int g, co
 // rigid inertia, bias force, contacts of the root's geom.  Children read the pose from the root's out-mailbox.
 struct LRootOut { int ncon, npresent; unsigned long long gbits; };
 template <class C>
-__device__ __noinline__ LRootOut l_root_out(const float* ms, float* sm, const LLane& w, int flags, float h0) {
+__device__ __noinline__ LRootOut l_root_out(const float* ms, float* sm, const LLane& w_, int flags, float h0) {
+  L_LANE_BY_VALUE(C, w, w_);
   const LHdr& H = l_hdr<C>(ms);
   const LBody& lb = l_bodies(ms)[0];
   LRootOut R; R.ncon = 0; R.npresent = 0; R.gbits = 0ull;
@@ -552,7 +592,8 @@ __device__ __noinline__ LRootOut l_root_out(const float* ms, float* sm, const LL
 }
 
 template <class C>
-__device__ __noinline__ LFkOut l_sweep_out(const float* ms, float* sm, const LLane& w, int flags, bool ztau) {
+__device__ __noinline__ LFkOut l_sweep_out(const float* ms, float* sm, const LLane& w_, int flags, bool ztau) {
+  L_LANE_BY_VALUE(C, w, w_);
   const LHdr& H = l_hdr<C>(ms);
   const LBody* MB = l_bodies(ms);
   const LGeom* MG = l_geoms(ms);
@@ -867,7 +908,8 @@ __device__ __forceinline__ void l_self_fix(float* sm, const LLane& w, bool on, f
 // default tangent (mju_makeFrame); impedance / R / aref as for the floor rows with tran = invweight0(b1) + invweight0(b2).
 // Returns the number of contacts of this lane's env; *dropped: more than L_MAXSELF touched.
 template <class C>
-__device__ __noinline__ int l_self_collide(const float* ms, float* sm, const LLane& w, int* dropped) {
+__device__ __noinline__ int l_self_collide(const float* ms, float* sm, const LLane& w_, int* dropped) {
+  L_LANE_BY_VALUE(C, w, w_);
   const LHdr& H = l_hdr<C>(ms);
   const LBody* MB = l_bodies(ms);
   const LGeom* MG = l_geoms(ms);
@@ -956,7 +998,8 @@ __device__ __noinline__ int l_self_collide(const float* ms, float* sm, const LLa
 // 6 x 6 system of its six dofs; the root's spatial acceleration stays in shared memory (LRT_A) for the outward sweeps.  Returns "the root
 // has constraint rows in its subtree" (lane 0).
 template <class C, bool SPD>
-__device__ __noinline__ bool l_root_in(const float* ms, float* sm, const LLane& w, bool need, int flags) {
+__device__ __noinline__ bool l_root_in(const float* ms, float* sm, const LLane& w_, bool need, int flags) {
+  L_LANE_BY_VALUE(C, w, w_);
   const LHdr& H = l_hdr<C>(ms);
   const LBody& lb = l_bodies(ms)[0];
   S6 p = l_rec_ld_pb<C>(w, 0);
@@ -1051,7 +1094,8 @@ __device__ __noinline__ bool l_root_in(const float* ms, float* sm, const LLane& 
 // SPD (compile time): the stable-PD system (LI_SPD, optionally LI_INTEGRATE; never a re-sweep) -- the two uses share no flag-dependent code,
 // so each instance carries only its own
 template <class C, bool SPD>
-__device__ __noinline__ void l_sweep_in(const float* ms, float* sm, const LLane& w, bool run, int flags, LSolveLane& st_) {
+__device__ __noinline__ void l_sweep_in(const float* ms, float* sm, const LLane& w_, bool run, int flags, LSolveLane& st_) {
+  L_LANE_BY_VALUE(C, w, w_);
   const LHdr& H = l_hdr<C>(ms);
   const LBody* MB = l_bodies(ms);
   LSolveLane st = st_;
@@ -1156,7 +1200,8 @@ __device__ __noinline__ void l_sweep_in(const float* ms, float* sm, const LLane&
 // root body of the acceleration sweep: the spatial acceleration solved at the end of the inward sweep (l_root_in) -> the six
 // free-joint accelerations S^T a, the root's out-mailbox, residuals of the root's contact rows
 template <class C>
-__device__ __noinline__ void l_root_acc(const float* ms, float* sm, const LLane& w, bool run, float* qout, bool* same) {
+__device__ __noinline__ void l_root_acc(const float* ms, float* sm, const LLane& w_, bool run, float* qout, bool* same) {
+  L_LANE_BY_VALUE(C, w, w_);
   const LHdr& H = l_hdr<C>(ms);
   const LBody& lb = l_bodies(ms)[0];
   if (run && w.li == 0) {
@@ -1177,7 +1222,8 @@ __device__ __noinline__ void l_root_acc(const float* ms, float* sm, const LLane&
 // qdd -> qacc (no iterate yet) or qstar (trial point of the line search); rs = J a - aref of every row; returns "the sign pattern
 // of the rows equals the working set" for this lane's env.
 template <class C>
-__device__ __noinline__ bool l_sweep_acc(const float* ms, float* sm, const LLane& w, bool run, bool to_qstar) {
+__device__ __noinline__ bool l_sweep_acc(const float* ms, float* sm, const LLane& w_, bool run, bool to_qstar) {
+  L_LANE_BY_VALUE(C, w, w_);
   const LHdr& H = l_hdr<C>(ms);
   const LBody* MB = l_bodies(ms);
   S6 ca = s6(v3(0.f, 0.f, 0.f), v3(0.f, 0.f, 0.f));
@@ -1247,7 +1293,8 @@ __device__ __forceinline__ void l_solve_plan(const float* ms, const LLane& w, LS
 // op 3: take   (set unchanged at the trial point: r := rs, phi := -D rs on the set)        [fin with an iterate: bookkeeping only]
 // op 4: sums at al = 0 and at al = 1 in one pass: out = g1, g2, s1(0), s1(1), s2(1)   (start of the line search)
 template <class C>
-__device__ __noinline__ void l_rows(float* sm, const LLane& w, bool run, int op, float al, float* out4) {
+__device__ __noinline__ void l_rows(float* sm, const LLane& w_, bool run, int op, float al, float* out4) {
+  L_LANE_BY_VALUE(C, w, w_);
   float g1 = 0.f, g2 = 0.f, s1 = 0.f, s2 = 0.f, s10 = 0.f;
   if (op == 4) al = 1.f;
   if (run) {
@@ -1308,7 +1355,8 @@ __device__ int g_lstats[32];
 // the lanes: lane i of the env owns row i), (H + D^-1) lam = -r(0) is solved across the 8 lanes, and a last solve applies lam.
 // Returns "sign pattern of all rows == working set" at the resulting point.
 template <class C>
-__device__ __noinline__ bool l_linsolve(const float* ms, float* sm, const LLane& w, bool run, int inflags, bool to_qstar, bool first, LSolveLane& st) {
+__device__ __noinline__ bool l_linsolve(const float* ms, float* sm, const LLane& w_, bool run, int inflags, bool to_qstar, bool first, LSolveLane& st) {
+  L_LANE_BY_VALUE(C, w, w_);
   const LHdr& H = l_hdr<C>(ms);
   if (!C::SELFCOL) {   // no geom-geom rows compiled in: the plain ABA pair
     l_sweep_in<C, false>(ms, sm, w, run, inflags, st);
@@ -2302,7 +2350,8 @@ __global__ void __launch_bounds__(256, 1) k_kin5(const float* __restrict__ gimg,
 // outward: body accelerations a_b = a_parent + sum_k qacc_k S_k of the given qacc (the ABA's a, without the bias accelerations pb
 // carries), residuals rs = J a - aref of the body's rows, and the body's net inertial force I_b a_b + pb_b into its record's pb slot
 template <class C>
-__device__ __noinline__ void l_inv_acc(const float* ms, float* sm, const LLane& w) {
+__device__ __noinline__ void l_inv_acc(const float* ms, float* sm, const LLane& w_) {
+  L_LANE_BY_VALUE(C, w, w_);
   const LHdr& H = l_hdr<C>(ms);
   const LBody* MB = l_bodies(ms);
   const float* qa = sm + C::qacc;
@@ -2372,7 +2421,8 @@ __device__ __forceinline__ S6 l_inv_rows(const LHdr& H, float* sm, const LLane& 
 // bias-force words at junctions); tau_k = S_k^T F + armature_k qacc_k - sg f_lim per hinge, the root's six on lane 0.  The result goes to
 // the qvel row of shared memory (dead after S1), which the kernel then copies out.
 template <class C>
-__device__ __noinline__ void l_inv_force(const float* ms, float* sm, const LLane& w) {
+__device__ __noinline__ void l_inv_force(const float* ms, float* sm, const LLane& w_) {
+  L_LANE_BY_VALUE(C, w, w_);
   const LHdr& H = l_hdr<C>(ms);
   const LBody* MB = l_bodies(ms);
   const float* qa = sm + C::qacc;
@@ -2488,7 +2538,8 @@ __device__ __forceinline__ void l_add10(float* I, const float* p) {
 
 // inward: composite inertias -> f of every dof (l_dof_fp)
 template <class C>
-__device__ __noinline__ void l_crb_in(const float* ms, float* sm, const LLane& w) {
+__device__ __noinline__ void l_crb_in(const float* ms, float* sm, const LLane& w_) {
+  L_LANE_BY_VALUE(C, w, w_);
   const LHdr& H = l_hdr<C>(ms);
   const LBody* MB = l_bodies(ms);
   const bool stepbar = (H.align & 16) && w.bar;
@@ -2536,7 +2587,8 @@ __device__ __noinline__ void l_crb_in(const float* ms, float* sm, const LLane& w
 // the dense [nv, nv] block, row by row, the env's lanes over the columns.  Both halves come from one expression, S_lo . f_hi, at one
 // site (two sites could contract the cross products into FMAs differently), so M is symmetric bit for bit.
 template <class C>
-__device__ __noinline__ void l_write_M(const float* ms, float* sm, const LLane& w, float* __restrict__ out) {
+__device__ __noinline__ void l_write_M(const float* ms, float* sm, const LLane& w_, float* __restrict__ out) {
+  L_LANE_BY_VALUE(C, w, w_);
   const LHdr& H = l_hdr<C>(ms);
   const LBody* MB = l_bodies(ms);
   if (!w.live) return;
@@ -2556,7 +2608,8 @@ __device__ __noinline__ void l_write_M(const float* ms, float* sm, const LLane& 
 
 // the [6, nv] block of body p: rows 0-2 jacp (velocity of the body origin), 3-5 jacr; the env's lanes over the columns
 template <class C>
-__device__ __noinline__ void l_write_jac(const float* ms, const float* sm, const LLane& w, int p, float* __restrict__ o) {
+__device__ __noinline__ void l_write_jac(const float* ms, const float* sm, const LLane& w_, int p, float* __restrict__ o) {
+  L_LANE_BY_VALUE(C, w, w_);
   const LHdr& H = l_hdr<C>(ms);
   const LBody& lb = l_bodies(ms)[p];
   if (!w.live) return;
