@@ -173,11 +173,23 @@ typedef struct SmplsimAux {
                           * xfrc_applied) in com-based form about the root subtree COM, rotation first -- not checked against a wheel. */
 } SmplsimAux;
 
+/* A camera of smplsim_render.  Camera frame as in MJCF: the camera looks along its -z axis, +y is up, +x is right. */
+#define SMPLSIM_CAM_FIXED 0    /* world pose */
+#define SMPLSIM_CAM_TRACKCOM 1 /* world axes; position = the env's robot centre of mass + pos (MJCF mode="trackcom") */
+#define SMPLSIM_CAM_BODY 2     /* rides on robot body `body` */
+typedef struct SmplsimCamera {
+  int32_t mode, body, exclude_body, pad_;  /* body: BODY mode; exclude_body: -1 = none, else that body's geoms are not drawn */
+  float pos[3];   /* FIXED: world position | TRACKCOM: offset from the robot COM | BODY: position in the body frame */
+  float mat[9];   /* row-major; columns = camera x, y, z axes in the world (FIXED, TRACKCOM) or body (BODY) frame */
+  float fovy;     /* vertical field of view, degrees, in (0, 180) */
+  float zfar;     /* depth of pixels that hit nothing */
+} SmplsimCamera;
+
 typedef struct SmplsimHandle SmplsimHandle;
 
 const char* smplsim_last_error(void);
-int smplsim_version(void);   /* 240 = this header (230: before smplsim_dynamics; 220: before smplsim_inverse; 210: before SmplsimAux.contact_wrench; 200: before SmplsimState.xfrc_applied;
-                              * 100: before pid_* state and aux.status) */
+int smplsim_version(void);   /* 250 = this header (240: before smplsim_ray / smplsim_render; 230: before smplsim_dynamics; 220: before smplsim_inverse;
+                              * 210: before SmplsimAux.contact_wrench; 200: before SmplsimState.xfrc_applied; 100: before pid_* state and aux.status) */
 
 /* MjModel.from_xml_string + MjData + setup_humanoid_properties/setup_controller
  * (base_env.py:139-142, humanoid_env.py:262-323). */
@@ -248,6 +260,34 @@ int smplsim_inverse(SmplsimHandle* h, const float* qpos_dev, const float* qvel_d
  * [MJ-upstream] mj_fullM / mj_rne / mj_jacBody (engine_support.c, engine_core_smooth.c); not checked against a MuJoCo wheel. */
 int smplsim_dynamics(SmplsimHandle* h, const float* qpos_dev, const float* qvel_dev, int n, float* qM_dev, float* qfrc_bias_dev,
                      const int32_t* jac_body, int njac, float* jac_dev, void* cuda_stream);
+
+/* Ray casting and camera images of the robot geoms and the floor, on caller body poses xpos[n,nbody,3] / xquat[n,nbody,4] (the
+ * layout of SmplsimAux.xpos / xquat: the post-step poses a batch holds, smplsim_kinematics of any qpos, or motion-table rows).
+ * Quaternions are normalised in the kernel.  Geometry: spheres, capsules, boxes and the infinite floor plane in closed form, fp32;
+ * the smallest x >= 0 wins, so a ray that starts inside a geom hits it on the way out, and the floor is hit from its front side only;
+ * geom margins are ignored [MJ-upstream: mj_ray, engine_ray.c].  Neither call writes env state or handle scratch a later step reads.
+ * Single-shape handle: any n >= 0.  Per-env shapes: n == num_envs, row i uses env i's shape.  Every handle kind is supported.
+ *
+ * smplsim_ray (mujoco.mj_ray for every ray): pnt[n,nray,3], vec[n,nray,3] -> dist[n,nray] = x with the hit at pnt + x vec (vec need
+ * not be unit), geomid[n,nray] = MuJoCo geom id (0 floor, i + 1 robot geom i); -1 / -1: no hit (also for vec = 0).  flg_static = 0
+ * skips the floor; bodyexclude (-1 = none) skips every geom of that robot body.  Each output may be NULL.
+ *
+ * smplsim_render: one image per env from *cam (host struct).  Row 0 is the top of the image, pixel (r, c) is shot through its centre;
+ * fovy is vertical, the horizontal field follows from width / height.  Outputs, each NULL = skipped:
+ *   depth[n,height,width] float32  z-depth along the camera's viewing axis (metres, not ray length); cam->zfar where nothing is hit
+ *   seg[n,height,width]   int32    MuJoCo geom id (0 floor, i + 1 robot geom i), -1 none
+ *   rgb[n,height,width,3] uint8    c = clamp(a (0.1 + 0.4 max(0, -n.f) + max(0, -n.l) s), 0, 1), u8 = floor(255 c + 0.5): n the unit
+ *                                  normal facing the ray, f the camera's forward axis, l = (0, 0, -1), s = 0 when the ray from
+ *                                  p + 1e-4 n towards -l hits a robot geom; albedo a = geom_rgb (host [ngeom*3], NULL: 0.8 0.6 0.4)
+ *                                  for robot geoms, a 0 / 0.8 grey checker of edge 5/3 m on the floor; no hit: t (0.4, 0.5, 0.6),
+ *                                  t = (d_z + 1) / 2 of the unit ray direction.  Details: csrc/render_kernels.cuh.
+ * SMPLSIM_EINVAL: a bad body index (cam->body, cam->exclude_body, bodyexclude), an unknown cam->mode, fovy outside (0, 180),
+ * width / height / nray <= 0 with n > 0, or every output NULL with n > 0. */
+int smplsim_ray(SmplsimHandle* h, const float* xpos_dev, const float* xquat_dev, int n, int nray, const float* pnt_dev,
+                const float* vec_dev, int flg_static, int bodyexclude, float* dist_dev, int32_t* geomid_dev, void* cuda_stream);
+int smplsim_render(SmplsimHandle* h, const float* xpos_dev, const float* xquat_dev, int n, const SmplsimCamera* cam,
+                   int width, int height, const float* geom_rgb, float* depth_dev, int32_t* seg_dev, uint8_t* rgb_dev,
+                   void* cuda_stream);
 
 /* compute_humanoid_self_obs_v1 / _v2 (humanoid_env.py:565-688) on caller-supplied body states:
  * qvel[N,nv] (v1), xpos, xquat, linvel, angvel [N,nbody,*] -> obs[N,self_obs_dim]. */

@@ -42,6 +42,11 @@ class SmplsimAuxC(C.Structure):
     ]
 
 
+class SmplsimCameraC(C.Structure):
+    _fields_ = [("mode", C.c_int32), ("body", C.c_int32), ("exclude_body", C.c_int32), ("pad_", C.c_int32), ("pos", C.c_float * 3),
+                ("mat", C.c_float * 9), ("fovy", C.c_float), ("zfar", C.c_float)]
+
+
 def _get(node: Any, key: str, default=None):
     if hasattr(node, "get"):
         return node.get(key, default)

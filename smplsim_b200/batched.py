@@ -118,6 +118,7 @@ class HumanoidBatchB200:
         if self.contact_wrench is not None:
             self._aux.contact_wrench = self.contact_wrench.data_ptr()
         self._xfrc = None           # mj_data.xfrc_applied (None: no external wrench; see xfrc_applied)
+        self._cams = {}             # named cameras of render(), resolved once (a tracking camera's offset needs host kinematics)
         self.gpu_launches = 0
 
     def __del__(self):
@@ -317,6 +318,98 @@ class HumanoidBatchB200:
             self._check(self._L().smplsim_dynamics(self._h, _ptr(q), _ptr(v), n, _ptr(out.get("qM")), _ptr(out.get("qfrc_bias")),
                                                    C.c_void_p(jb.ctypes.data) if bodies else None, len(bodies),
                                                    _ptr(jac) if bodies else None, self._stream()))
+            self.gpu_launches += 1
+        return out
+
+    # ------------------------------------------------------------------ ray casting and cameras (mj_ray, mujoco.Renderer)
+    def _checked(self, name, t, shape):
+        """A caller tensor checked as xfrc_applied is: shape (None entries free), float32, this batch's device, contiguous."""
+        if not isinstance(t, torch.Tensor):
+            raise ValueError(f"{name} must be a torch.Tensor, got {type(t).__name__}")
+        if t.dim() != len(shape) or any(s is not None and t.shape[i] != s for i, s in enumerate(shape)):
+            want = "[" + ", ".join("n" if s is None else str(s) for s in shape) + "]"
+            raise ValueError(f"{name} must have shape {want}, got {tuple(t.shape)}")
+        if t.dtype != torch.float32:
+            raise ValueError(f"{name} must be float32, got {t.dtype}")
+        dv = self.device
+        if t.device.type != dv.type or (dv.index is not None and t.device.index != dv.index):
+            raise ValueError(f"{name} must live on {dv}, got {t.device}")
+        if not t.is_contiguous():
+            raise ValueError(f"{name} must be contiguous")
+        return t
+
+    def _poses(self, xpos, xquat):
+        """Body poses of the call: the batch's own post-step xpos / xquat by default."""
+        if (xpos is None) != (xquat is None):
+            raise ValueError("give both xpos and xquat, or neither (the batch's own poses)")
+        if xpos is None:
+            return self.xpos, self.xquat
+        nb = self.model.nbody
+        self._checked("xpos", xpos, (None, nb, 3))
+        self._checked("xquat", xquat, (xpos.shape[0], nb, 4))
+        return xpos, xquat
+
+    def ray(self, pnt: torch.Tensor, vec: torch.Tensor, xpos: Optional[torch.Tensor] = None, xquat: Optional[torch.Tensor] = None,
+            flg_static: bool = True, bodyexclude: int = -1):
+        """``mujoco.mj_ray`` for every ray of every row: ``pnt`` / ``vec`` ``[n, R, 3]`` against the robot geoms (and the floor with
+        ``flg_static``) posed by ``xpos [n, nbody, 3]`` / ``xquat [n, nbody, 4]`` (default: this batch's post-step poses).  Returns
+        ``dist [n, R]`` (the hit is at ``pnt + dist * vec``; vec need not be unit) and ``geomid [n, R]`` (0 floor, i + 1 robot geom i),
+        -1 / -1 for no hit.  ``bodyexclude`` (-1 none) skips that robot body's geoms.  Any n on a one-shape batch, n == num_envs with
+        per-env shapes.  Writes no env state."""
+        xpos, xquat = self._poses(xpos, xquat)
+        n = xpos.shape[0]
+        self._checked("pnt", pnt, (n, None, 3))
+        self._checked("vec", vec, (n, pnt.shape[1], 3))
+        R = pnt.shape[1]
+        dist = torch.empty(n, R, dtype=torch.float32, device=self.device)
+        gid = torch.empty(n, R, dtype=torch.int32, device=self.device)
+        if n and R:
+            self._check(self._L().smplsim_ray(self._h, _ptr(xpos), _ptr(xquat), n, R, _ptr(pnt), _ptr(vec), int(bool(flg_static)),
+                                              int(bodyexclude), _ptr(dist), _ptr(gid), self._stream()))
+            self.gpu_launches += 1
+        return {"dist": dist, "geomid": gid}
+
+    def render(self, camera: Any = "side", width: int = 320, height: int = 240, depth: bool = False, segmentation: bool = False,
+               rgb: bool = True, xpos: Optional[torch.Tensor] = None, xquat: Optional[torch.Tensor] = None,
+               geom_rgb: Optional[Sequence] = None):
+        """One image per row from ``camera`` (a name of ``smplsim_b200.camera``: ``"back"``, ``"side"``, ``"front_side"``, their ids
+        0-2, ``"egocentric"``; or a ``camera.Camera``) of the robot posed by ``xpos`` / ``xquat`` (default: this batch's post-step
+        poses).  Returns a dict with the outputs asked for: ``depth [n, H, W]`` float32 z-depth in metres (the camera's zfar where
+        nothing is hit), ``segmentation [n, H, W]`` int32 MuJoCo geom ids (0 floor, i + 1 robot geom i, -1 none), ``rgb [n, H, W, 3]``
+        uint8.  Row 0 is the top of the image.  ``geom_rgb``: ``[ngeom, 3]`` albedo of the robot geoms (default 0.8 0.6 0.4).  The
+        shading is this project's, stated in include/smplsim.h; it is not MuJoCo's OpenGL renderer.  Writes no env state."""
+        from . import camera as _cam
+        if isinstance(camera, (str, int, np.integer)) and not isinstance(camera, bool):
+            key = (type(camera).__name__, camera)
+            if key not in self._cams:
+                self._cams[key] = _cam.named(self.model, camera)
+            cam = self._cams[key]
+        else:
+            cam = _cam.named(self.model, camera)
+        xpos, xquat = self._poses(xpos, xquat)
+        n, f32 = xpos.shape[0], dict(device=self.device)
+        if int(width) <= 0 or int(height) <= 0:
+            raise ValueError(f"width and height must be positive, got {width} x {height}")
+        H, W = int(height), int(width)
+        out = {}
+        if depth:
+            out["depth"] = torch.empty(n, H, W, dtype=torch.float32, **f32)
+        if segmentation:
+            out["segmentation"] = torch.empty(n, H, W, dtype=torch.int32, **f32)
+        if rgb:
+            out["rgb"] = torch.empty(n, H, W, 3, dtype=torch.uint8, **f32)
+        if not out:
+            raise ValueError("render: ask for at least one of depth / segmentation / rgb")
+        tab = None
+        if geom_rgb is not None:
+            tab = np.ascontiguousarray(np.asarray(geom_rgb, dtype=np.float32))
+            if tab.shape != (self.model.ngeom, 3):
+                raise ValueError(f"geom_rgb must have shape ({self.model.ngeom}, 3), got {tab.shape}")
+        if n:
+            cs = cam.c_struct()
+            self._check(self._L().smplsim_render(self._h, _ptr(xpos), _ptr(xquat), n, C.byref(cs), W, H,
+                                                 C.c_void_p(tab.ctypes.data) if tab is not None else None, _ptr(out.get("depth")),
+                                                 _ptr(out.get("segmentation")), _ptr(out.get("rgb")), self._stream()))
             self.gpu_launches += 1
         return out
 

@@ -12,6 +12,7 @@
 #include <vector>
 
 #include "aux_kernels.cuh"
+#include "render_kernels.cuh"
 
 #ifdef SMPLSIM_EMU
 #define L_LAUNCH(kern, grid, block, smem, stream, ...) emu::launch(dim3(grid), dim3(block), smem, [&]() { kern(__VA_ARGS__); })
@@ -41,6 +42,7 @@ struct SmplsimHandle {
   int nmodels = 1, nblocks = 0;
   int* dslot_env = nullptr;     // [nblocks * warps per CTA * envs per warp] slot -> env (-1: none)
   int* dblk_img = nullptr;      // [nblocks] CTA -> table
+  int* denv_model = nullptr;    // [num_envs] env -> table (device copy of env_model; ray casting and rendering)
   LMap map() const { LMap m; m.slot_env = dslot_env; m.blk_img = dblk_img; return m; }
 };
 
@@ -59,7 +61,7 @@ struct DeviceGuard {   // every entry point runs on the handle's device and rest
 };
 
 extern "C" const char* smplsim_last_error(void) { return g_err.c_str(); }
-extern "C" int smplsim_version(void) { return 240; }   // 240: smplsim_dynamics; 230: smplsim_inverse; 220: SmplsimAux.contact_wrench; 210: SmplsimState.xfrc_applied; 200: lane-chain kernels (ABI structs of 110)
+extern "C" int smplsim_version(void) { return 250; }   // 250: smplsim_ray / smplsim_render; 240: smplsim_dynamics; 230: smplsim_inverse; 220: SmplsimAux.contact_wrench; 210: SmplsimState.xfrc_applied; 200: lane-chain kernels (ABI structs of 110)
 
 template <class C>
 static size_t cta_smem(const SmplsimHandle* h, int wpb) { return (size_t)h->img.hdr()->bytes + 16 + (size_t)wpb * C::EPW * C::total * 4; }
@@ -176,7 +178,7 @@ static void run_dynamics(SmplsimHandle* h, const LDynArgs& a, cudaStream_t st) {
   } while (0)
 
 static void free_handle(SmplsimHandle* h) {
-  cudaFree(h->dimg); cudaFree(h->gscr); cudaFree(h->gsens); cudaFree(h->gpfl); cudaFree(h->gbody); cudaFree(h->dslot_env); cudaFree(h->dblk_img);
+  cudaFree(h->dimg); cudaFree(h->gscr); cudaFree(h->gsens); cudaFree(h->gpfl); cudaFree(h->gbody); cudaFree(h->dslot_env); cudaFree(h->dblk_img); cudaFree(h->denv_model);
   delete h;
 }
 
@@ -265,6 +267,8 @@ static int create_impl(const SmplsimModelDesc* s, int nmodels, const int32_t* en
     if (e == cudaSuccess) e = cudaMemcpy(h->dslot_env, slot_env.data(), slot_env.size() * sizeof(int), cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaMalloc(&h->dblk_img, blk_img.size() * sizeof(int));
     if (e == cudaSuccess) e = cudaMemcpy(h->dblk_img, blk_img.data(), blk_img.size() * sizeof(int), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMalloc(&h->denv_model, (size_t)num_envs * sizeof(int));
+    if (e == cudaSuccess) e = cudaMemcpy(h->denv_model, h->env_model.data(), (size_t)num_envs * sizeof(int), cudaMemcpyHostToDevice);
   }
   if (e == cudaSuccess) e = cudaMalloc(&h->gscr, gs * (size_t)num_envs * 4 + 16);
   if (e == cudaSuccess) e = cudaMalloc(&h->gsens, (size_t)6 * H.nb * num_envs * 4);
@@ -421,6 +425,73 @@ extern "C" int smplsim_dynamics(SmplsimHandle* h, const float* qpos_dev, const f
   for (int j = 0; j < njac; j++) a.jb[j] = (unsigned char)jac_body[j];
   a.map = h->map();
   L_DISPATCH(h, run_dynamics<C_>(h, a, (cudaStream_t)stream));
+  CUDA_TRY(cudaGetLastError());
+  return SMPLSIM_OK;
+}
+
+// ray casting / rendering: the scene of n rows of body poses (render_kernels.cuh)
+static RScene render_scene(const SmplsimHandle* h, const float* xpos, const float* xquat) {
+  const LHdr& H = *h->img.hdr();
+  RScene s; std::memset(&s, 0, sizeof s);
+  s.gimg = h->dimg; s.env_img = h->denv_model; s.xpos = xpos; s.xquat = xquat;
+  s.img_words = H.bytes / 4; s.geom_off = H.geom_off; s.nb = H.nb; s.ng = H.ng;
+  // the plane's frame: x = world x projected on the plane (world y if the normal is along x), y = normal x x
+  double n[3] = {H.plane_n[0], H.plane_n[1], H.plane_n[2]}, u[3] = {1, 0, 0};
+  if (std::fabs(n[0]) > 0.9) { u[0] = 0; u[1] = 1; }
+  double d = u[0] * n[0] + u[1] * n[1] + u[2] * n[2];
+  for (int k = 0; k < 3; k++) u[k] -= d * n[k];
+  double un = std::sqrt(u[0] * u[0] + u[1] * u[1] + u[2] * u[2]);
+  for (int k = 0; k < 3; k++) u[k] /= un;
+  double v[3] = {n[1] * u[2] - n[2] * u[1], n[2] * u[0] - n[0] * u[2], n[0] * u[1] - n[1] * u[0]};
+  for (int k = 0; k < 3; k++) { s.p0[k] = H.plane_pos[k]; s.pn[k] = H.plane_n[k]; s.pu[k] = (float)u[k]; s.pv[k] = (float)v[k]; }
+  return s;
+}
+
+extern "C" int smplsim_ray(SmplsimHandle* h, const float* xpos_dev, const float* xquat_dev, int n, int nray, const float* pnt_dev,
+                           const float* vec_dev, int flg_static, int bodyexclude, float* dist_dev, int32_t* geomid_dev, void* stream) {
+  if (!h || n < 0) return fail(SMPLSIM_EINVAL, "smplsim_ray: null handle or n < 0");
+  const LHdr& H = *h->img.hdr();
+  if (bodyexclude < -1 || bodyexclude >= H.nb) return fail(SMPLSIM_EINVAL, "smplsim_ray: bodyexclude out of range [-1, nbody)");
+  if (n == 0) return SMPLSIM_OK;   // nothing is read: empty tensors may come as NULL
+  if (nray <= 0) return fail(SMPLSIM_EINVAL, "smplsim_ray: nray <= 0");
+  if (!dist_dev && !geomid_dev) return fail(SMPLSIM_EINVAL, "smplsim_ray: no output requested");
+  if (!xpos_dev || !xquat_dev || !pnt_dev || !vec_dev) return fail(SMPLSIM_EINVAL, "smplsim_ray: null argument");
+  if (h->nblocks && n != h->num_envs) return fail(SMPLSIM_EINVAL, "smplsim_ray: with per-env body shapes n must be the handle's num_envs (row i uses env i's shape)");
+  const long grid = (long)n * ((nray + R_THREADS - 1) / R_THREADS);
+  if (grid > 0x7fffffffL) return fail(SMPLSIM_EINVAL, "smplsim_ray: n x nray too large for one launch");
+  DeviceGuard guard(h->device);
+  RRayArgs a; std::memset(&a, 0, sizeof a);
+  a.s = render_scene(h, xpos_dev, xquat_dev);
+  a.pnt = pnt_dev; a.vec = vec_dev; a.dist = dist_dev; a.geomid = geomid_dev; a.nray = nray; a.flg_static = flg_static ? 1 : 0;
+  a.bodyexclude = bodyexclude;
+  L_LAUNCH(k_ray, (int)grid, R_THREADS, 0, (cudaStream_t)stream, a);
+  CUDA_TRY(cudaGetLastError());
+  return SMPLSIM_OK;
+}
+
+extern "C" int smplsim_render(SmplsimHandle* h, const float* xpos_dev, const float* xquat_dev, int n, const SmplsimCamera* cam, int width,
+                              int height, const float* geom_rgb, float* depth_dev, int32_t* seg_dev, uint8_t* rgb_dev, void* stream) {
+  if (!h || !cam || n < 0) return fail(SMPLSIM_EINVAL, "smplsim_render: null handle / camera or n < 0");
+  const LHdr& H = *h->img.hdr();
+  if (cam->mode < SMPLSIM_CAM_FIXED || cam->mode > SMPLSIM_CAM_BODY) return fail(SMPLSIM_EINVAL, "smplsim_render: unknown camera mode");
+  if (cam->mode == SMPLSIM_CAM_BODY && (cam->body < 0 || cam->body >= H.nb)) return fail(SMPLSIM_EINVAL, "smplsim_render: camera body out of range [0, nbody)");
+  if (cam->exclude_body < -1 || cam->exclude_body >= H.nb) return fail(SMPLSIM_EINVAL, "smplsim_render: exclude_body out of range [-1, nbody)");
+  if (!(cam->fovy > 0.f && cam->fovy < 180.f)) return fail(SMPLSIM_EINVAL, "smplsim_render: fovy outside (0, 180) degrees");
+  if (n == 0) return SMPLSIM_OK;
+  if (width <= 0 || height <= 0) return fail(SMPLSIM_EINVAL, "smplsim_render: width / height <= 0");
+  if (!depth_dev && !seg_dev && !rgb_dev) return fail(SMPLSIM_EINVAL, "smplsim_render: no output requested");
+  if (!xpos_dev || !xquat_dev) return fail(SMPLSIM_EINVAL, "smplsim_render: null xpos / xquat");
+  if (h->nblocks && n != h->num_envs) return fail(SMPLSIM_EINVAL, "smplsim_render: with per-env body shapes n must be the handle's num_envs (row i uses env i's shape)");
+  const int tiles_x = (width + R_CTA_W - 1) / R_CTA_W, tiles = tiles_x * ((height + R_CTA_H - 1) / R_CTA_H);
+  if ((long)n * tiles > 0x7fffffffL) return fail(SMPLSIM_EINVAL, "smplsim_render: n x image too large for one launch");
+  DeviceGuard guard(h->device);
+  RRenderArgs a; std::memset(&a, 0, sizeof a);
+  a.s = render_scene(h, xpos_dev, xquat_dev);
+  a.cam = *cam;
+  a.depth = depth_dev; a.seg = seg_dev; a.rgb = rgb_dev; a.W = width; a.H = height; a.tiles_x = tiles_x; a.tiles = tiles;
+  for (int g = 0; g < H.ng; g++)
+    for (int k = 0; k < 3; k++) a.rgb_tab[3 * g + k] = geom_rgb ? geom_rgb[3 * g + k] : (k == 0 ? 0.8f : k == 1 ? 0.6f : 0.4f);   // <default> rgba of the MJCFs
+  L_LAUNCH(k_render, n * tiles, R_THREADS, 0, (cudaStream_t)stream, a);
   CUDA_TRY(cudaGetLastError());
   return SMPLSIM_OK;
 }

@@ -206,8 +206,15 @@ class HumanoidEnvB200(_EnvBase):
         info["critic_state"] = obs
         return obs, float(rew[0].item()), died, timed_out, info
 
-    def render(self):        # called every step by worker 0 even when headless (agent.py:96-97): cheap no-op
-        return None
+    def render(self):
+        """``render_mode == "rgb_array"`` and not ``headless``: the ``[240, 320, 3]`` uint8 frame of ``cfg.env.camera`` (a name of
+        ``smplsim_b200.camera`` or a MuJoCo camera id 0-2: back, side, front_side) at the current state -- mujoco.Renderer's default
+        size (base_env.py:159-162).  Every other configuration returns None: worker 0 calls this every step even when headless
+        (agent.py:96-97)."""
+        if self.render_mode != "rgb_array" or self.headless:
+            return None
+        frame = self._b.render(camera=self.cfg.env.camera, width=320, height=240)["rgb"]
+        return frame[0].cpu().numpy()
 
     def close(self):
         pass

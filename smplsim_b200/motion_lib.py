@@ -145,6 +145,19 @@ class MotionLibB200:
         qacc = (qvel[hi] - qvel[lo]) / self._motion_dt[clip][:, None]
         return self.env.inverse(qpos, qvel, qacc, contact_wrench=contact_wrench)
 
+    def render_clip(self, motion_id: int, camera="side", width: int = 320, height: int = 240, **kw):
+        """``env.render`` of every frame of clip ``motion_id`` from the library's ``xpos`` / ``xquat`` tables: ``rgb [F, H, W, 3]``
+        uint8 (F = the clip's frame count).  Further keywords go to ``render`` (``geom_rgb``).  Needs a one-shape batch."""
+        K = self.num_motions()
+        if not 0 <= int(motion_id) < K:
+            raise ValueError(f"motion_id must be in [0, {K}), got {motion_id}")
+        s = int(self.length_starts[int(motion_id)].item())
+        f = int(self._motion_num_frames[int(motion_id)].item())
+        nb = self.env.model.nbody
+        xpos = self.tables["xpos"][s:s + f].view(f, nb, 3)
+        xquat = self.tables["xquat"][s:s + f].view(f, nb, 4)
+        return self.env.render(camera=camera, width=width, height=height, xpos=xpos, xquat=xquat, **kw)["rgb"]
+
     # ------------------------------------------------------------------ sampling (motion_lib_base.py:231-312), on the device
     def _uniform(self):
         K = self._num_unique_motions
