@@ -188,7 +188,7 @@ typedef struct SmplsimCamera {
 typedef struct SmplsimHandle SmplsimHandle;
 
 const char* smplsim_last_error(void);
-int smplsim_version(void);   /* 250 = this header (240: before smplsim_ray / smplsim_render; 230: before smplsim_dynamics; 220: before smplsim_inverse;
+int smplsim_version(void);   /* 260 = this header (250: before smplsim_set_env_params; 240: before smplsim_ray / smplsim_render; 230: before smplsim_dynamics; 220: before smplsim_inverse;
                               * 210: before SmplsimAux.contact_wrench; 200: before SmplsimState.xfrc_applied; 100: before pid_* state and aux.status) */
 
 /* MjModel.from_xml_string + MjData + setup_humanoid_properties/setup_controller
@@ -288,6 +288,43 @@ int smplsim_ray(SmplsimHandle* h, const float* xpos_dev, const float* xquat_dev,
 int smplsim_render(SmplsimHandle* h, const float* xpos_dev, const float* xquat_dev, int n, const SmplsimCamera* cam,
                    int width, int height, const float* geom_rgb, float* depth_dev, int32_t* seg_dev, uint8_t* rgb_dev,
                    void* cuda_stream);
+
+/* Per-env physics parameters (domain randomization).  Env e is simulated exactly as the handle's model (env e's shape on a per-env-shapes
+ * handle) with these fields replaced -- MuJoCo's behaviour when MjModel fields are edited in place without mj_setConst:
+ *   friction[N]            sliding friction mu (friction[0]) of every floor and geom-geom contact: pyramid directions n +- mu t and the
+ *                          rows' R / D (the impratio scaling);
+ *   gravity[N,3]           opt.gravity;
+ *   kp, kd, torque_limit [N,nu]   act_kp / act_kd / act_torque_lim, the values the configured controller reads (stable PD: torque and
+ *                          the (M + h kd) system, quirk Q1 with the env's own kd and masses on both sides; pd; simple_pid: gains and the
+ *                          clamp of the torque and of the integral; torque: the clamp only, act_scale stays the model's);
+ *   body_mass_scale[N,nbody]      body b's mass AND rotational inertia times s_b; its centre of mass does not move.
+ * body_invweight0 / dof_invweight0, and with them the constraint regularisation, keep the nominal model's values (mj_setConst is
+ * not rerun).  Every field is a device pointer to a full [N, ...] float32 array, or NULL. */
+typedef struct SmplsimEnvParams {
+  const float* friction;
+  const float* gravity;
+  const float* kp;
+  const float* kd;
+  const float* torque_limit;
+  const float* body_mass_scale;
+} SmplsimEnvParams;
+/* smplsim_set_env_params: for the envs whose mask byte is non-zero (mask_dev NULL: all), each non-NULL field of *p overwrites that
+ * parameter in the handle's per-env records; a NULL field keeps the current value.  The first call allocates the records (one per env,
+ * [mu | g 3 | kp nu | kd nu | torque_limit nu | mass_scale nbody] padded to 16 bytes: 944 B for SMPL) and fills them with the model's
+ * values, in stream order on cuda_stream; launches on other streams must be ordered after it by the caller.  Every call runs
+ * asynchronously on the stream.  Nothing the caller passes is kept
+ * after the call returns; the values are not checked (finite, mu >= 1e-5, gains >= 0, limits and scales > 0 is the caller's part).
+ * While records exist, smplsim_step, smplsim_mj_step, smplsim_reset (its Fall init runs substeps), smplsim_inverse, smplsim_dynamics
+ * and smplsim_render (TRACKCOM) use them; inverse and dynamics then need n == num_envs (row i uses env i's parameters), else
+ * SMPLSIM_EINVAL.  kinematics, ray, self_obs, motion_gather and gae do not depend on them.  Without records every call runs exactly
+ * as before (the same kernels).
+ * smplsim_get_env_params: copies the current values into the non-NULL fields of *out ([N, ...] device arrays), the model's values
+ * when no records exist.  smplsim_clear_env_params: synchronizes with the device and frees the records; the handle is again exactly
+ * what it was before the first set. */
+int smplsim_set_env_params(SmplsimHandle* h, const SmplsimEnvParams* p, const uint8_t* mask_dev, void* cuda_stream);
+int smplsim_get_env_params(SmplsimHandle* h, float* friction_dev, float* gravity_dev, float* kp_dev, float* kd_dev,
+                           float* torque_limit_dev, float* body_mass_scale_dev, void* cuda_stream);
+int smplsim_clear_env_params(SmplsimHandle* h);
 
 /* compute_humanoid_self_obs_v1 / _v2 (humanoid_env.py:565-688) on caller-supplied body states:
  * qvel[N,nv] (v1), xpos, xquat, linvel, angvel [N,nbody,*] -> obs[N,self_obs_dim]. */

@@ -47,6 +47,11 @@ class SmplsimCameraC(C.Structure):
                 ("mat", C.c_float * 9), ("fovy", C.c_float), ("zfar", C.c_float)]
 
 
+class SmplsimEnvParamsC(C.Structure):
+    _fields_ = [("friction", C.c_void_p), ("gravity", C.c_void_p), ("kp", C.c_void_p), ("kd", C.c_void_p), ("torque_limit", C.c_void_p),
+                ("body_mass_scale", C.c_void_p)]
+
+
 def _get(node: Any, key: str, default=None):
     if hasattr(node, "get"):
         return node.get(key, default)

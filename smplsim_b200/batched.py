@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .abi import SmplsimAuxC, SmplsimStateC, env_cfg_from, model_from_cfg
+from .abi import SmplsimAuxC, SmplsimEnvParamsC, SmplsimStateC, env_cfg_from, model_from_cfg
 from .model import ModelDesc
 
 
@@ -221,6 +221,98 @@ class HumanoidBatchB200:
         """The wrench pointer of this call (NULL: none); the tensor is kept referenced until the next call."""
         self._state.xfrc_applied = None if self._xfrc is None else self._xfrc.data_ptr()
         self._keep_xfrc = self._xfrc
+
+    # ------------------------------------------------------------------ per-env physics parameters (domain randomization)
+    ENV_PARAMS = ("friction", "gravity", "kp", "kd", "torque_limit", "body_mass_scale")
+
+    def _env_param_shapes(self):
+        m, N = self.model, self.num_envs
+        return {"friction": (N,), "gravity": (N, 3), "kp": (N, m.nu), "kd": (N, m.nu), "torque_limit": (N, m.nu),
+                "body_mass_scale": (N, m.nbody)}
+
+    def set_env_params(self, env_ids: Optional[torch.Tensor] = None, *, friction: Optional[torch.Tensor] = None,
+                       gravity: Optional[torch.Tensor] = None, kp: Optional[torch.Tensor] = None, kd: Optional[torch.Tensor] = None,
+                       torque_limit: Optional[torch.Tensor] = None, body_mass_scale: Optional[torch.Tensor] = None):
+        """Per-env physics parameters for domain randomization.  For the envs in ``env_ids`` (None = all; an index tensor or a
+        bool/uint8 mask, as in ``reset``) each given value replaces that env's parameter; a parameter left None keeps its current value.
+        Env ``e`` is then simulated as the model (its own shape with per-env shapes) with these fields replaced, as MuJoCo does when
+        ``MjModel`` fields are edited in place without ``mj_setConst``:
+
+        - ``friction [N]``: sliding friction of every floor and geom-geom contact;
+        - ``gravity [N, 3]``;
+        - ``kp``, ``kd``, ``torque_limit [N, nu]``: the gains and torque limits the configured controller reads (``model.act_kp`` /
+          ``act_kd`` / ``act_torque_lim``; in torque mode only the clamp);
+        - ``body_mass_scale [N, nbody]``: each body's mass and rotational inertia times the scale; its centre of mass stays.
+
+        The invweight0 values, and with them the constraint regularisation, stay the nominal model's.  Values are full
+        ``[num_envs, ...]`` float32 tensors on this batch's device; rows outside ``env_ids`` are ignored.  Raises ``ValueError`` for a
+        wrong shape, dtype or device, non-finite values, ``friction < 1e-5``, ``kp`` or ``kd < 0``, ``torque_limit <= 0`` or
+        ``body_mass_scale <= 0`` in the selected rows.  Checking the values costs one host sync: call this at reset time, not every
+        step.  ``step``, ``mj_step``, ``reset``, ``inverse``, ``dynamics`` and ``render`` (TRACKCOM) use the values from the next call on;
+        ``inverse`` and ``dynamics`` then take ``n == num_envs`` rows (row i = env i).  ``clear_env_params`` goes back to the model."""
+        vals = {"friction": friction, "gravity": gravity, "kp": kp, "kd": kd, "torque_limit": torque_limit, "body_mass_scale": body_mass_scale}
+        shapes, dv = self._env_param_shapes(), self.device
+        given = {}
+        for name, t in vals.items():
+            if t is None:
+                continue
+            if not isinstance(t, torch.Tensor):
+                raise ValueError(f"{name} must be a torch.Tensor, got {type(t).__name__}")
+            if tuple(t.shape) != shapes[name]:
+                raise ValueError(f"{name} must have shape {shapes[name]}, got {tuple(t.shape)}")
+            if t.dtype != torch.float32:
+                raise ValueError(f"{name} must be float32, got {t.dtype}")
+            if t.device.type != dv.type or (dv.index is not None and t.device.index != dv.index):
+                raise ValueError(f"{name} must live on {dv}, got {t.device}")
+            given[name] = t.contiguous()
+        mask = None
+        if env_ids is not None:
+            if env_ids.dtype in (torch.bool, torch.uint8) and env_ids.numel() == self.num_envs:
+                mask = env_ids.to(dv, torch.uint8).contiguous()
+            else:
+                if env_ids.numel() == 0:
+                    return
+                mask = torch.zeros(self.num_envs, dtype=torch.uint8, device=dv)
+                mask[env_ids.to(dv).long()] = 1
+        if not given:
+            return
+        sel = None if mask is None else mask.bool()
+        bad = []
+        for name, x in given.items():   # elementwise on the device; the one host sync is the .cpu() below
+            b = ~torch.isfinite(x)
+            if name == "friction":
+                b = b | (x < 1e-5)
+            elif name in ("kp", "kd"):
+                b = b | (x < 0)
+            elif name in ("torque_limit", "body_mass_scale"):
+                b = b | (x <= 0)
+            if sel is not None:
+                b = b & sel.view((-1,) + (1,) * (b.dim() - 1))
+            bad.append(b.any())
+        flags = torch.stack(bad).cpu().tolist()
+        rules = {"friction": "finite and >= 1e-5", "gravity": "finite", "kp": "finite and >= 0", "kd": "finite and >= 0",
+                 "torque_limit": "finite and > 0", "body_mass_scale": "finite and > 0"}
+        for name, f in zip(given, flags):
+            if f:
+                raise ValueError(f"{name} must be {rules[name]} in the selected envs")
+        p = SmplsimEnvParamsC(**{k: v.data_ptr() for k, v in given.items()})
+        self._check(self._L().smplsim_set_env_params(self._h, C.byref(p), _ptr(mask), self._stream()))
+        self.gpu_launches += 1
+        self._keep_prm = (mask, given)
+
+    @property
+    def env_params(self) -> dict:
+        """The current per-env parameters as a dict of new ``[num_envs, ...]`` float32 tensors (keys as ``set_env_params`` takes them);
+        the model's values (each env's shape) where nothing has been set."""
+        out = {k: torch.empty(s, dtype=torch.float32, device=self.device) for k, s in self._env_param_shapes().items()}
+        self._check(self._L().smplsim_get_env_params(self._h, *[_ptr(out[k]) for k in self.ENV_PARAMS], self._stream()))
+        self.gpu_launches += 1
+        return out
+
+    def clear_env_params(self):
+        """Drop every per-env parameter: the batch simulates the model again, exactly as before the first ``set_env_params``
+        (synchronizes with the device)."""
+        self._check(self._L().smplsim_clear_env_params(self._h))
 
     # ------------------------------------------------------------------ raw physics / kinematics (parity + tools)
     def mj_step(self, ctrl: torch.Tensor, nsub: int = 1):

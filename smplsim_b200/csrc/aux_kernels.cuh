@@ -100,3 +100,65 @@ __global__ void k_gae(const float* __restrict__ rew, const float* __restrict__ n
     prev_v = v; prev_a = a;
   }
 }
+
+// ------------------------------------------------------------------ per-env parameter records (smplsim_set_env_params / _get_env_params)
+// One record of w words per env: [mu | gravity 3 | kp nu | kd nu | torque limit nu | mass scale nb | pad] (LCfg::PRM_*).  One thread per
+// word.  set: rec NULL is not allowed; init = 1 first fills every env's record with its table's values (env_img: env -> table, NULL: one
+// table), then the envs whose mask byte is set (mask NULL: all) take each non-NULL field.  get: rec NULL reads the tables' values.
+struct PrmArgs {
+  float* rec;
+  const float* gimg;       // the handle's tables, img_words floats each
+  const int* env_img;
+  const uint8_t* mask;
+  const float* f[6];       // mu [N], gravity [N,3], kp / kd / torque limit [N,nu], mass scale [N,nb]
+  float* o[6];             // (get) the same layout
+  int img_words, n, nu, nb, w, init;
+};
+// field of word j and its column (-1: padding)
+__device__ __forceinline__ int prm_field(const PrmArgs& a, int j, int* col) {
+  const int kp = 4, kd = kp + a.nu, tl = kd + a.nu, ms = tl + a.nu;
+  if (j == 0) { *col = 0; return 0; }
+  if (j < kp) { *col = j - 1; return 1; }
+  if (j < kd) { *col = j - kp; return 2; }
+  if (j < tl) { *col = j - kd; return 3; }
+  if (j < ms) { *col = j - tl; return 4; }
+  if (j < ms + a.nb) { *col = j - ms; return 5; }
+  *col = 0;
+  return -1;
+}
+__device__ __forceinline__ float prm_nominal(const PrmArgs& a, int e, int fld, int col) {
+  const float* img = a.gimg + (size_t)(a.env_img ? a.env_img[e] : 0) * (size_t)a.img_words;
+  const LHdr& H = *(const LHdr*)img;
+  const LBody* B = (const LBody*)((const char*)img + LM_BODY_OFF);
+  switch (fld) {
+    case 0: return H.mu;
+    case 1: return H.grav[col];
+    case 2: return B[1 + col / 3].kp[col % 3];
+    case 3: return B[1 + col / 3].kd[col % 3];
+    case 4: return B[1 + col / 3].tlim[col % 3];
+    case 5: return 1.0f;
+    default: return 0.f;
+  }
+}
+__device__ __forceinline__ int prm_width(const PrmArgs& a, int fld) { return fld == 0 ? 1 : fld == 1 ? 3 : fld == 5 ? a.nb : a.nu; }
+
+__global__ void k_prm_set(PrmArgs a) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long)a.n * a.w) return;
+  const int e = (int)(i / a.w), j = (int)(i % a.w);
+  int col;
+  const int fld = prm_field(a, j, &col);
+  float v = a.init ? prm_nominal(a, e, fld, col) : a.rec[i];
+  if (fld >= 0 && a.f[fld] && (!a.mask || a.mask[e])) v = a.f[fld][(size_t)e * prm_width(a, fld) + col];
+  a.rec[i] = v;
+}
+
+__global__ void k_prm_get(PrmArgs a) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long)a.n * a.w) return;
+  const int e = (int)(i / a.w), j = (int)(i % a.w);
+  int col;
+  const int fld = prm_field(a, j, &col);
+  if (fld < 0 || !a.o[fld]) return;
+  a.o[fld][(size_t)e * prm_width(a, fld) + col] = a.rec ? a.rec[i] : prm_nominal(a, e, fld, col);
+}

@@ -41,14 +41,20 @@
 #define L_ST_SELF_CONTACT 32 // SMPLSIM_STATUS_SELF_CONTACT: a geom pair MuJoCo would collide touches (not simulated)
 
 // ------------------------------------------------------------------ compile-time sizes / per-env shared-memory layout (words)
-template <int NB_, int NV_, int NG_, int NS_, int NMBI_, int NMBO_, int NCS_, int NLS_, int SELFCOL_ = 0, int XFRC_ = 0>
+template <int NB_, int NV_, int NG_, int NS_, int NMBI_, int NMBO_, int NCS_, int NLS_, int SELFCOL_ = 0, int XFRC_ = 0, int PRM_ = 0>
 struct LCfg {
   static constexpr int NB = NB_, NV = NV_, NQ = NV_ + 1, NU = NV_ - 6, NG = NG_, NS = NS_, NMBI = NMBI_, NMBO = NMBO_, NCS = NCS_, NLS = NLS_;
   static constexpr int SELFCOL = SELFCOL_, LPE = LM_LPE, EPW = 32 / LM_LPE;   // SELFCOL: geom-geom (two-body) rows compiled in
   static constexpr int XFRC = XFRC_;   // external body wrenches (SmplsimState.xfrc_applied) compiled in; same layout as without
+  static constexpr int PRM = PRM_;     // per-env physics parameters (smplsim_set_env_params records) compiled in; same layout as without
   typedef LCfg<NB_, NV_, NG_, NS_, NMBI_, NMBO_, NCS_, NLS_, SELFCOL_, 1> WithXfrc;
+  typedef LCfg<NB_, NV_, NG_, NS_, NMBI_, NMBO_, NCS_, NLS_, SELFCOL_, 0, 1> WithPrm;        // reset, inverse, dynamics
+  typedef LCfg<NB_, NV_, NG_, NS_, NMBI_, NMBO_, NCS_, NLS_, SELFCOL_, 1, 1> WithXfrcPrm;    // step: one instance for records with or without a wrench
   static constexpr int BODYW = 24, MBIW = 28, MBOW = 32, CONW = 24, LIMW = 8, RECW = 28, ROOTW = 44;
   static constexpr int r4(int n) { return (n + 3) & ~3; }
+  // per-env parameter record (words; 16-byte rows in global memory, L2-resident): [mu | gravity 3 | kp NU | kd NU | torque limit NU |
+  // mass scale NB | pad]
+  static constexpr int PRM_MU = 0, PRM_G = 1, PRM_KP = 4, PRM_KD = PRM_KP + NU, PRM_TL = PRM_KD + NU, PRM_MS = PRM_TL + NU, PRMW = r4(PRM_MS + NB);
   static constexpr int qpos = 0, qvel = qpos + r4(NQ), qacc = qvel + r4(NV), act = qacc + r4(NV), tau = act + r4(NU),
                        body = tau + r4(NU), mbi = body + BODYW * NB, mbo = mbi + MBIW * NMBI, root = mbo + MBOW * NMBO, con = root + ROOTW,
                        lim = con + CONW * NCS, pfl = lim + LIMW * NLS, PFLW = r4((NS + 3) / 4), misc = pfl + PFLW, tsk = misc + 8,
@@ -136,6 +142,41 @@ template <class C> __device__ __forceinline__ const LHdr& l_hdr(const float* ms)
 __device__ __forceinline__ const LBody* l_bodies(const float* ms) { return (const LBody*)((const char*)ms + LM_BODY_OFF); }
 __device__ __forceinline__ const LGeom* l_geoms(const float* ms) { return (const LGeom*)((const char*)ms + ((const LHdr*)ms)->geom_off); }
 
+// Per-env physics parameters.  The PRM instances read friction, gravity, the controller gains / torque limits and the body mass scales
+// from this env's record (LCfg::PRM_*); every other instance reads the table, and for it these accessors are the table reads they
+// replace, at the same places.  The kernel prologue (l_prm_stage) parks the record's address and the env's friction in spare task words
+// of the env's shared-memory row, so no accessor needs the lane's env index or a header load: friction is a shared-memory read like
+// the table's, and the sweeps fetch a body's gains and mass scale at the top of each sweep step, next to its lane record, off the
+// chain that consumes them.  Indexed by actuator i (= dof - 6).
+#define L_TSK_PRM 8   // (PRM instances) task words 8, 9: this env's parameter record (8-byte address); word 10: its friction
+#define L_TSK_MU 10
+template <class C> __device__ __forceinline__ const float* l_prm(const float* sm) { return *(const float* const*)(sm + C::tsk + L_TSK_PRM); }
+template <class C> __device__ __forceinline__ float l_mu(const LHdr& H, const float* sm) {
+  if constexpr (C::PRM) return sm[C::tsk + L_TSK_MU];
+  else return H.mu;
+}
+template <class C> __device__ __forceinline__ V3 l_grav(const float* sm) {   // PRM instances only
+  const float* g = l_prm<C>(sm) + C::PRM_G;
+  return v3(__ldg(g), __ldg(g + 1), __ldg(g + 2));
+}
+template <class C> __device__ __forceinline__ float l_kp(const float* sm, const LBody& lb, int i, int k) {
+  if constexpr (C::PRM) return __ldg(l_prm<C>(sm) + C::PRM_KP + i);
+  else return lb.kp[k];
+}
+template <class C> __device__ __forceinline__ float l_kd(const float* sm, const LBody& lb, int i, int k) {
+  if constexpr (C::PRM) return __ldg(l_prm<C>(sm) + C::PRM_KD + i);
+  else return lb.kd[k];
+}
+template <class C> __device__ __forceinline__ float l_tlim(const float* sm, const LBody& lb, int i, int k) {
+  if constexpr (C::PRM) return __ldg(l_prm<C>(sm) + C::PRM_TL + i);
+  else return lb.tlim[k];
+}
+// (PRM) the three hinges' values of body b (b < 1: body 1's, ignored) from record word w0 (PRM_KP, PRM_KD or PRM_TL)
+template <class C> __device__ __forceinline__ void l_prm_ld3(const float* sm, int w0, int b, float* o) {
+  const float* r = l_prm<C>(sm) + w0 + 3 * ((b < 1 ? 1 : b) - 1);
+  o[0] = __ldg(r); o[1] = __ldg(r + 1); o[2] = __ldg(r + 2);
+}
+
 __device__ __forceinline__ float l_gsum(float v) {
 #pragma unroll
   for (int o = LM_LPE / 2; o > 0; o >>= 1) v += __shfl_xor_sync(L_FULL, v, o);
@@ -183,9 +224,10 @@ __device__ __forceinline__ S6 l_wrench(const LHdr& H, V3 cp, V3 t1, int k) {
 
 // direction of pyramid row k in the contact frame (n, t1, t2 = n x t1): n +- mu t1 | n +- mu t2.  The row's unit wrench about the
 // root origin is x_k = [cp x d_k ; d_k], so sums over rows factor through 3-vectors: sum D x x^T = X G X^T with G = D sum d d^T
-__device__ __forceinline__ V3 l_pyr_dir(const LHdr& H, V3 n, V3 t1, V3 t2, int k) {
+// mu: the env's sliding friction (l_mu)
+__device__ __forceinline__ V3 l_pyr_dir(float mu, V3 n, V3 t1, V3 t2, int k) {
   V3 t = (k < 2) ? t1 : t2;
-  float sg = (k & 1) ? -H.mu : H.mu;
+  float sg = (k & 1) ? -mu : mu;
   return n + sg * t;
 }
 
@@ -414,7 +456,7 @@ __device__ __forceinline__ bool l_rows_eval(const LHdr& H, float* sm, const LLan
     float rs[4];
 #pragma unroll
     for (int k = 0; k < 4; k++) {
-      rs[k] = dot(l_pyr_dir(H, n, t1, t2, k), ac) - e[8 + k];
+      rs[k] = dot(l_pyr_dir(l_mu<C>(H, sm), n, t1, t2, k), ac) - e[8 + k];
       if (rs[k] < 0.f) nf |= 2 << k;
     }
     if (c < C::NCS) ((float4*)(sm + C::con + C::CONW * c))[LCE_RS / 4] = make_float4(rs[0], rs[1], rs[2], rs[3]);
@@ -426,11 +468,15 @@ __device__ __forceinline__ bool l_rows_eval(const LHdr& H, float* sm, const LLan
 
 // rigid inertia, bias force, sensors, xquat of the body whose pose is P; returns pb
 template <class C>
-__device__ __forceinline__ S6 l_body_post(const LBody& lb, float* sm, const LLane& w, int b, int flags, const LPose& P, float* br, int ci) {
+__device__ __forceinline__ S6 l_body_post(float msc, const LBody& lb, float* sm, const LLane& w, int b, int flags, const LPose& P, float* br, int ci) {
   S6 pbv = s6(v3(0.f, 0.f, 0.f), v3(0.f, 0.f, 0.f));
   if (flags & LF_VEL) {
     float t[12];
     l_rigid10(lb, P.q, P.x, t);
+    if constexpr (C::PRM) {   // mass and rotational inertia times the env's scale msc, centre of mass unchanged: the whole row scales
+#pragma unroll
+      for (int j = 0; j < 10; j++) t[j] *= msc;
+    }
     t[10] = __int_as_float(ci); t[11] = 0.f;
     l_st12(br + LBR_R10, t);
     pbv = rb_mul(t, P.ab) + cross_force(P.v, rb_mul(t, P.v));
@@ -499,9 +545,9 @@ __device__ __forceinline__ int l_narrow(const LHdr& H, const LGeom& G, int g, co
       if (dist > H.margin) continue;
       cp = X.c + sg * X.ax - (G.size[0] + 0.5f * dist) * pn;
     }
-    float pm = dist - H.margin, imp = l_impedance(H, pm);
-    float R0 = fmaxf((1.f - imp) / imp * (tiw0 + H.mu * H.mu * tiw0), 1e-15f);
-    float R1 = R0 / fmaxf(H.impratio, 1e-15f), mu = H.mu * sqrtf(R1 / R0);
+    float pm = dist - H.margin, imp = l_impedance(H, pm), mu0 = l_mu<C>(H, sm);
+    float R0 = fmaxf((1.f - imp) / imp * (tiw0 + mu0 * mu0 * tiw0), 1e-15f);
+    float R1 = R0 / fmaxf(H.impratio, 1e-15f), mu = mu0 * sqrtf(R1 / R0);
     float kterm = H.K * imp * pm;
     // working set inherited from the slot's previous substep; a new contact starts from the rows that would be violated if the
     // body kept the acceleration it had in the previous substep
@@ -514,7 +560,7 @@ __device__ __forceinline__ int l_narrow(const LHdr& H, const LGeom& G, int g, co
       const V3 vc = vb.l + cross(vb.a, cp), pc = pa.l + cross(pa.a, cp);   // velocity / previous acceleration of the contact point
 #pragma unroll
       for (int k = 0; k < 4; k++) {
-        V3 d = l_pyr_dir(H, pn, t1, t2, k);
+        V3 d = l_pyr_dir(l_mu<C>(H, sm), pn, t1, t2, k);
         e[8 + k] = -H.B * dot(d, vc) - kterm;
         if (dot(d, pc) - e[8 + k] < 0.f) guess |= 2 << k;
       }
@@ -570,14 +616,15 @@ __device__ __noinline__ LRootOut l_root_out(const float* ms, float* sm, const LL
       if (flags & LF_VEL) {
         V3 vl = ld3(qvel), wv = qvel[3] * c0 + qvel[4] * c1 + qvel[5] * c2;
         P.v = s6(wv, vl);
-        P.ab = s6(v3(0.f, 0.f, 0.f), v3(-H.grav[0], -H.grav[1], -H.grav[2]) + cross(vl, wv));
+        if constexpr (C::PRM) { const V3 g = l_grav<C>(sm); P.ab = s6(v3(0.f, 0.f, 0.f), v3(-g.x, -g.y, -g.z) + cross(vl, wv)); }
+        else P.ab = s6(v3(0.f, 0.f, 0.f), v3(-H.grav[0], -H.grav[1], -H.grav[2]) + cross(vl, wv));   // (this form keeps the instance's SASS)
         const float* qa = sm + C::qacc;   // acceleration of the previous substep (qacc_warmstart), new rotation columns
         P.pa = s6(qa[3] * c0 + qa[4] * c1 + qa[5] * c2, ld3(qa));
       }
       l_mbo_put_pose(mo, P);
       LGeomCtx X;
       if ((flags & LF_COLLIDE) && lb.ngeom > 0) alloc = l_broad(H, l_geoms(ms)[lb.geom0], P, h0, X);
-      pbv = l_body_post<C>(lb, sm, w, 0, flags, P, br, alloc << 8);
+      pbv = l_body_post<C>(C::PRM ? __ldg(l_prm<C>(sm) + C::PRM_MS) : 1.f, lb, sm, w, 0, flags, P, br, alloc << 8);
       if (alloc) {
         int cnt = l_narrow<C>(H, l_geoms(ms)[lb.geom0], lb.geom0, X, P.v, P.pa, lb.tiw0, sm, w, 0, alloc);
         if (cnt) R.gbits = 1ull << (lb.geom0 + 1);
@@ -615,6 +662,11 @@ __device__ __noinline__ LFkOut l_sweep_out(const float* ms, float* sm, const LLa
     const bool actv = live && b >= 0;
     float K[18], kc[3];
     if (flags & LF_GOUT) l_rec_ld_Kc<C>(w, b, K, kc);
+    float gkp[3], gkd[3], gtl[3], gms = 1.f;   // (PRM) this body's gains, limits and mass scale, fetched with its lane record
+    if constexpr (C::PRM) {
+      if (spd_torque) { l_prm_ld3<C>(sm, C::PRM_KP, b, gkp); l_prm_ld3<C>(sm, C::PRM_KD, b, gkd); l_prm_ld3<C>(sm, C::PRM_TL, b, gtl); }
+      if (flags & LF_VEL) gms = __ldg(l_prm<C>(sm) + C::PRM_MS + (b < 0 ? 0 : b));
+    }
     S6 pbv = s6(v3(0.f, 0.f, 0.f), v3(0.f, 0.f, 0.f));
     float* br = sm + C::body + C::BODYW * (actv ? b : 0);
     int alloc = 0, nlr = 0;   // contact entries / limit rows this lane wants
@@ -643,8 +695,9 @@ __device__ __noinline__ LFkOut l_sweep_out(const float* ms, float* sm, const LLa
             const int i = d0 + k - 6;
             float q = k == 0 ? q0 : k == 1 ? q1 : q2, qd = k == 0 ? qd0 : k == 1 ? qd1 : qd2;
             float tgt = fmaf(sm[C::act + i], lb.ascale[k], lb.aoffset[k]);
-            float tq = -lb.kp[k] * (q + qd * hh - tgt) - lb.kd[k] * (qd + qdd * hh);
-            tq = fminf(fmaxf(tq, -lb.tlim[k]), lb.tlim[k]);
+            float tq = -(C::PRM ? gkp[k] : lb.kp[k]) * (q + qd * hh - tgt) - (C::PRM ? gkd[k] : lb.kd[k]) * (qd + qdd * hh);
+            const float tl = C::PRM ? gtl[k] : lb.tlim[k];
+            tq = fminf(fmaxf(tq, -tl), tl);
             sm[C::tau + i] = ztau ? 0.f : tq;
           }
         }
@@ -716,7 +769,7 @@ __device__ __noinline__ LFkOut l_sweep_out(const float* ms, float* sm, const LLa
     }
     if (actv && (flags & LF_FK)) {
       const LBody& lb = MB[b];
-      pbv = l_body_post<C>(lb, sm, w, b, flags, P, br, cb | (alloc << 8) | (lbs << 16) | (lcnt << 24));
+      pbv = l_body_post<C>(gms, lb, sm, w, b, flags, P, br, cb | (alloc << 8) | (lbs << 16) | (lcnt << 24));
       if (alloc) {
         int cnt = l_narrow<C>(H, MG[lb.geom0], lb.geom0, X, P.v, P.pa, lb.tiw0, sm, w, cb, alloc);
         if (cnt) gbits |= 1ull << (lb.geom0 + 1);
@@ -790,7 +843,7 @@ __device__ __forceinline__ void l_fold_contacts(const LHdr& H, float* sm, const 
 #pragma unroll
     for (int k = 0; k < 4; k++) {
       if (!(info & (2 << k))) continue;
-      V3 d = l_pyr_dir(H, n, t1, t2, k);
+      V3 d = l_pyr_dir(l_mu<C>(H, sm), n, t1, t2, k);
       V3 dd = D * d;
       gxx = fmaf(dd.x, d.x, gxx); gyy = fmaf(dd.y, d.y, gyy); gzz = fmaf(dd.z, d.z, gzz);
       gxy = fmaf(dd.x, d.y, gxy); gxz = fmaf(dd.x, d.z, gxz); gyz = fmaf(dd.y, d.z, gyz);
@@ -851,7 +904,7 @@ __device__ __forceinline__ void l_self_wrench(const LHdr& H, float* sm, const LL
     const V3 n = ld3(eb + LSB_N), t1 = ld3(ea + LCE_T1), t2 = cross(n, t1), cp = ld3(ea + LCE_CP);
     V3 f = v3(0.f, 0.f, 0.f);
 #pragma unroll
-    for (int k = 0; k < 4; k++) f = f + eb[LSB_LAM + k] * l_pyr_dir(H, n, t1, t2, k);
+    for (int k = 0; k < 4; k++) f = f + eb[LSB_LAM + k] * l_pyr_dir(l_mu<C>(H, sm), n, t1, t2, k);
     if (b == b1) f = -1.0f * f;
     p.l = p.l - f; p.a = p.a - cross(cp, f);
   }
@@ -882,7 +935,7 @@ __device__ __forceinline__ void l_self_part(const LHdr& H, float* sm, const LLan
     const V3 n = ld3(eb + LSB_N), t1 = ld3(ea + LCE_T1), t2 = cross(n, t1), cp = ld3(ea + LCE_CP);
     const V3 ac = a.l + cross(a.a, cp);
 #pragma unroll
-    for (int k = 0; k < 4; k++) eb[(b == b2 ? LSB_P2 : LSB_P1) + k] = dot(l_pyr_dir(H, n, t1, t2, k), ac);
+    for (int k = 0; k < 4; k++) eb[(b == b2 ? LSB_P2 : LSB_P1) + k] = dot(l_pyr_dir(l_mu<C>(H, sm), n, t1, t2, k), ac);
   }
 }
 // rows li + 8 q of the env's geom-geom rows (row = 4 * contact + k): rs = part2 - part1 - aref into entry A; rs[q] (0 without a row)
@@ -963,8 +1016,9 @@ __device__ __noinline__ int l_self_collide(const float* ms, float* sm, const LLa
       const V3 t2 = cross(n, t1);
       const float pm = dist - H.margin, imp = l_impedance(H, pm);
       const float tran = MB[b1].tiw0 + MB[b2].tiw0;
-      const float R0 = fmaxf((1.f - imp) / imp * (tran + H.mu * H.mu * tran), 1e-15f);
-      const float R1 = R0 / fmaxf(H.impratio, 1e-15f), mu = H.mu * sqrtf(R1 / R0);
+      const float mu0 = l_mu<C>(H, sm);
+      const float R0 = fmaxf((1.f - imp) / imp * (tran + mu0 * mu0 * tran), 1e-15f);
+      const float R1 = R0 / fmaxf(H.impratio, 1e-15f), mu = mu0 * sqrtf(R1 / R0);
       const S6 v1 = ld6(w.gbody + 10 * b1 + 4), v2 = ld6(w.gbody + 10 * b2 + 4);
       const V3 vc = (v2.l + cross(v2.a, pos)) - (v1.l + cross(v1.a, pos));
       ((int*)ea)[LCE_INFO] = 1 | 30 | 32 | LCE_SELF | (g2 << 8);
@@ -972,7 +1026,7 @@ __device__ __noinline__ int l_self_collide(const float* ms, float* sm, const LLa
       ea[LCE_D] = 1.0f / (2.f * mu * mu * R0);
 #pragma unroll
       for (int k = 0; k < 4; k++) {
-        ea[LCE_AREF + k] = -H.B * dot(l_pyr_dir(H, n, t1, t2, k), vc) - H.K * imp * pm;
+        ea[LCE_AREF + k] = -H.B * dot(l_pyr_dir(l_mu<C>(H, sm), n, t1, t2, k), vc) - H.K * imp * pm;
         ea[LCE_PHI + k] = 0.f; ea[LCE_R + k] = 0.f; ea[LCE_RS + k] = 0.f;
         eb[LSB_LAM + k] = 0.f; eb[LSB_P1 + k] = 0.f; eb[LSB_P2 + k] = 0.f; eb[LSB_R0 + k] = 0.f;
       }
@@ -1117,6 +1171,8 @@ __device__ __noinline__ void l_sweep_in(const float* ms, float* sm, const LLane&
     const bool need = actv && (!resweep || ((st.rc_bits >> t) & 1u));
     if (resweep && !__any_sync(L_FULL, need)) continue;
     S6 p = l_rec_ld_pb<C>(w, b);
+    float gkp[3], gkd[3];   // (PRM, stable-PD system) this body's gains, fetched with its lane record
+    if constexpr (C::PRM && SPD) { l_prm_ld3<C>(sm, C::PRM_KP, b, gkp); l_prm_ld3<C>(sm, C::PRM_KD, b, gkd); }
     float K[18], kc[3];   // written by the lanes that need the body; the others leave the record as it is
     if (need) {
       const LBody& lb = MB[b];
@@ -1158,7 +1214,7 @@ __device__ __noinline__ void l_sweep_in(const float* ms, float* sm, const LLane&
         float s[6], Uv[6];
         l_s6arr(S, s);
         sym_mul(A, s, Uv);
-        float D = lb.arm[k] + (spd ? hh * lb.kd[k] : lD[k]);
+        float D = lb.arm[k] + (spd ? hh * (C::PRM ? gkd[k] : lb.kd[k]) : lD[k]);
 #pragma unroll
         for (int j = 0; j < 6; j++) D = fmaf(s[j], Uv[j], D);
         float di = l_rcp(D), tin;
@@ -1169,7 +1225,7 @@ __device__ __noinline__ void l_sweep_in(const float* ms, float* sm, const LLane&
             sm[C::qvel + d] = qd; sm[C::qpos + d + 1] = q;
           }
           float tgt = fmaf(sm[C::act + i], lb.ascale[k], lb.aoffset[k]);
-          tin = -lb.kp[k] * (q + qd * hh - tgt) - lb.kd[k] * qd;
+          tin = -(C::PRM ? gkp[k] : lb.kp[k]) * (q + qd * hh - tgt) - (C::PRM ? gkd[k] : lb.kd[k]) * qd;
         } else tin = sm[C::tau + i] + lT[k];
         float uu = tin - dot6(S, p);
         sym_rank1(A, Uv, di);
@@ -1647,17 +1703,18 @@ __device__ __noinline__ void l_torque_elem(const float* ms, float* sm, const LLa
       if (mode == SMPLSIM_CTRL_TORQUE) tq = a * lb.ascale[k];
       else if (mode == SMPLSIM_CTRL_SIMPLE_PID) {   // stateful: integral / last error live in HBM (L2-resident, 2 x nu words per env)
         size_t o = (size_t)w.env * H.nu + i;
-        float dt = H.h * (float)H.cfg.nsubsteps, lim = lb.tlim[k];
+        float dt = H.h * (float)H.cfg.nsubsteps, lim = l_tlim<C>(sm, lb, i, k);
         float err = fmaf(a, lb.ascale[k], lb.aoffset[k]) - sm[C::qpos + 7 + i], le = sta.pid_last_error[o];
         float derr = (le != le) ? 0.f : err - le;
         float in = fminf(fmaxf(fmaf(err, dt, sta.pid_integral[o]), -lim), lim);
         sta.pid_integral[o] = in; sta.pid_last_error[o] = err;
-        tq = lb.kp[k] * err + in + lb.kd[k] * derr / dt;
+        tq = l_kp<C>(sm, lb, i, k) * err + in + l_kd<C>(sm, lb, i, k) * derr / dt;
       } else {
         float tgt = fmaf(a, lb.ascale[k], lb.aoffset[k]), q = sm[C::qpos + 7 + i], qd = sm[C::qvel + 6 + i];
-        tq = -lb.kp[k] * (q - tgt) - lb.kd[k] * qd;
+        tq = -l_kp<C>(sm, lb, i, k) * (q - tgt) - l_kd<C>(sm, lb, i, k) * qd;
       }
-      sm[C::tau + i] = fminf(fmaxf(tq, -lb.tlim[k]), lb.tlim[k]);
+      const float tl = l_tlim<C>(sm, lb, i, k);
+      sm[C::tau + i] = fminf(fmaxf(tq, -tl), tl);
     }
   }
   __syncwarp();
@@ -2022,7 +2079,7 @@ __device__ __noinline__ void l_contact_wrench(const float* ms, float* sm, const 
 #pragma unroll
       for (int k = 0; k < 4; k++) {
         const float fk = take ? ((info & (2 << k)) ? -ce[LCE_D] * ce[LCE_RS + k] : 0.f) : ce[LCE_PHI + k];
-        fc = fc + fk * l_pyr_dir(H, n0, t1, t2, k);
+        fc = fc + fk * l_pyr_dir(l_mu<C>(H, sm), n0, t1, t2, k);
       }
       f = f + fc; t = t + cross(ld3(ce + LCE_CP) - rc, fc);
     }
@@ -2033,7 +2090,7 @@ __device__ __noinline__ void l_contact_wrench(const float* ms, float* sm, const 
       const V3 n = ld3(eb + LSB_N), t1 = ld3(ea + LCE_T1), t2 = cross(n, t1);
       V3 fc = z;
 #pragma unroll
-      for (int k = 0; k < 4; k++) fc = fc + (take ? eb[LSB_LAM + k] : ea[LCE_PHI + k]) * l_pyr_dir(H, n, t1, t2, k);
+      for (int k = 0; k < 4; k++) fc = fc + (take ? eb[LSB_LAM + k] : ea[LCE_PHI + k]) * l_pyr_dir(l_mu<C>(H, sm), n, t1, t2, k);
       if (b == b1) fc = -1.0f * fc;
       f = f + fc; t = t + cross(ld3(ea + LCE_CP) - rc, fc);
     }
@@ -2159,6 +2216,18 @@ __device__ __forceinline__ float* l_setup(const float* __restrict__ gimg, int im
   return smem + img_bytes / 4 + 4 + (size_t)(wib * C::EPW + sub) * C::total;
 }
 
+// (PRM) the env's record address and friction into its task words (L_TSK_PRM / L_TSK_MU); lanes without a live env get env 0's
+template <class C>
+__device__ __forceinline__ void l_prm_stage(const float* ms, float* sm, const LLane& w) {
+  static_assert((C::tsk & 1) == 0, "the record address needs an 8-byte aligned task word");
+  if (w.li == 0) {
+    const float* r = l_hdr<C>(ms).prm + (size_t)(w.live ? w.env : 0) * C::PRMW;
+    *(const float**)(sm + C::tsk + L_TSK_PRM) = r;
+    sm[C::tsk + L_TSK_MU] = __ldg(r + C::PRM_MU);
+  }
+  __syncwarp();
+}
+
 // stable PD, stale inertia (quirk Q1): rebuild the (M + h Kd) factors of the state of the last forward pass for the current
 // state / action.  On entry qpos / qvel / act hold the current state; qpos_fwd / qvel_fwd come from HBM.
 template <class C>
@@ -2184,6 +2253,7 @@ __global__ void __launch_bounds__(256, 1) k_step5(const float* __restrict__ gimg
   const size_t eo = w.live ? (size_t)w.env : 0;   // lanes without a live env keep running (predicated): warp collectives stay legal
   const bool spd = (H.cfg.control_mode == SMPLSIM_CTRL_UHC_PD);
   LSolveLane st; st.dirty_bits = 0u; st.rc_bits = 0u;
+  if constexpr (C::PRM) l_prm_stage<C>(ms, sm, w);
   if (w.live && w.li == 0) { sm[C::misc + LMI_DISP] = 0.f; sm[C::misc + LMI_DISP + 1] = 0.f; ((int*)sm)[C::misc + LMI_NSELF] = 0; ((int*)sm)[C::misc + LMI_NCON] = 0; ((int*)sm)[C::misc + LMI_NLIM] = 0; }
   if (w.live) for (int i = w.li; i < (H.nslot + 3) / 4; i += LM_LPE) ((int*)sm)[C::pfl + i] = w.gpfl ? w.gpfl[i] : 0;   // working set of the previous call
   l_copy_in<C>(sm + C::act, a.action + eo * H.nu, H.nu, w);
@@ -2246,6 +2316,7 @@ __global__ void __launch_bounds__(256, 1) k_reset5(const float* __restrict__ gim
   float* sm = l_setup<C>(gimg, img_bytes, w, ms, a.n, a.map, a.gscr, a.gsens, a.gpfl, a.gbody);
   const LHdr& H = l_hdr<C>(ms);
   if (w.live && a.mask && !a.mask[w.env]) w.live = false;
+  if constexpr (C::PRM) l_prm_stage<C>(ms, sm, w);
   size_t eo = w.live ? (size_t)w.env : 0;
   const SmplsimEnvCfg& c = H.cfg;
   int init = a.init_mode < 0 ? c.state_init : a.init_mode;
@@ -2411,7 +2482,7 @@ __device__ __forceinline__ S6 l_inv_rows(const LHdr& H, float* sm, const LLane& 
     const V3 t1 = ld3(ce + LCE_T1), t2 = cross(n, t1);
     V3 fc = v3(0.f, 0.f, 0.f);
 #pragma unroll
-    for (int k = 0; k < 4; k++) if (info & (2 << k)) fc = fc + (-ce[LCE_D] * ce[LCE_RS + k]) * l_pyr_dir(H, n, t1, t2, k);
+    for (int k = 0; k < 4; k++) if (info & (2 << k)) fc = fc + (-ce[LCE_D] * ce[LCE_RS + k]) * l_pyr_dir(l_mu<C>(H, sm), n, t1, t2, k);
     f.l = f.l + fc; f.a = f.a + cross(ld3(ce + LCE_CP), fc);
   }
   return f;
@@ -2485,6 +2556,7 @@ __global__ void __launch_bounds__(256, 1) k_inverse5(const float* __restrict__ g
   float* sm = l_setup<C>(gimg, img_bytes, w, ms, a.n, a.map, a.gscr, nullptr, nullptr);
   const LHdr& H = l_hdr<C>(ms);
   const size_t eo = w.live ? (size_t)w.env : 0;
+  if constexpr (C::PRM) l_prm_stage<C>(ms, sm, w);
   if (w.live && w.li == 0) { ((int*)sm)[C::misc + LMI_NSELF] = 0; ((int*)sm)[C::misc + LMI_NCON] = 0; ((int*)sm)[C::misc + LMI_NLIM] = 0; }
   if (w.live) for (int i = w.li; i < (H.nslot + 3) / 4; i += LM_LPE) ((int*)sm)[C::pfl + i] = 0;
   l_copy_in<C>(sm + C::qpos, a.qpos + eo * (H.nv + 1), H.nv + 1, w);
@@ -2635,6 +2707,7 @@ __global__ void __launch_bounds__(256, 1) k_dyn5(const float* __restrict__ gimg,
   float* sm = l_setup<C>(gimg, img_bytes, w, ms, a.n, a.map, a.gscr, nullptr, nullptr);
   const LHdr& H = l_hdr<C>(ms);
   const size_t eo = w.live ? (size_t)w.env : 0;
+  if constexpr (C::PRM) l_prm_stage<C>(ms, sm, w);
   l_copy_in<C>(sm + C::qpos, a.qpos + eo * (H.nv + 1), H.nv + 1, w);
   if (a.qvel) l_copy_in<C>(sm + C::qvel, a.qvel + eo * H.nv, H.nv, w);
   else if (w.live) for (int i = w.li; i < H.nv; i += LM_LPE) sm[C::qvel + i] = 0.f;

@@ -38,7 +38,9 @@ struct LHdr {
   float B, h, grav[3], plane_pos[3];
   float plane_n[3], t1_default[3], pad1[2];
   float rarm[6], pad4[2];                      // armature of the six free-joint dofs
-  unsigned long long legal_mask, pad2;
+  unsigned long long legal_mask;
+  const float* prm;                            // device address of the handle's per-env parameter records (smplsim_set_env_params; NULL: none).
+                                               // Written into the device copy of the table only; read by the kernel instances with LCfg::PRM
   SmplsimEnvCfg cfg;
   signed char sched[LM_TMAX][LM_LPE];          // body of (step, lane) or -1
   unsigned char step_ng[LM_TMAX];              // per step: max geoms of a scheduled body (uniform loop bounds)

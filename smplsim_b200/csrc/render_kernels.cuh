@@ -213,19 +213,28 @@ __global__ void __launch_bounds__(R_THREADS) k_ray(RRayArgs a) {
   if (a.geomid) a.geomid[r] = gid;
 }
 
-// camera position and world axes (thread 0; after r_stage)
+// camera position and world axes (thread 0; after r_stage).  PRM: the handle has per-env parameter records (LHdr::prm), whose mass
+// scales weight the TRACKCOM centre of mass; the instance without them is the one every other call runs.
+template <int PRM>
 __device__ __forceinline__ void r_camera(const RRenderArgs& a, int env, const float* sbx, float* sc) {
   const SmplsimCamera& c = a.cam;
   V3 e = ld3(c.pos);
   V3 ax[3] = {v3(c.mat[0], c.mat[3], c.mat[6]), v3(c.mat[1], c.mat[4], c.mat[7]), v3(c.mat[2], c.mat[5], c.mat[8])};
   if (c.mode == SMPLSIM_CAM_TRACKCOM) {   // robot centre of mass, in body order
     const LBody* B = (const LBody*)((const char*)r_img(a.s, env) + LM_BODY_OFF);
+    const float* msc = nullptr;   // (PRM) this env's mass scales: record words [4 + 3 nu, 4 + 3 nu + nb) (LCfg::PRM_MS)
+    if constexpr (PRM != 0) {
+      const LHdr& H = *(const LHdr*)r_img(a.s, env);
+      msc = H.prm + (size_t)env * (size_t)((4 + 3 * H.nu + H.nb + 3) & ~3) + 4 + 3 * H.nu;
+    }
     V3 mc = v3(0.f, 0.f, 0.f);
     float m = 0.f;
     for (int b = 0; b < a.s.nb; b++) {
       const float* Rb = sbx + 12 * b;
-      mc = mc + B[b].mass * (v3(Rb[9], Rb[10], Rb[11]) + mrot(Rb, ld3(B[b].ipos)));
-      m += B[b].mass;
+      float mb = B[b].mass;
+      if constexpr (PRM != 0) mb *= __ldg(msc + b);
+      mc = mc + mb * (v3(Rb[9], Rb[10], Rb[11]) + mrot(Rb, ld3(B[b].ipos)));
+      m += mb;
     }
     e = e + (1.0f / m) * mc;
   } else if (c.mode == SMPLSIM_CAM_BODY) {
@@ -252,13 +261,14 @@ __device__ __forceinline__ bool r_shadowed(const RGeom* sg, const unsigned* smas
 
 __device__ __forceinline__ unsigned char r_u8(float c) { return (unsigned char)floorf(255.0f * fminf(fmaxf(c, 0.f), 1.f) + 0.5f); }
 
+template <int PRM>
 __global__ void __launch_bounds__(R_THREADS) k_render(RRenderArgs a) {
   __shared__ float sbx[12 * LM_MAXB];
   __shared__ RGeom sg[LM_MAXG];
   __shared__ float sc[12];
   const int env = blockIdx.x / a.tiles, tile = blockIdx.x % a.tiles;
   r_stage(a.s, env, sbx, sg);
-  if (threadIdx.x == 0) r_camera(a, env, sbx, sc);
+  if (threadIdx.x == 0) r_camera<PRM>(a, env, sbx, sc);
   __syncthreads();
   const V3 e = ld3(sc), cx = ld3(sc + 3), cy = ld3(sc + 6), cz = ld3(sc + 9);
   const int wid = threadIdx.x >> 5, lane = threadIdx.x & 31;

@@ -44,6 +44,9 @@ struct SmplsimHandle {
   int* dblk_img = nullptr;      // [nblocks] CTA -> table
   int* denv_model = nullptr;    // [num_envs] env -> table (device copy of env_model; ray casting and rendering)
   LMap map() const { LMap m; m.slot_env = dslot_env; m.blk_img = dblk_img; return m; }
+  // per-env physics parameters (smplsim_set_env_params): prmw words per env; NULL: none, and the kernels without them run
+  float* prm = nullptr;
+  int prmw = 0;
 };
 
 static thread_local std::string g_err;
@@ -61,7 +64,7 @@ struct DeviceGuard {   // every entry point runs on the handle's device and rest
 };
 
 extern "C" const char* smplsim_last_error(void) { return g_err.c_str(); }
-extern "C" int smplsim_version(void) { return 250; }   // 250: smplsim_ray / smplsim_render; 240: smplsim_dynamics; 230: smplsim_inverse; 220: SmplsimAux.contact_wrench; 210: SmplsimState.xfrc_applied; 200: lane-chain kernels (ABI structs of 110)
+extern "C" int smplsim_version(void) { return 260; }   // 260: smplsim_set_env_params; 250: smplsim_ray / smplsim_render; 240: smplsim_dynamics; 230: smplsim_inverse; 220: SmplsimAux.contact_wrench; 210: SmplsimState.xfrc_applied; 200: lane-chain kernels (ABI structs of 110)
 
 template <class C>
 static size_t cta_smem(const SmplsimHandle* h, int wpb) { return (size_t)h->img.hdr()->bytes + 16 + (size_t)wpb * C::EPW * C::total * 4; }
@@ -95,27 +98,35 @@ static int pick_wpb(SmplsimHandle* h) {
   h->env_words = C::total;
   if (cudaFuncSetAttribute(k_step5<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem) != cudaSuccess) return -1;
   if (cudaFuncSetAttribute(k_step5<typename C::WithXfrc>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem) != cudaSuccess) return -1;
+  if (cudaFuncSetAttribute(k_step5<typename C::WithXfrcPrm>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem) != cudaSuccess) return -1;
   if (cudaFuncSetAttribute(k_reset5<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem) != cudaSuccess) return -1;
+  if (cudaFuncSetAttribute(k_reset5<typename C::WithPrm>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem) != cudaSuccess) return -1;
   if (cudaFuncSetAttribute(k_kin5<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem) != cudaSuccess) return -1;
-  if constexpr (!C::SELFCOL)
+  if constexpr (!C::SELFCOL) {
     if (cudaFuncSetAttribute(k_inverse5<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem) != cudaSuccess) return -1;
+    if (cudaFuncSetAttribute(k_inverse5<typename C::WithPrm>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem) != cudaSuccess) return -1;
+  }
   if (cudaFuncSetAttribute(k_dyn5<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem) != cudaSuccess) return -1;
+  if (cudaFuncSetAttribute(k_dyn5<typename C::WithPrm>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem) != cudaSuccess) return -1;
   return best;
 }
 
 // step and mj_step: the instance with the external-wrench code compiled in only when the caller passes xfrc_applied (same layout,
 // shared memory and CTA size; without a wrench the kernel is the one without that code).  The contact wrench output is a run-time
-// argument of every instance (NULL: not written).
+// argument of every instance (NULL: not written).  While the handle has per-env parameter records, the instance with both the
+// parameter reads and the wrench code runs (its wrench pointer may be NULL).
 template <class C>
 static void run_step(SmplsimHandle* h, const LStepArgs& a, const float* xfrc, float* cwrench, cudaStream_t st) {
   int wpb = h->wpb, per = wpb * C::EPW, grid = h->nblocks ? h->nblocks : (a.n + per - 1) / per;
-  if (xfrc) L_LAUNCH(k_step5<typename C::WithXfrc>, grid, 32 * wpb, h->smem, st, h->dimg, h->img.hdr()->bytes, a, xfrc, cwrench);
+  if (h->prm) L_LAUNCH(k_step5<typename C::WithXfrcPrm>, grid, 32 * wpb, h->smem, st, h->dimg, h->img.hdr()->bytes, a, xfrc, cwrench);
+  else if (xfrc) L_LAUNCH(k_step5<typename C::WithXfrc>, grid, 32 * wpb, h->smem, st, h->dimg, h->img.hdr()->bytes, a, xfrc, cwrench);
   else L_LAUNCH(k_step5<C>, grid, 32 * wpb, h->smem, st, h->dimg, h->img.hdr()->bytes, a, nullptr, cwrench);
 }
 template <class C>
 static void run_reset(SmplsimHandle* h, const LResetArgs& a, float* cwrench, cudaStream_t st) {
-  int wpb = h->wpb, per = wpb * C::EPW;
-  L_LAUNCH(k_reset5<C>, h->nblocks ? h->nblocks : (a.n + per - 1) / per, 32 * wpb, h->smem, st, h->dimg, h->img.hdr()->bytes, a);
+  int wpb = h->wpb, per = wpb * C::EPW, grid = h->nblocks ? h->nblocks : (a.n + per - 1) / per;
+  if (h->prm) L_LAUNCH(k_reset5<typename C::WithPrm>, grid, 32 * wpb, h->smem, st, h->dimg, h->img.hdr()->bytes, a);
+  else L_LAUNCH(k_reset5<C>, grid, 32 * wpb, h->smem, st, h->dimg, h->img.hdr()->bytes, a);
   if (cwrench) {
     const int row = 6 * h->img.hdr()->nb;
     L_LAUNCH(k_zero_wrench, (int)(((long)a.n * row + 255) / 256), 256, 0, st, cwrench, a.mask, a.n, row);
@@ -128,11 +139,16 @@ static void run_kin(SmplsimHandle* h, const LKinArgs& a, cudaStream_t st) {
 }
 // inverse dynamics: instances without the geom-geom rows only (smplsim_inverse refuses self-collision handles).  One shape: launches of
 // at most num_envs rows (the handle's scratch rows), in order on the caller's stream; per-env shapes: n == num_envs, one launch.
+// Per-env parameter records: n == num_envs, one launch of the instance that reads them (row i = env i).
 template <class C>
 static void run_inverse(SmplsimHandle* h, const LInvArgs& a, cudaStream_t st) {
   if constexpr (!C::SELFCOL) {
     const LHdr& H = *h->img.hdr();
     const int wpb = h->wpb, per = wpb * C::EPW;
+    if (h->prm) {
+      L_LAUNCH(k_inverse5<typename C::WithPrm>, h->nblocks ? h->nblocks : (a.n + per - 1) / per, 32 * wpb, h->smem, st, h->dimg, H.bytes, a);
+      return;
+    }
     if (h->nblocks) {
       L_LAUNCH(k_inverse5<C>, h->nblocks, 32 * wpb, h->smem, st, h->dimg, H.bytes, a);
       return;
@@ -151,6 +167,10 @@ template <class C>
 static void run_dynamics(SmplsimHandle* h, const LDynArgs& a, cudaStream_t st) {
   const LHdr& H = *h->img.hdr();
   const int wpb = h->wpb, per = wpb * C::EPW;
+  if (h->prm) {
+    L_LAUNCH(k_dyn5<typename C::WithPrm>, h->nblocks ? h->nblocks : (a.n + per - 1) / per, 32 * wpb, h->smem, st, h->dimg, H.bytes, a);
+    return;
+  }
   if (h->nblocks) {
     L_LAUNCH(k_dyn5<C>, h->nblocks, 32 * wpb, h->smem, st, h->dimg, H.bytes, a);
     return;
@@ -178,7 +198,7 @@ static void run_dynamics(SmplsimHandle* h, const LDynArgs& a, cudaStream_t st) {
   } while (0)
 
 static void free_handle(SmplsimHandle* h) {
-  cudaFree(h->dimg); cudaFree(h->gscr); cudaFree(h->gsens); cudaFree(h->gpfl); cudaFree(h->gbody); cudaFree(h->dslot_env); cudaFree(h->dblk_img); cudaFree(h->denv_model);
+  cudaFree(h->prm); cudaFree(h->dimg); cudaFree(h->gscr); cudaFree(h->gsens); cudaFree(h->gpfl); cudaFree(h->gbody); cudaFree(h->dslot_env); cudaFree(h->dblk_img); cudaFree(h->denv_model);
   delete h;
 }
 
@@ -395,6 +415,7 @@ extern "C" int smplsim_inverse(SmplsimHandle* h, const float* qpos_dev, const fl
   if (n == 0) return SMPLSIM_OK;   // nothing is read: empty tensors may come as NULL
   if (!qpos_dev || !qvel_dev || !qacc_dev || !qfrc_inverse_dev) return fail(SMPLSIM_EINVAL, "smplsim_inverse: null argument");
   if (h->nblocks && n != h->num_envs) return fail(SMPLSIM_EINVAL, "smplsim_inverse: with per-env body shapes n must be the handle's num_envs (row i uses env i's shape)");
+  if (h->prm && n != h->num_envs) return fail(SMPLSIM_EINVAL, "smplsim_inverse: with per-env parameters n must be the handle's num_envs (row i uses env i's parameters)");
   DeviceGuard guard(h->device);
   LInvArgs a; std::memset(&a, 0, sizeof a);
   a.qpos = qpos_dev; a.qvel = qvel_dev; a.qacc = qacc_dev; a.qfrc = qfrc_inverse_dev; a.cwrench = contact_wrench_dev; a.gscr = h->gscr; a.n = n;
@@ -418,6 +439,7 @@ extern "C" int smplsim_dynamics(SmplsimHandle* h, const float* qpos_dev, const f
   if (!qM_dev && !qfrc_bias_dev && !njac) return fail(SMPLSIM_EINVAL, "smplsim_dynamics: no output requested");
   if (!qpos_dev) return fail(SMPLSIM_EINVAL, "smplsim_dynamics: null qpos");
   if (h->nblocks && n != h->num_envs) return fail(SMPLSIM_EINVAL, "smplsim_dynamics: with per-env body shapes n must be the handle's num_envs (row i uses env i's shape)");
+  if (h->prm && n != h->num_envs) return fail(SMPLSIM_EINVAL, "smplsim_dynamics: with per-env parameters n must be the handle's num_envs (row i uses env i's parameters)");
   DeviceGuard guard(h->device);
   LDynArgs a; std::memset(&a, 0, sizeof a);
   a.qpos = qpos_dev; a.qvel = qvel_dev; a.qM = qM_dev; a.bias = qfrc_bias_dev; a.jac = njac ? jac_dev : nullptr; a.gscr = h->gscr; a.n = n;
@@ -482,6 +504,8 @@ extern "C" int smplsim_render(SmplsimHandle* h, const float* xpos_dev, const flo
   if (!depth_dev && !seg_dev && !rgb_dev) return fail(SMPLSIM_EINVAL, "smplsim_render: no output requested");
   if (!xpos_dev || !xquat_dev) return fail(SMPLSIM_EINVAL, "smplsim_render: null xpos / xquat");
   if (h->nblocks && n != h->num_envs) return fail(SMPLSIM_EINVAL, "smplsim_render: with per-env body shapes n must be the handle's num_envs (row i uses env i's shape)");
+  const bool prm = h->prm && cam->mode == SMPLSIM_CAM_TRACKCOM;   // the robot COM with the env's mass scales
+  if (prm && n != h->num_envs) return fail(SMPLSIM_EINVAL, "smplsim_render: a TRACKCOM camera with per-env parameters needs n == num_envs (row i uses env i's masses)");
   const int tiles_x = (width + R_CTA_W - 1) / R_CTA_W, tiles = tiles_x * ((height + R_CTA_H - 1) / R_CTA_H);
   if ((long)n * tiles > 0x7fffffffL) return fail(SMPLSIM_EINVAL, "smplsim_render: n x image too large for one launch");
   DeviceGuard guard(h->device);
@@ -491,8 +515,85 @@ extern "C" int smplsim_render(SmplsimHandle* h, const float* xpos_dev, const flo
   a.depth = depth_dev; a.seg = seg_dev; a.rgb = rgb_dev; a.W = width; a.H = height; a.tiles_x = tiles_x; a.tiles = tiles;
   for (int g = 0; g < H.ng; g++)
     for (int k = 0; k < 3; k++) a.rgb_tab[3 * g + k] = geom_rgb ? geom_rgb[3 * g + k] : (k == 0 ? 0.8f : k == 1 ? 0.6f : 0.4f);   // <default> rgba of the MJCFs
-  L_LAUNCH(k_render, n * tiles, R_THREADS, 0, (cudaStream_t)stream, a);
+  if (prm) L_LAUNCH(k_render<1>, n * tiles, R_THREADS, 0, (cudaStream_t)stream, a);
+  else L_LAUNCH(k_render<0>, n * tiles, R_THREADS, 0, (cudaStream_t)stream, a);
   CUDA_TRY(cudaGetLastError());
+  return SMPLSIM_OK;
+}
+
+// ------------------------------------------------------------------ per-env physics parameters
+// The records' base address goes into the header of every device table (LHdr::prm), where the PRM kernel instances read it from the
+// staged copy; the other instances never read that word.  So the kernels keep their argument lists, and without records the launches
+// are exactly the ones before records existed.
+// Written in stream order on the caller's stream (set: before the records' fill and every later launch there); clear writes NULL
+// after a device synchronization, when no launch is left that could read it.
+static cudaError_t put_prm_ptr(SmplsimHandle* h, float* const* src, cudaStream_t st) {   // (the host emulator copies at once)
+  const LHdr& H = *h->img.hdr();
+  cudaError_t e = cudaSuccess;
+  for (int k = 0; k < h->nmodels && e == cudaSuccess; k++)
+#ifdef SMPLSIM_EMU
+    e = cudaMemcpy((char*)h->dimg + (size_t)H.bytes * k + offsetof(LHdr, prm), src, sizeof(float*), cudaMemcpyHostToDevice);
+#else
+    e = cudaMemcpyAsync((char*)h->dimg + (size_t)H.bytes * k + offsetof(LHdr, prm), src, sizeof(float*), cudaMemcpyHostToDevice, st);
+#endif
+  return e;
+}
+static PrmArgs prm_args(const SmplsimHandle* h) {
+  const LHdr& H = *h->img.hdr();
+  PrmArgs a; std::memset(&a, 0, sizeof a);
+  a.rec = h->prm; a.gimg = h->dimg; a.env_img = h->denv_model; a.img_words = H.bytes / 4; a.n = h->num_envs; a.nu = H.nu; a.nb = H.nb;
+  a.w = (4 + 3 * H.nu + H.nb + 3) & ~3;
+  return a;
+}
+
+extern "C" int smplsim_set_env_params(SmplsimHandle* h, const SmplsimEnvParams* p, const uint8_t* mask_dev, void* stream) {
+  if (!h || !p) return fail(SMPLSIM_EINVAL, "smplsim_set_env_params: null handle or params");
+  DeviceGuard guard(h->device);
+  int init = 0;
+  if (!h->prm) {
+    int w = 0;
+    L_DISPATCH(h, w = C_::PRMW);
+    float* rec = nullptr;
+    CUDA_TRY(cudaMalloc(&rec, (size_t)w * h->num_envs * 4));
+    h->prm = rec; h->prmw = w; init = 1;
+    const cudaError_t e = put_prm_ptr(h, &h->prm, (cudaStream_t)stream);   // the source is the handle's own field
+    if (e != cudaSuccess) {
+      cudaDeviceSynchronize(); cudaFree(rec); h->prm = nullptr; h->prmw = 0;
+      return fail(SMPLSIM_ECUDA, std::string("smplsim_set_env_params: ") + cudaGetErrorString(e));
+    }
+  }
+  PrmArgs a = prm_args(h);
+  if (a.w != h->prmw) return fail(SMPLSIM_EINVAL, "smplsim_set_env_params: record layout mismatch");
+  a.mask = mask_dev; a.init = init;
+  a.f[0] = p->friction; a.f[1] = p->gravity; a.f[2] = p->kp; a.f[3] = p->kd; a.f[4] = p->torque_limit; a.f[5] = p->body_mass_scale;
+  const long tot = (long)a.n * a.w;
+  L_LAUNCH(k_prm_set, (int)((tot + 255) / 256), 256, 0, (cudaStream_t)stream, a);
+  CUDA_TRY(cudaGetLastError());
+  return SMPLSIM_OK;
+}
+
+extern "C" int smplsim_get_env_params(SmplsimHandle* h, float* friction_dev, float* gravity_dev, float* kp_dev, float* kd_dev,
+                                      float* torque_limit_dev, float* body_mass_scale_dev, void* stream) {
+  if (!h) return fail(SMPLSIM_EINVAL, "smplsim_get_env_params: null handle");
+  DeviceGuard guard(h->device);
+  PrmArgs a = prm_args(h);
+  a.o[0] = friction_dev; a.o[1] = gravity_dev; a.o[2] = kp_dev; a.o[3] = kd_dev; a.o[4] = torque_limit_dev; a.o[5] = body_mass_scale_dev;
+  const long tot = (long)a.n * a.w;
+  L_LAUNCH(k_prm_get, (int)((tot + 255) / 256), 256, 0, (cudaStream_t)stream, a);
+  CUDA_TRY(cudaGetLastError());
+  return SMPLSIM_OK;
+}
+
+extern "C" int smplsim_clear_env_params(SmplsimHandle* h) {
+  if (!h) return fail(SMPLSIM_EINVAL, "smplsim_clear_env_params: null handle");
+  if (!h->prm) return SMPLSIM_OK;
+  DeviceGuard guard(h->device);
+  CUDA_TRY(cudaDeviceSynchronize());   // no launch that reads the records is still queued
+  static float* const none = nullptr;
+  CUDA_TRY(put_prm_ptr(h, &none, 0));
+  CUDA_TRY(cudaDeviceSynchronize());
+  CUDA_TRY(cudaFree(h->prm));
+  h->prm = nullptr; h->prmw = 0;
   return SMPLSIM_OK;
 }
 
