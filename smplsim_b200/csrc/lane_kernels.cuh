@@ -530,13 +530,17 @@ __device__ __forceinline__ int l_narrow(const LHdr& H, const LGeom& G, int g, co
     float nn = sqrtf(dot(t1, t1));
     t1 = (nn < 1e-15f) ? v3(1.f, 0.f, 0.f) : (1.0f / nn) * t1;
   }
+  int nlow = 0;   // box: lower-facing corners seen so far
 #pragma unroll 1
   for (int i = 0; i < npt && cnt < alloc; i++) {
     V3 cp; float dist;
+    int pt = i;     // the contact point's index within the geom, which keys its working-set slot
     if (G.type == SMPLSIM_GEOM_BOX) {
       const float s0 = (i & 1) ? 1.f : -1.f, s1 = (i & 2) ? 1.f : -1.f, s2 = (i & 4) ? 1.f : -1.f;   // corner = centre +- e0 +- e1 +- e2
       const float l = s0 * X.l0 + s1 * X.l1 + s2 * X.l2;
-      if (X.d0 + l > H.margin || l > 0.f) continue;
+      if (l > 0.f) continue;
+      pt = min(nlow++, alloc - 1);   // its rank among the (generically four) lower-facing corners
+      if (X.d0 + l > H.margin) continue;
       dist = X.d0 + l;
       cp = X.c + (s0 * X.e0 + s1 * X.e1 + s2 * X.e2) - (0.5f * dist) * pn;
     } else {
@@ -549,9 +553,12 @@ __device__ __forceinline__ int l_narrow(const LHdr& H, const LGeom& G, int g, co
     float R0 = fmaxf((1.f - imp) / imp * (tiw0 + mu0 * mu0 * tiw0), 1e-15f);
     float R1 = R0 / fmaxf(H.impratio, 1e-15f), mu = mu0 * sqrtf(R1 / R0);
     float kterm = H.K * imp * pm;
-    // working set inherited from the slot's previous substep; a new contact starts from the rows that would be violated if the
-    // body kept the acceleration it had in the previous substep
-    int slot = G.slot0 + cnt, pv = pf[slot], guess = 32;   // bit 5: new this substep
+    // working set: the rows that would be violated if the body kept the acceleration it had in the previous substep, plus, for a
+    // contact the slot held in the previous substep, the rows active at its end.  Taking the union cuts the CTA's slowest env's
+    // extra solves; the prediction alone, for every contact, was worse than the inherited set (DESIGN.md 3).  The slot belongs to
+    // the point (capsule end, box corner), not to the contact's position in the geom's list: a heel corner that lifts off must not
+    // hand its rows to the toe corner behind it
+    int slot = G.slot0 + pt, pv = pf[slot], guess = 32;   // bit 5: new this substep
     float e[12];
     e[1] = cp.x; e[2] = cp.y; e[3] = cp.z; e[4] = t1.x; e[5] = t1.y; e[6] = t1.z;
     e[7] = 1.0f / (2.f * mu * mu * R0);
@@ -565,7 +572,7 @@ __device__ __forceinline__ int l_narrow(const LHdr& H, const LGeom& G, int g, co
         if (dot(d, pc) - e[8 + k] < 0.f) guess |= 2 << k;
       }
     }
-    e[0] = __int_as_float(1 | ((pv & 1) ? (pv & 30) : guess) | (g << 8) | (slot << 16));
+    e[0] = __int_as_float(1 | ((pv & 1) ? ((pv | guess) & 30) : guess) | (g << 8) | (slot << 16));
 #ifdef SMPLSIM_STATS
     e[0] = __int_as_float(__float_as_int(e[0]) | ((((pv & 1) ? (pv & 30) : 30) >> 1) << 24) | (((guess & 30) >> 1) << 28));
 #endif
@@ -1397,8 +1404,10 @@ __device__ __noinline__ void l_rows(float* sm, const LLane& w_, bool run, int op
 #ifdef SMPLSIM_STATS
 // debug build (tools/solver_stats.py): why does the first solve of a substep miss?  counters: [0] env-substeps, [1] with rows,
 // [2] first pass ok, [3..8] histogram of extra solves 1..6+, [9] rows predicted active but rs >= 0, [10] rows predicted inactive
-// but rs < 0, [11] ... of which in a contact new this substep, [12] limit rows flipped, [13] contacts, [14] new contacts
-__device__ int g_lstats[32];
+// but rs < 0, [11] ... of which in a contact new this substep, [12] limit rows flipped, [13] contacts, [14] new contacts,
+// [32..38] histogram of the per-warp maximum of extra solves 0..6+, [39..45] the same per CTA (l_stat_tail)
+#define L_NSTATS 64
+__device__ int g_lstats[L_NSTATS];
 #define L_STAT(i, v) atomicAdd(&g_lstats[i], v)
 #else
 #define L_STAT(i, v) do { } while (0)
@@ -1671,6 +1680,19 @@ __device__ __noinline__ int l_solve(const float* ms, float* sm, const LLane& w, 
   return iters;
 }
 
+#ifdef SMPLSIM_STATS
+// what the warps wait on: the maximum of the extra solves over the live envs of a warp (it loops until all of them converge) and
+// of a CTA (its warps meet at the next substep's barrier).  Every thread of the CTA makes the call.
+__device__ void l_stat_tail(const LLane& w, int iters) {
+  int m = w.live ? min(iters, 6) : -1;
+  for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(L_FULL, m, o));
+  if (w.lane == 0 && m >= 0) L_STAT(32 + m, 1);
+  int c = -1;
+  for (int k = 0; k <= 6; k++) if (__syncthreads_or(m >= k)) c = k;
+  if (threadIdx.x == 0 && c >= 0) L_STAT(39 + c, 1);
+}
+#endif
+
 // the state rows the kernels read and write: SmplsimState without its trailing xfrc_applied, which k_step5 takes as a parameter of its
 // own.  The kernels keep a copy of their argument struct on the stack (parts of it are passed by reference), so it keeps the size it had
 // before the wrench existed.
@@ -1863,6 +1885,9 @@ __device__ __noinline__ void l_substeps(const float* ms, float* sm, const LLane&
       if (badacc) { fo->mask = fk2.mask; fo->iters = it2; }
     }
     l_save_working_set<C>(ms, sm, w);
+#ifdef SMPLSIM_STATS
+    l_stat_tail(w, fo->iters);
+#endif
     bad |= badacc;
     fo->status |= bad | extra;
     if (raw && bad) restore = true;

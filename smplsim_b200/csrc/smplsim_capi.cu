@@ -645,13 +645,13 @@ extern "C" int smplsim_gae(const float* rewards_dev, const float* not_done_dev, 
 }
 
 #ifdef SMPLSIM_STATS
-extern "C" int smplsim_debug_stats(int* out32, int reset) {
+extern "C" int smplsim_debug_stats(int* out, int reset) {   // out: L_NSTATS counters
 #ifdef SMPLSIM_EMU
-  for (int i = 0; i < 32; i++) { out32[i] = g_lstats[i]; if (reset) g_lstats[i] = 0; }
+  for (int i = 0; i < L_NSTATS; i++) { out[i] = g_lstats[i]; if (reset) g_lstats[i] = 0; }
 #else
   cudaDeviceSynchronize();
-  cudaMemcpyFromSymbol(out32, g_lstats, sizeof(int) * 32);
-  if (reset) { int z[32] = {0}; cudaMemcpyToSymbol(g_lstats, z, sizeof z); }
+  cudaMemcpyFromSymbol(out, g_lstats, sizeof(int) * L_NSTATS);
+  if (reset) { int z[L_NSTATS] = {0}; cudaMemcpyToSymbol(g_lstats, z, sizeof z); }
 #endif
   return 0;
 }
