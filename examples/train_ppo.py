@@ -5,6 +5,7 @@ smplsim_gae (advantages), PPOLearner (AgentPPO.update_params semantics, gradient
 
     python examples/train_ppo.py --env speed --num-envs 4096 --horizon 16 --epochs 5
     python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.1 examples/train_ppo.py --env getup
+    python examples/train_ppo.py --env im --num-envs 4096      # motion imitation (HumanoidImB200) on synthetic clips
 
 ``--horizon x --num-envs`` plays the role of ``learning.min_batch_size`` (51 200 in the reference yaml = 4096 envs x 12.5 steps)."""
 import argparse
@@ -24,7 +25,7 @@ from smplsim_b200.ppo import PolicyGaussian, PPOLearner, Value  # noqa: E402
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--env", default="speed", choices=["speed", "reach", "getup"])
+    ap.add_argument("--env", default="speed", choices=["speed", "reach", "getup", "im"])
     ap.add_argument("--num-envs", type=int, default=4096, help="envs on THIS GPU")
     ap.add_argument("--horizon", type=int, default=16)
     ap.add_argument("--epochs", type=int, default=5)
@@ -37,7 +38,13 @@ def main():
     if world > 1:
         torch.distributed.init_process_group("nccl", device_id=torch.device(dev))
     torch.manual_seed(a.seed)                         # identical initial weights on every rank
-    env = HumanoidBatchB200(make_cfg(env=a.env), num_envs=a.num_envs, device=dev, seed=a.seed, rank=rank, with_aux=False)
+    if a.env == "im":     # every env tracks a clip of the library; the synthetic clips stand in for an AMASS table (motion_loader.py)
+        from smplsim_b200.imitation import HumanoidImB200
+        from smplsim_b200.motion_lib import synthetic_tables
+        env = HumanoidImB200(make_cfg(env="im"), lambda b: synthetic_tables(b, num_clips=64, frames=300), num_envs=a.num_envs, device=dev,
+                             seed=a.seed, rank=rank)
+    else:
+        env = HumanoidBatchB200(make_cfg(env=a.env), num_envs=a.num_envs, device=dev, seed=a.seed, rank=rank, with_aux=False)
     policy = PolicyGaussian(env.num_obs, env.num_actions, a.units, "silu", -2.5, True).to(dev)
     value = Value(env.num_obs, a.units, "silu").to(dev)
     learner = PPOLearner(policy, value)               # gamma .99, tau .95, clip .2, 10 epochs, lr 5e-5 / 3e-4, grad clip 25

@@ -188,7 +188,7 @@ typedef struct SmplsimCamera {
 typedef struct SmplsimHandle SmplsimHandle;
 
 const char* smplsim_last_error(void);
-int smplsim_version(void);   /* 260 = this header (250: before smplsim_set_env_params; 240: before smplsim_ray / smplsim_render; 230: before smplsim_dynamics; 220: before smplsim_inverse;
+int smplsim_version(void);   /* 270 = this header (260: before smplsim_imitation; 250: before smplsim_set_env_params; 240: before smplsim_ray / smplsim_render; 230: before smplsim_dynamics; 220: before smplsim_inverse;
                               * 210: before SmplsimAux.contact_wrench; 200: before SmplsimState.xfrc_applied; 100: before pid_* state and aux.status) */
 
 /* MjModel.from_xml_string + MjData + setup_humanoid_properties/setup_controller
@@ -339,6 +339,75 @@ int smplsim_motion_gather(SmplsimHandle* h, const int32_t* motion_ids_dev, const
                           const float* motion_len_dev, const int32_t* num_frames_dev, const float* motion_dt_dev,
                           const int32_t* length_starts_dev, int num_tables, const float* const* tables_dev,
                           const int32_t* widths, float* const* outs_dev, int32_t* frame_idx_dev, void* cuda_stream);
+
+/* Motion-imitation task: every env tracks one clip of a motion library.  One launch, run after smplsim_step / smplsim_reset on the same
+ * stream, writes the env's observation row, reward, flags and position error; the stepper itself runs as SMPLSIM_TASK_NONE.  The
+ * reference ships no imitation task in its MuJoCo env layer (SURVEY.md 3.4), so the definitions are this project's, after the published
+ * PHC formulation.
+ *
+ * Per env e: clip id m = motion_ids[e] (clamped to [0, num_motions)), clip start time t0 = motion_t0[e], step counter p = progress[e]
+ * (SmplsimState.progress, already incremented by the step), control period dt = (float)(model.timestep * nsubsteps), the product taken
+ * in double precision.  ref(t) is the row of the tables picked by the frame rule of smplsim_motion_gather (phase clip, float idx0,
+ * blend, int() truncation, quirk Q12) for clip m at time t; times are t0 + k dt evaluated in float32 as ONE fused multiply-add.
+ * Simulated body state: p_b, q_b = aux.xpos / xquat (post-integration), v_b, w_b = aux.body_linvel / body_angvel (the values obs v2
+ * uses, quirk Q2); ^ marks the reference.  h = the heading-inverse quaternion of the simulated root (the one the self observation
+ * uses: with has_upright_start = 0 the root is first multiplied by (0.5, -0.5, -0.5, -0.5); heading = atan2 of the rotated x axis;
+ * h = rotation by -heading about z).  h * v rotates the vector v; (x) is the quaternion product; q^-1 is the conjugate (the tables and
+ * the stepper hold unit quaternions); six(q) = [q * (1,0,0), q * (0,0,1)].  B = cfg.tracked_bodies (J = num_tracked entries; NULL:
+ * all nbody bodies in order, num_tracked must then be nbody).
+ *
+ * Observation, target = ref(t0 + (p + 1) dt), the pose to reach by the next step.  obs row = [self obs, self_obs_dim words copied from
+ * self_obs_dev | 24 J words], the 24 J words grouped by kind, bodies in the order of B:
+ *     3J  h * (p^_b - p_b)
+ *     6J  six(h (x) q^_b (x) q_b^-1 (x) h^-1)
+ *     3J  h * (v^_b - v_b)
+ *     3J  h * (w^_b - w_b)
+ *     3J  h * (p^_b - p_root)            p_root = the simulated root position
+ *     6J  six(h (x) q^_b)
+ * Reward, compared with ref(t0 + p dt), the pose that should have been reached now:
+ *     r = w_pos exp(-k_pos mean_B |p^_b - p_b|^2) + w_rot exp(-k_rot mean_B th_b^2) + w_vel exp(-k_vel mean_B |v^_b - v_b|^2)
+ *       + w_angvel exp(-k_angvel mean_B |w^_b - w_b|^2),   th_b = 2 atan2(|xyz|, |w|) of q^_b (x) q_b^-1, in [0, pi].
+ * Flags, same reference row:
+ *     terminated = (p > 1 and max_B |p^_b - p_b| > termination_distance) or aux.status has bit 1, 2 or 4 (the stepper put the env back
+ *                  to qpos0, so it is no longer on its clip; aux.status NULL: not consulted);
+ *     truncated  = t0 + (p + 1) dt > motion_len[m] (no next target) or p > episode_length (strict, quirk Q7).
+ * mpjpe = mean_B |p^_b - p_b| in metres.  frames (may be NULL) receives the two table rows used, [N,2] = (now, next).
+ * The means and the maximum are reduced in a fixed order: the outputs are bit-reproducible. */
+typedef struct SmplsimImitationCfg {
+  float k_pos, k_rot, k_vel, k_angvel;   /* defaults of the `im` cfg group: 100, 10, 0.1, 0.1 */
+  float w_pos, w_rot, w_vel, w_angvel;   /*                                 0.5, 0.3, 0.1, 0.1 */
+  float termination_distance;            /* metres (0.25) */
+  int32_t episode_length;
+  int32_t self_obs_dim;                  /* must be the handle's self-observation width (the head of a smplsim_step observation row) */
+  int32_t num_tracked;                   /* J, in [1, nbody] */
+  const int32_t* tracked_bodies;         /* host array [num_tracked] of robot body indices (0 = root), or NULL */
+} SmplsimImitationCfg;
+/* Device tables of a motion library (the layout smplsim_motion_gather takes), read in place. */
+typedef struct SmplsimMotionTables {
+  const float* xpos;          /* [total_frames, nbody*3] */
+  const float* xquat;         /* [total_frames, nbody*4] */
+  const float* body_vel;      /* [total_frames, nbody*3] */
+  const float* body_ang_vel;  /* [total_frames, nbody*3] */
+  const float* motion_len;    /* [num_motions] seconds */
+  const int32_t* num_frames;  /* [num_motions] */
+  const float* motion_dt;     /* [num_motions] frame period */
+  const int32_t* length_starts; /* [num_motions] first row of the clip */
+  int32_t num_motions;
+  int32_t nbody;              /* bodies per table row; must be the handle's */
+} SmplsimMotionTables;
+/* Width of the observation row smplsim_imitation writes for num_tracked bodies: self-observation width + 24 num_tracked. */
+int smplsim_imitation_obs_dim(const SmplsimHandle* h, int num_tracked);
+/* For the envs whose mask byte is non-zero (mask_dev NULL: all): obs_dev[N, smplsim_imitation_obs_dim] and frames_dev; unless obs_only
+ * (the call after a reset) also reward_dev[N], terminated_dev[N], truncated_dev[N], mpjpe_dev[N].  obs_only != 0 leaves those four
+ * untouched (they may be NULL).  self_obs_dev: the observation rows smplsim_step / smplsim_reset wrote, row stride = smplsim_obs_dim(h).
+ * aux: xpos, xquat, body_linvel, body_angvel are read (required), status if non-NULL.  Works on every handle kind (SMPL, SMPL-X,
+ * per-env shapes, self-collision); reads no handle scratch and writes no env state, so the stepper's results do not depend on it.
+ * SMPLSIM_EINVAL: a null argument, num_tracked outside [1, nbody], a tracked body outside [0, nbody), tracked_bodies NULL with
+ * num_tracked != nbody, tab->nbody != the handle's, num_motions < 1, self_obs_dim != the handle's. */
+int smplsim_imitation(SmplsimHandle* h, const SmplsimImitationCfg* cfg, const SmplsimMotionTables* tab, const int32_t* motion_ids_dev,
+                      const float* motion_t0_dev, const int32_t* progress_dev, const SmplsimAux* aux, const float* self_obs_dev,
+                      const uint8_t* mask_dev, int obs_only, float* obs_dev, float* reward_dev, uint8_t* terminated_dev,
+                      uint8_t* truncated_dev, float* mpjpe_dev, int32_t* frames_dev, void* cuda_stream);
 
 /* estimate_advantages (smpl_sim/learning/learning_utils.py:198-218) on a [T,N] device rollout: reverse scan per env,
  * delta = r + gamma*V' *not_dead - V ; A = delta + gamma*tau*A' *not_done ; returns = V + A.  next_value (may be NULL = 0)

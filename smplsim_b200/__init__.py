@@ -5,4 +5,11 @@ Drop-in for the hot path of ZhengyiLuo/SMPLSim (``HumanoidEnv.step`` =
 """
 from .model import ModelDesc, load_model  # noqa: F401
 
-__all__ = ["ModelDesc", "load_model"]
+__all__ = ["ModelDesc", "load_model", "HumanoidImB200"]
+
+
+def __getattr__(name):          # the env classes need torch: imported on first use
+    if name == "HumanoidImB200":
+        from .imitation import HumanoidImB200
+        return HumanoidImB200
+    raise AttributeError(name)

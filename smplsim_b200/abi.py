@@ -6,7 +6,8 @@ from typing import Any
 
 from .model import ModelDesc, SmplsimModelDescC  # noqa: F401
 
-TASKS = {"HumanoidEnv": 0, "HumanoidSpeed": 1, "HumanoidReach": 2, "HumanoidGetup": 3}
+TASKS = {"HumanoidEnv": 0, "HumanoidSpeed": 1, "HumanoidReach": 2, "HumanoidGetup": 3,
+         "HumanoidIm": 0}   # imitation: the stepper runs SMPLSIM_TASK_NONE, the task is smplsim_imitation (imitation.py)
 CTRL_MODES = {"uhc_pd": 0, "pd": 1, "torque": 2, "simple_pid": 3, "default": 2}   # "default": ctrl = action (humanoid_env.py:409-410) = torque mode, scale 1, no limit
 STATE_INITS = {"Default": 0, "Fall": 1, "MoCap": 2}
 _AVAILABLE_CONTROLLERS = ["uhc_pd", "simple_pid", "pd", "torque", "default"]   # humanoid_env.py:32
@@ -50,6 +51,19 @@ class SmplsimCameraC(C.Structure):
 class SmplsimEnvParamsC(C.Structure):
     _fields_ = [("friction", C.c_void_p), ("gravity", C.c_void_p), ("kp", C.c_void_p), ("kd", C.c_void_p), ("torque_limit", C.c_void_p),
                 ("body_mass_scale", C.c_void_p)]
+
+
+class SmplsimImitationCfgC(C.Structure):
+    _fields_ = [("k_pos", C.c_float), ("k_rot", C.c_float), ("k_vel", C.c_float), ("k_angvel", C.c_float),
+                ("w_pos", C.c_float), ("w_rot", C.c_float), ("w_vel", C.c_float), ("w_angvel", C.c_float),
+                ("termination_distance", C.c_float), ("episode_length", C.c_int32), ("self_obs_dim", C.c_int32),
+                ("num_tracked", C.c_int32), ("tracked_bodies", C.c_void_p)]
+
+
+class SmplsimMotionTablesC(C.Structure):
+    _fields_ = [("xpos", C.c_void_p), ("xquat", C.c_void_p), ("body_vel", C.c_void_p), ("body_ang_vel", C.c_void_p),
+                ("motion_len", C.c_void_p), ("num_frames", C.c_void_p), ("motion_dt", C.c_void_p), ("length_starts", C.c_void_p),
+                ("num_motions", C.c_int32), ("nbody", C.c_int32)]
 
 
 def _get(node: Any, key: str, default=None):

@@ -52,6 +52,11 @@ ENV_GROUPS: Dict[str, Dict[str, Any]] = {
     "getup": dict(_ENV_COMMON, task="HumanoidGetup", state_init="Fall", recovery_steps=60, tar_height_min=0.5,
                   tar_height_max=1.2, height_change_steps_min=100, height_change_steps_max=200,
                   contact_bodies=list(_FEET)),
+    # motion imitation (imitation.py; not a reference group: its MuJoCo env layer ships no imitation task).  reward gains k and
+    # weights w over (position, rotation, velocity, angular velocity); tracked_bodies: body names or indices, None = all
+    "im": dict(_ENV_COMMON, task="HumanoidIm", state_init="MoCap", self_obs_v=2, create_vel_sensors=True, contact_bodies=list(_FEET),
+               im_k_pos=100.0, im_k_rot=10.0, im_k_vel=0.1, im_k_angvel=0.1, im_w_pos=0.5, im_w_rot=0.3, im_w_vel=0.1, im_w_angvel=0.1,
+               termination_distance=0.25, tracked_bodies=None),
 }
 # robot group -- smpl_sim/data/cfg/robot/{smpl,smplx}_humanoid.yaml
 _ROBOT_COMMON = dict(
@@ -91,6 +96,8 @@ def make_cfg(env: str = "base_env", robot: str = "smpl_humanoid", overrides: Opt
     c.update(top)
     c["env"] = Cfg.wrap(copy.deepcopy(ENV_GROUPS[env]))
     c["robot"] = Cfg.wrap(copy.deepcopy(ROBOT_GROUPS[robot]))
+    if c["env"].get("create_vel_sensors"):      # an env group that needs the body-velocity sensors (obs v2) turns them on in the robot
+        c["robot"]["create_vel_sensors"] = True
     c["output_dir"] = f"outputs/{c['exp_name']}"
     for k, v in (overrides or {}).items():
         _apply_override(c, k, v)

@@ -59,20 +59,22 @@ struct GatherArgs {
   const float* tables[SM_MAXTABLES]; float* outs[SM_MAXTABLES]; int widths[SM_MAXTABLES];
   int32_t* frame_idx; int n, ntab;
 };
-__global__ void k_motion_gather(GatherArgs a) {
-  int lane = threadIdx.x & 31;
-  int i = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (i >= a.n) return;
-  int id = a.ids[i];
-  float len = a.mlen[id], dt = a.mdt[id], t = a.times[i];
-  int nf = a.nframes[id];
-  // motion_lib_base.py:448-458 + :321-323 (quirk Q12): phase clip, float idx0, blend, int() truncation
+// the frame of a clip (length len, nf frames, frame period dt) at time t: motion_lib_base.py:448-458 + :321-323 (quirk Q12): phase clip,
+// float idx0, blend, int() truncation.  The one frame rule of the library: the gather and the imitation task both call it.
+__device__ __forceinline__ int motion_frame(float len, float dt, int nf, float t) {
   float phase = fminf(fmaxf(t / len, 0.f), 1.f);
   if (t < 0.f) t = 0.f;
   float idx0 = phase * (float)(nf - 1);
   float idx1 = fminf(idx0 + 1.f, (float)(nf - 1));
   float blend = fminf(fmaxf((t - idx0 * dt) / dt, 0.f), 1.f);
-  int fr = (int)((1.0f - blend) * idx0 + blend * idx1);
+  return (int)((1.0f - blend) * idx0 + blend * idx1);
+}
+__global__ void k_motion_gather(GatherArgs a) {
+  int lane = threadIdx.x & 31;
+  int i = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (i >= a.n) return;
+  int id = a.ids[i];
+  int fr = motion_frame(a.mlen[id], a.mdt[id], a.nframes[id], a.times[i]);
   size_t row = (size_t)(fr + a.starts[id]);
   if (lane == 0 && a.frame_idx) a.frame_idx[i] = (int)row;
   for (int k = 0; k < a.ntab; k++) {

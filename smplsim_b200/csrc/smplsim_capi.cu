@@ -12,6 +12,7 @@
 #include <vector>
 
 #include "aux_kernels.cuh"
+#include "imitation_kernels.cuh"
 #include "render_kernels.cuh"
 
 #ifdef SMPLSIM_EMU
@@ -47,6 +48,7 @@ struct SmplsimHandle {
   // per-env physics parameters (smplsim_set_env_params): prmw words per env; NULL: none, and the kernels without them run
   float* prm = nullptr;
   int prmw = 0;
+  double ctrl_dt = 0;      // control period: model.timestep * nsubsteps (smplsim_imitation)
 };
 
 static thread_local std::string g_err;
@@ -64,7 +66,7 @@ struct DeviceGuard {   // every entry point runs on the handle's device and rest
 };
 
 extern "C" const char* smplsim_last_error(void) { return g_err.c_str(); }
-extern "C" int smplsim_version(void) { return 260; }   // 260: smplsim_set_env_params; 250: smplsim_ray / smplsim_render; 240: smplsim_dynamics; 230: smplsim_inverse; 220: SmplsimAux.contact_wrench; 210: SmplsimState.xfrc_applied; 200: lane-chain kernels (ABI structs of 110)
+extern "C" int smplsim_version(void) { return 270; }   // 270: smplsim_imitation; 260: smplsim_set_env_params; 250: smplsim_ray / smplsim_render; 240: smplsim_dynamics; 230: smplsim_inverse; 220: SmplsimAux.contact_wrench; 210: SmplsimState.xfrc_applied; 200: lane-chain kernels (ABI structs of 110)
 
 template <class C>
 static size_t cta_smem(const SmplsimHandle* h, int wpb) { return (size_t)h->img.hdr()->bytes + 16 + (size_t)wpb * C::EPW * C::total * 4; }
@@ -254,6 +256,7 @@ static int create_impl(const SmplsimModelDesc* s, int nmodels, const int32_t* en
     return fail(SMPLSIM_EUNSUPPORTED, msg);
   }
   h->num_envs = num_envs; h->device = cuda_device; h->selfcol = cfg->self_collision ? 1 : 0;
+  h->ctrl_dt = s->timestep * cfg->nsubsteps;
   DeviceGuard guard(cuda_device);
   cudaError_t e = cudaDeviceGetAttribute(&h->max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, cuda_device);
 #ifndef SMPLSIM_EMU
@@ -630,6 +633,48 @@ extern "C" int smplsim_motion_gather(SmplsimHandle* h, const int32_t* motion_ids
   for (int k = 0; k < num_tables; k++) { a.tables[k] = tables_dev[k]; a.outs[k] = outs_dev[k]; a.widths[k] = widths[k]; }
   int wpb = 8;
   L_LAUNCH(k_motion_gather, (n + wpb - 1) / wpb, 32 * wpb, 0, (cudaStream_t)stream, a);
+  CUDA_TRY(cudaGetLastError());
+  return SMPLSIM_OK;
+}
+
+extern "C" int smplsim_imitation_obs_dim(const SmplsimHandle* h, int num_tracked) {
+  return h && num_tracked >= 0 ? h->img.hdr()->self_obs_dim + 24 * num_tracked : SMPLSIM_EINVAL;
+}
+
+extern "C" int smplsim_imitation(SmplsimHandle* h, const SmplsimImitationCfg* cfg, const SmplsimMotionTables* tab, const int32_t* motion_ids_dev,
+                                 const float* motion_t0_dev, const int32_t* progress_dev, const SmplsimAux* aux, const float* self_obs_dev,
+                                 const uint8_t* mask_dev, int obs_only, float* obs_dev, float* reward_dev, uint8_t* terminated_dev,
+                                 uint8_t* truncated_dev, float* mpjpe_dev, int32_t* frames_dev, void* stream) {
+  if (!h || !cfg || !tab || !aux) return fail(SMPLSIM_EINVAL, "smplsim_imitation: null handle / cfg / tables / aux");
+  const LHdr& H = *h->img.hdr();
+  if (cfg->num_tracked < 1 || cfg->num_tracked > H.nb) return fail(SMPLSIM_EINVAL, "smplsim_imitation: num_tracked outside [1, nbody]");
+  if (!cfg->tracked_bodies && cfg->num_tracked != H.nb) return fail(SMPLSIM_EINVAL, "smplsim_imitation: tracked_bodies NULL needs num_tracked == nbody");
+  if (cfg->tracked_bodies)
+    for (int j = 0; j < cfg->num_tracked; j++)
+      if (cfg->tracked_bodies[j] < 0 || cfg->tracked_bodies[j] >= H.nb) return fail(SMPLSIM_EINVAL, "smplsim_imitation: tracked body out of range [0, nbody)");
+  if (tab->nbody != H.nb) return fail(SMPLSIM_EINVAL, "smplsim_imitation: the tables' nbody is not the handle's");
+  if (tab->num_motions < 1) return fail(SMPLSIM_EINVAL, "smplsim_imitation: num_motions < 1");
+  if (cfg->self_obs_dim != H.self_obs_dim) return fail(SMPLSIM_EINVAL, "smplsim_imitation: self_obs_dim is not the handle's self-observation width");
+  if (!tab->xpos || !tab->xquat || !tab->body_vel || !tab->body_ang_vel || !tab->motion_len || !tab->num_frames || !tab->motion_dt || !tab->length_starts)
+    return fail(SMPLSIM_EINVAL, "smplsim_imitation: null motion table");
+  if (!aux->xpos || !aux->xquat || !aux->body_linvel || !aux->body_angvel) return fail(SMPLSIM_EINVAL, "smplsim_imitation: aux needs xpos, xquat, body_linvel, body_angvel");
+  if (!motion_ids_dev || !motion_t0_dev || !progress_dev || !self_obs_dev || !obs_dev) return fail(SMPLSIM_EINVAL, "smplsim_imitation: null argument");
+  if (!obs_only && (!reward_dev || !terminated_dev || !truncated_dev || !mpjpe_dev)) return fail(SMPLSIM_EINVAL, "smplsim_imitation: null reward / flag / mpjpe output");
+  DeviceGuard guard(h->device);
+  ImArgs a; std::memset(&a, 0, sizeof a);
+  a.txpos = tab->xpos; a.txquat = tab->xquat; a.tvel = tab->body_vel; a.tangvel = tab->body_ang_vel;
+  a.mlen = tab->motion_len; a.nframes = tab->num_frames; a.mdt = tab->motion_dt; a.starts = tab->length_starts; a.nmotion = tab->num_motions;
+  a.ids = motion_ids_dev; a.t0 = motion_t0_dev; a.progress = progress_dev; a.mask = mask_dev;
+  a.xpos = aux->xpos; a.xquat = aux->xquat; a.linvel = aux->body_linvel; a.angvel = aux->body_angvel; a.status = aux->status;
+  a.self_obs = self_obs_dev; a.obs = obs_dev; a.reward = reward_dev; a.mpjpe = mpjpe_dev; a.terminated = terminated_dev; a.truncated = truncated_dev;
+  a.frames = frames_dev;
+  a.k[0] = cfg->k_pos; a.k[1] = cfg->k_rot; a.k[2] = cfg->k_vel; a.k[3] = cfg->k_angvel;
+  a.w[0] = cfg->w_pos; a.w[1] = cfg->w_rot; a.w[2] = cfg->w_vel; a.w[3] = cfg->w_angvel;
+  a.term_dist = cfg->termination_distance; a.dt = (float)h->ctrl_dt; a.episode_length = cfg->episode_length;
+  a.n = h->num_envs; a.nb = H.nb; a.J = cfg->num_tracked; a.self_dim = H.self_obs_dim; a.self_stride = H.obs_dim; a.obs_only = obs_only ? 1 : 0;
+  for (int j = 0; j < a.J; j++) a.body[j] = (unsigned char)(cfg->tracked_bodies ? cfg->tracked_bodies[j] : j);
+  const int wpb = 8;
+  L_LAUNCH(k_imitation, (a.n + wpb - 1) / wpb, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a);
   CUDA_TRY(cudaGetLastError());
   return SMPLSIM_OK;
 }

@@ -15,7 +15,6 @@ from typing import Dict
 import numpy as np
 import torch
 
-from . import _lib
 from .batched import HumanoidBatchB200
 
 TABLE_KEYS = ("qpos", "qvel", "xpos", "xquat", "body_vel", "body_ang_vel", "dof_pos", "dof_vel")
@@ -87,8 +86,7 @@ class MotionLibB200:
         self._keys = TABLE_KEYS + tuple(k for k in OPTIONAL_KEYS if k in tables)
         for k in self._keys[len(TABLE_KEYS):]:
             self.tables[k] = torch.as_tensor(tables[k], dtype=torch.float32, device=dv).contiguous()
-        self.widths = (C.c_int32 * len(self._keys))(*[self.tables[k].shape[1] for k in self._keys])
-        self._tabs = (C.c_void_p * len(self._keys))(*[self.tables[k].data_ptr() for k in self._keys])
+        self._ptrs = {}          # tuple of table keys -> (table pointers, widths) of gather_into
         K = int(self._motion_lengths.shape[0])
         # per-motion shape parameters (motion_lib_base.py:_motion_bodies, 17 = 16 betas + gender) and library bookkeeping
         self._motion_bodies = torch.as_tensor(tables["motion_bodies"], dtype=torch.float32, device=dv) if "motion_bodies" in tables else torch.zeros(K, 17, device=dv)
@@ -115,13 +113,8 @@ class MotionLibB200:
         tm = motion_times.to(dv, torch.float32).contiguous()
         n = ids.shape[0]
         outs = {k: torch.empty(n, self.tables[k].shape[1], dtype=torch.float32, device=dv) for k in self._keys}
-        optr = (C.c_void_p * len(self._keys))(*[outs[k].data_ptr() for k in self._keys])
         frame = torch.empty(n, dtype=torch.int32, device=dv)
-        _lib.check(_lib.lib().smplsim_motion_gather(self.env._h, ids.data_ptr(), tm.data_ptr(), n, self._motion_lengths.data_ptr(),
-                                                    self._motion_num_frames.data_ptr(), self._motion_dt.data_ptr(), self.length_starts.data_ptr(),
-                                                    len(self._keys), self._tabs, self.widths, optr, frame.data_ptr(),
-                                                    C.c_void_p(torch.cuda.current_stream(dv).cuda_stream)))
-        self.env.gpu_launches += 1
+        self.gather_into(self._keys, ids, tm, [outs[k] for k in self._keys], frame)
         nb = self.env.model.nbody
         xpos = outs["xpos"].view(n, nb, 3)
         if offset is not None:
@@ -130,6 +123,22 @@ class MotionLibB200:
         return dict(root_pos=xpos[:, 0], root_rot=xquat[:, 0], dof_pos=outs["dof_pos"], root_vel=bv[:, 0], root_ang_vel=bav[:, 0],
                     dof_vel=outs["dof_vel"], xpos=xpos, xquat=xquat, body_vel=bv, body_ang_vel=bav, qpos=outs["qpos"], qvel=outs["qvel"],
                     motion_aa=outs.get("motion_aa"), motion_bodies=self._motion_bodies[ids.long()], frame_idx=frame)
+
+    def gather_into(self, keys, motion_ids: torch.Tensor, motion_times: torch.Tensor, outs, frame_idx=None):
+        """The frame gather of ``get_motion_state_intervaled`` for the tables ``keys`` only, into the caller's ``outs`` (one ``[n, width]``
+        float32 tensor per key): nothing is allocated.  ``motion_ids`` int32 / ``motion_times`` float32, contiguous, on the env's device."""
+        env, n = self.env, motion_ids.shape[0]
+        keys = tuple(keys)
+        if keys not in self._ptrs:
+            self._ptrs[keys] = ((C.c_void_p * len(keys))(*[self.tables[k].data_ptr() for k in keys]),
+                                (C.c_int32 * len(keys))(*[self.tables[k].shape[1] for k in keys]))
+        tabs, widths = self._ptrs[keys]
+        optr = (C.c_void_p * len(keys))(*[o.data_ptr() for o in outs])
+        env._check(env._L().smplsim_motion_gather(env._h, motion_ids.data_ptr(), motion_times.data_ptr(), n, self._motion_lengths.data_ptr(),
+                                                  self._motion_num_frames.data_ptr(), self._motion_dt.data_ptr(), self.length_starts.data_ptr(),
+                                                  len(keys), tabs, widths, optr, None if frame_idx is None else frame_idx.data_ptr(),
+                                                  env._stream()))
+        env.gpu_launches += 1
 
     def inverse_dynamics(self, contact_wrench: bool = False):
         """``env.inverse`` over every frame of the library: ``qfrc_inverse [total_frames, nv]`` (and ``contact_wrench [total_frames,
