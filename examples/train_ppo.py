@@ -6,6 +6,7 @@ smplsim_gae (advantages), PPOLearner (AgentPPO.update_params semantics, gradient
     python examples/train_ppo.py --env speed --num-envs 4096 --horizon 16 --epochs 5
     python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.1 examples/train_ppo.py --env getup
     python examples/train_ppo.py --env im --num-envs 4096      # motion imitation (HumanoidImB200) on synthetic clips
+    python examples/train_ppo.py --env im --amp                # ... plus the AMP style reward (HumanoidAmpB200, AMPLearner)
 
 ``--horizon x --num-envs`` plays the role of ``learning.min_batch_size`` (51 200 in the reference yaml = 4096 envs x 12.5 steps)."""
 import argparse
@@ -31,6 +32,7 @@ def main():
     ap.add_argument("--epochs", type=int, default=5)
     ap.add_argument("--units", type=int, nargs="+", default=[2048, 1536, 1024, 1024, 512, 512])   # data/cfg/learning/simple_mlp.yaml
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--amp", action="store_true", help="adversarial motion priors: discriminator reward mixed into the task reward")
     a = ap.parse_args()
     rank, world, local = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("LOCAL_RANK", 0))
     torch.cuda.set_device(local)
@@ -44,7 +46,14 @@ def main():
         env = HumanoidImB200(make_cfg(env="im"), lambda b: synthetic_tables(b, num_clips=64, frames=300), num_envs=a.num_envs, device=dev,
                              seed=a.seed, rank=rank)
     else:
-        env = HumanoidBatchB200(make_cfg(env=a.env), num_envs=a.num_envs, device=dev, seed=a.seed, rank=rank, with_aux=False)
+        env = HumanoidBatchB200(make_cfg(env=a.env), num_envs=a.num_envs, device=dev, seed=a.seed, rank=rank, with_aux=a.amp)
+    amp_learner = None
+    if a.amp:             # the demonstrations: the imitation env's library, or synthetic clips for the other tasks
+        from smplsim_b200.amp import HumanoidAmpB200
+        from smplsim_b200.motion_lib import MotionLibB200, synthetic_tables
+        lib = None if a.env == "im" else MotionLibB200(env, synthetic_tables(env, num_clips=64, frames=300))
+        env = HumanoidAmpB200(env, lib)
+        amp_learner = env.make_learner()
     policy = PolicyGaussian(env.num_obs, env.num_actions, a.units, "silu", -2.5, True).to(dev)
     value = Value(env.num_obs, a.units, "silu").to(dev)
     learner = PPOLearner(policy, value)               # gamma .99, tau .95, clip .2, 10 epochs, lr 5e-5 / 3e-4, grad clip 25
@@ -60,12 +69,17 @@ def main():
         batch = sampler.sample(a.horizon)
         torch.cuda.synchronize(); t1 = time.time()
         info = learner.update(batch)
+        if amp_learner is not None:
+            info.update(amp_learner.update(env.drain_amp_obs()))
         torch.cuda.synchronize(); t2 = time.time()
         ts, tu = max_over_ranks(t1 - t0, dev), max_over_ranks(t2 - t1, dev)
         if rank == 0:
             n = a.horizon * a.num_envs * world
             print(f"epoch {ep}: {n} samples  sample {ts:.2f}s ({n / ts / 1e3:.0f}k env-steps/s)  update {tu:.2f}s  "
                   f"reward {info['mean_reward']:.4f}  policy_loss {info['policy_loss']:.4f}  value_loss {info['value_loss']:.4f}", flush=True)
+            if amp_learner is not None:
+                print(f"  amp: task reward {float(env.extras['task_rew_buf'].mean()):.4f}  disc reward {float(env.disc_rew_buf.mean()):.4f}  "
+                      f"disc_loss {info['disc_loss']:.4f}  acc agent {info['disc_agent_acc']:.3f} demo {info['disc_demo_acc']:.3f}", flush=True)
     if world > 1:
         torch.distributed.destroy_process_group()
 

@@ -188,7 +188,7 @@ typedef struct SmplsimCamera {
 typedef struct SmplsimHandle SmplsimHandle;
 
 const char* smplsim_last_error(void);
-int smplsim_version(void);   /* 270 = this header (260: before smplsim_imitation; 250: before smplsim_set_env_params; 240: before smplsim_ray / smplsim_render; 230: before smplsim_dynamics; 220: before smplsim_inverse;
+int smplsim_version(void);   /* 280 = this header (270: before smplsim_amp_obs / smplsim_amp_demo; 260: before smplsim_imitation; 250: before smplsim_set_env_params; 240: before smplsim_ray / smplsim_render; 230: before smplsim_dynamics; 220: before smplsim_inverse;
                               * 210: before SmplsimAux.contact_wrench; 200: before SmplsimState.xfrc_applied; 100: before pid_* state and aux.status) */
 
 /* MjModel.from_xml_string + MjData + setup_humanoid_properties/setup_controller
@@ -408,6 +408,63 @@ int smplsim_imitation(SmplsimHandle* h, const SmplsimImitationCfg* cfg, const Sm
                       const float* motion_t0_dev, const int32_t* progress_dev, const SmplsimAux* aux, const float* self_obs_dev,
                       const uint8_t* mask_dev, int obs_only, float* obs_dev, float* reward_dev, uint8_t* terminated_dev,
                       uint8_t* truncated_dev, float* mpjpe_dev, int32_t* frames_dev, void* cuda_stream);
+
+/* Adversarial motion priors (AMP): the discriminator's observation of an env's last K control steps and of a motion library's clips.
+ * The per-frame feature is the reference's compute_humanoid_observations_smpl with has_smpl_params = False (smpl_sim/envs/nv/humanoid.py:
+ * 2530-2602, dof_to_obs :2276-2309, remove_base_rot :2523-2527); quaternions here are wxyz, the reference's xyzw.  One frame, F floats:
+ *     root_h                              root_pos.z, only if root_height_obs (the column is dropped, not zeroed, as in the _smpl variant)
+ *     r = root_rot, and r = r (x) conj(0.5, 0.5, 0.5, 0.5) unless upright_start (remove_base_rot; the rule of the heading below)
+ *     h = the heading-inverse of r (rotation by -atan2 of r's rotated x axis about z; the h of smplsim_imitation)
+ *     tan_norm(local_root_obs ? h (x) r : r)     6   tan_norm(q) = [q * (1,0,0), q * (0,0,1)]
+ *     h * root_vel, h * root_ang_vel             3 + 3 (world-frame velocities)
+ *     dof_obs                             6 (nbody - 1): per non-root body b, its 3 hinge angles e = dof_pos[3(b-1) : 3b] as an exp map:
+ *                                         a = |e| wrapped by atan2(sin a, cos a); |a| <= 1e-5 -> the identity, else the rotation by a about
+ *                                         e / |e|; then tan_norm
+ *     dof_vel                             nv - 6
+ *     h * (key_pos_k - root_pos)          3 per key body, in the order of cfg.key_bodies
+ * F = 232 for SMPL (24 bodies, 4 key bodies, root height), 484 for SMPL-X.  A model whose non-root bodies do not all have exactly 3
+ * hinges: SMPLSIM_EUNSUPPORTED (the reference asserts on them).
+ * Sources:
+ *   simulated env e, the post-step state: root_pos, key_pos = aux.xpos, root_rot = aux.xquat[e, 0], root_vel = qvel[0:3], root_ang_vel =
+ *     root_rot * qvel[3:6] (MuJoCo's body-frame angular velocity rotated to world), dof_pos = qpos[7:], dof_vel = qvel[6:] -- all from the
+ *     same post-integration state, which is what Isaac's rigid-body / dof tensors hold after simulate.  (smplsim_imitation and obs v2
+ *     read the pre-integration body velocities instead, quirk Q2.)
+ *   motion library, clip m at time t: ref(t) = the row of the xpos, xquat, body_vel[0], body_ang_vel[0], dof_pos, dof_vel tables that the
+ *     frame rule of smplsim_motion_gather picks (nearest frame, no slerp, quirk Q12); the clip id is clamped to [0, num_motions).
+ * AMP observation: K = num_steps frames newest first, amp_obs[N, K, F], frame k = control step p - k.  dt = (float)(model.timestep *
+ * nsubsteps).  Times t - k dt and t0 + (p - k) dt are one float32 fused multiply-add, as in smplsim_imitation.
+ * Nothing is reduced and nothing is atomic: the outputs are bit-reproducible.  Neither call writes env state or handle scratch; every
+ * handle kind (SMPL, SMPL-X, per-env shapes, self-collision) is supported. */
+#define SMPLSIM_AMP_PUSH 0     /* frames 0..K-2 move to 1..K-1 in place, the current simulated frame goes to 0 (after every env step) */
+#define SMPLSIM_AMP_FILL 1     /* the current simulated frame in all K slots (Default / Fall resets) */
+#define SMPLSIM_AMP_FILL_REF 2 /* the current simulated frame at 0, ref(t0 + (p - k) dt) of the env's clip in slot k >= 1 (MoCap resets) */
+typedef struct SmplsimAmpCfg {
+  int32_t num_steps;             /* K >= 1 (numAMPObsSteps: 10) */
+  int32_t num_key_bodies;        /* in [0, nbody] */
+  const int32_t* key_bodies;     /* host array [num_key_bodies] of robot body indices (0 = root); may be NULL when num_key_bodies = 0 */
+  int32_t local_root_obs;        /* 0/1 */
+  int32_t root_height_obs;       /* 0/1 */
+} SmplsimAmpCfg;
+/* The tables of ref(t): a motion library (SmplsimMotionTables, read in place) plus its joint tables. */
+typedef struct SmplsimAmpTables {
+  const SmplsimMotionTables* motion;
+  const float* dof_pos;          /* [total_frames, nv - 6] */
+  const float* dof_vel;          /* [total_frames, nv - 6] */
+} SmplsimAmpTables;
+/* F of cfg on this handle (negative SMPLSIM_E* for a bad cfg). */
+int smplsim_amp_obs_dim(const SmplsimHandle* h, const SmplsimAmpCfg* cfg);
+/* The envs whose mask byte is non-zero (mask_dev NULL: all) get their amp_obs_dev[N, K, F] row updated by mode; the others are not
+ * written.  st: qpos, qvel (and progress for FILL_REF) are read; aux: xpos, xquat.  FILL_REF also reads tab, motion_ids_dev[N] and
+ * motion_t0_dev[N] (the clip and the clip time of step 0, as smplsim_imitation); the other modes ignore them (they may be NULL).
+ * SMPLSIM_EINVAL: a null required pointer, num_steps < 1, a bad key body, tab->motion->nbody != the handle's, num_motions < 1, an
+ * unknown mode. */
+int smplsim_amp_obs(SmplsimHandle* h, const SmplsimAmpCfg* cfg, const SmplsimState* st, const SmplsimAux* aux, const SmplsimAmpTables* tab,
+                    const int32_t* motion_ids_dev, const float* motion_t0_dev, const uint8_t* mask_dev, int mode, float* amp_obs_dev,
+                    void* cuda_stream);
+/* Demonstration rows: out[i, k] = ref(motion_times[i] - k dt) of clip motion_ids[i], for n >= 0 caller rows (any n on every handle kind:
+ * nothing depends on the env's body shape).  SMPLSIM_EINVAL as smplsim_amp_obs. */
+int smplsim_amp_demo(SmplsimHandle* h, const SmplsimAmpCfg* cfg, const SmplsimAmpTables* tab, const int32_t* motion_ids_dev,
+                     const float* motion_times_dev, int n, float* out_dev, void* cuda_stream);
 
 /* estimate_advantages (smpl_sim/learning/learning_utils.py:198-218) on a [T,N] device rollout: reverse scan per env,
  * delta = r + gamma*V' *not_dead - V ; A = delta + gamma*tau*A' *not_done ; returns = V + A.  next_value (may be NULL = 0)

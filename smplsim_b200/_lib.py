@@ -62,6 +62,10 @@ _SYMBOLS = {
     "smplsim_imitation_obs_dim": (C.c_int, [C.c_void_p, C.c_int]),
     "smplsim_imitation": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                     C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "smplsim_amp_obs_dim": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "smplsim_amp_obs": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                  C.c_void_p, C.c_void_p]),
+    "smplsim_amp_demo": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "smplsim_gae": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_int, C.c_int, C.c_void_p,
                               C.c_void_p, C.c_void_p]),
     "smplsim_smem_bytes_per_env": (C.c_int, [C.c_void_p]),

@@ -66,6 +66,18 @@ class SmplsimMotionTablesC(C.Structure):
                 ("num_motions", C.c_int32), ("nbody", C.c_int32)]
 
 
+class SmplsimAmpCfgC(C.Structure):
+    _fields_ = [("num_steps", C.c_int32), ("num_key_bodies", C.c_int32), ("key_bodies", C.c_void_p), ("local_root_obs", C.c_int32),
+                ("root_height_obs", C.c_int32)]
+
+
+class SmplsimAmpTablesC(C.Structure):
+    _fields_ = [("motion", C.c_void_p), ("dof_pos", C.c_void_p), ("dof_vel", C.c_void_p)]
+
+
+AMP_PUSH, AMP_FILL, AMP_FILL_REF = 0, 1, 2     # SMPLSIM_AMP_* modes of smplsim_amp_obs
+
+
 def _get(node: Any, key: str, default=None):
     if hasattr(node, "get"):
         return node.get(key, default)

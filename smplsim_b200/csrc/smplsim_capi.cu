@@ -13,6 +13,7 @@
 
 #include "aux_kernels.cuh"
 #include "imitation_kernels.cuh"
+#include "amp_kernels.cuh"
 #include "render_kernels.cuh"
 
 #ifdef SMPLSIM_EMU
@@ -66,7 +67,7 @@ struct DeviceGuard {   // every entry point runs on the handle's device and rest
 };
 
 extern "C" const char* smplsim_last_error(void) { return g_err.c_str(); }
-extern "C" int smplsim_version(void) { return 270; }   // 270: smplsim_imitation; 260: smplsim_set_env_params; 250: smplsim_ray / smplsim_render; 240: smplsim_dynamics; 230: smplsim_inverse; 220: SmplsimAux.contact_wrench; 210: SmplsimState.xfrc_applied; 200: lane-chain kernels (ABI structs of 110)
+extern "C" int smplsim_version(void) { return 280; }   // 280: smplsim_amp_obs / smplsim_amp_demo; 270: smplsim_imitation; 260: smplsim_set_env_params; 250: smplsim_ray / smplsim_render; 240: smplsim_dynamics; 230: smplsim_inverse; 220: SmplsimAux.contact_wrench; 210: SmplsimState.xfrc_applied; 200: lane-chain kernels (ABI structs of 110)
 
 template <class C>
 static size_t cta_smem(const SmplsimHandle* h, int wpb) { return (size_t)h->img.hdr()->bytes + 16 + (size_t)wpb * C::EPW * C::total * 4; }
@@ -675,6 +676,98 @@ extern "C" int smplsim_imitation(SmplsimHandle* h, const SmplsimImitationCfg* cf
   for (int j = 0; j < a.J; j++) a.body[j] = (unsigned char)(cfg->tracked_bodies ? cfg->tracked_bodies[j] : j);
   const int wpb = 8;
   L_LAUNCH(k_imitation, (a.n + wpb - 1) / wpb, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a);
+  CUDA_TRY(cudaGetLastError());
+  return SMPLSIM_OK;
+}
+
+// ------------------------------------------------------------------ adversarial motion priors (amp_kernels.cuh)
+static int amp_dim(const LHdr& H, const SmplsimAmpCfg* cfg) {
+  return (cfg->root_height_obs ? 1 : 0) + 12 + 6 * (H.nb - 1) + (H.nv - 6) + 3 * cfg->num_key_bodies;
+}
+// the arguments every AMP call shares; "" when they are good, else the reason (SMPLSIM_EINVAL, or EUNSUPPORTED when *code says so)
+static std::string amp_check(const SmplsimHandle* h, const SmplsimAmpCfg* cfg, int* code) {
+  *code = SMPLSIM_EINVAL;
+  if (!h || !cfg) return "null handle / cfg";
+  const LHdr& H = *h->img.hdr();
+  if (cfg->num_steps < 1) return "num_steps < 1";
+  if (cfg->num_key_bodies < 0 || cfg->num_key_bodies > H.nb) return "num_key_bodies outside [0, nbody]";
+  if (cfg->num_key_bodies > 0 && !cfg->key_bodies) return "key_bodies NULL with num_key_bodies > 0";
+  for (int k = 0; k < cfg->num_key_bodies; k++)
+    if (cfg->key_bodies[k] < 0 || cfg->key_bodies[k] >= H.nb) return "key body out of range [0, nbody)";
+  // dof_to_obs takes every non-root joint as a 3-dof exp map (the reference asserts on any other joint)
+  bool hinge3 = H.nv == 6 + 3 * (H.nb - 1);
+  for (int b = 1; b < H.nb && hinge3; b++) hinge3 = h->img.bodies()[b].dofadr == 6 + 3 * (b - 1);
+  if (!hinge3) { *code = SMPLSIM_EUNSUPPORTED; return "every non-root body must have exactly 3 hinges"; }
+  return "";
+}
+static std::string amp_tables(const LHdr& H, const SmplsimAmpTables* tab, AmpArgs& a) {
+  if (!tab || !tab->motion) return "null motion tables";
+  const SmplsimMotionTables* m = tab->motion;
+  if (m->nbody != H.nb) return "the tables' nbody is not the handle's";
+  if (m->num_motions < 1) return "num_motions < 1";
+  if (!m->xpos || !m->xquat || !m->body_vel || !m->body_ang_vel || !m->motion_len || !m->num_frames || !m->motion_dt || !m->length_starts ||
+      !tab->dof_pos || !tab->dof_vel)
+    return "null motion table";
+  a.txpos = m->xpos; a.txquat = m->xquat; a.tvel = m->body_vel; a.tangvel = m->body_ang_vel; a.tdof = tab->dof_pos; a.tdofv = tab->dof_vel;
+  a.mlen = m->motion_len; a.nframes = m->num_frames; a.mdt = m->motion_dt; a.starts = m->length_starts; a.nmotion = m->num_motions;
+  return "";
+}
+static void amp_common(const SmplsimHandle* h, const SmplsimAmpCfg* cfg, AmpArgs& a) {
+  const LHdr& H = *h->img.hdr();
+  a.K = cfg->num_steps; a.F = amp_dim(H, cfg); a.nb = H.nb; a.nv = H.nv; a.nkey = cfg->num_key_bodies;
+  a.local_root = cfg->local_root_obs ? 1 : 0; a.root_h = cfg->root_height_obs ? 1 : 0; a.dt = (float)h->ctrl_dt;
+  for (int k = 0; k < a.nkey; k++) a.key[k] = (unsigned char)cfg->key_bodies[k];
+}
+
+extern "C" int smplsim_amp_obs_dim(const SmplsimHandle* h, const SmplsimAmpCfg* cfg) {
+  int code;
+  const std::string why = amp_check(h, cfg, &code);
+  if (!why.empty()) return fail(code, "smplsim_amp_obs_dim: " + why);
+  return amp_dim(*h->img.hdr(), cfg);
+}
+
+extern "C" int smplsim_amp_obs(SmplsimHandle* h, const SmplsimAmpCfg* cfg, const SmplsimState* st, const SmplsimAux* aux,
+                               const SmplsimAmpTables* tab, const int32_t* motion_ids_dev, const float* motion_t0_dev, const uint8_t* mask_dev,
+                               int mode, float* amp_obs_dev, void* stream) {
+  int code;
+  std::string why = amp_check(h, cfg, &code);
+  if (!why.empty()) return fail(code, "smplsim_amp_obs: " + why);
+  if (mode < SMPLSIM_AMP_PUSH || mode > SMPLSIM_AMP_FILL_REF) return fail(SMPLSIM_EINVAL, "smplsim_amp_obs: unknown mode");
+  if (!st || !st->qpos || !st->qvel || !aux || !aux->xpos || !aux->xquat || !amp_obs_dev)
+    return fail(SMPLSIM_EINVAL, "smplsim_amp_obs: null state (qpos, qvel), aux (xpos, xquat) or output");
+  AmpArgs a; std::memset(&a, 0, sizeof a);
+  if (mode == SMPLSIM_AMP_FILL_REF) {
+    why = amp_tables(*h->img.hdr(), tab, a);
+    if (!why.empty()) return fail(SMPLSIM_EINVAL, "smplsim_amp_obs: " + why);
+    if (!motion_ids_dev || !motion_t0_dev || !st->progress) return fail(SMPLSIM_EINVAL, "smplsim_amp_obs: FILL_REF needs motion_ids, motion_t0 and state.progress");
+  }
+  DeviceGuard guard(h->device);
+  amp_common(h, cfg, a);
+  a.ids = motion_ids_dev; a.t0 = motion_t0_dev; a.progress = st->progress; a.mask = mask_dev;
+  a.qpos = st->qpos; a.qvel = st->qvel; a.xpos = aux->xpos; a.xquat = aux->xquat; a.out = amp_obs_dev;
+  a.n = h->num_envs; a.mode = mode;
+  const int wpb = 8;
+  L_LAUNCH(k_amp_obs, (a.n + wpb - 1) / wpb, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a);
+  CUDA_TRY(cudaGetLastError());
+  return SMPLSIM_OK;
+}
+
+extern "C" int smplsim_amp_demo(SmplsimHandle* h, const SmplsimAmpCfg* cfg, const SmplsimAmpTables* tab, const int32_t* motion_ids_dev,
+                                const float* motion_times_dev, int n, float* out_dev, void* stream) {
+  int code;
+  std::string why = amp_check(h, cfg, &code);
+  if (!why.empty()) return fail(code, "smplsim_amp_demo: " + why);
+  if (n < 0) return fail(SMPLSIM_EINVAL, "smplsim_amp_demo: n < 0");
+  AmpArgs a; std::memset(&a, 0, sizeof a);
+  why = amp_tables(*h->img.hdr(), tab, a);
+  if (!why.empty()) return fail(SMPLSIM_EINVAL, "smplsim_amp_demo: " + why);
+  if (n == 0) return SMPLSIM_OK;
+  if (!motion_ids_dev || !motion_times_dev || !out_dev) return fail(SMPLSIM_EINVAL, "smplsim_amp_demo: null motion_ids / motion_times / output");
+  DeviceGuard guard(h->device);
+  amp_common(h, cfg, a);
+  a.ids = motion_ids_dev; a.t0 = motion_times_dev; a.out = out_dev; a.n = n; a.mode = AMP_DEMO;
+  const int wpb = 8;
+  L_LAUNCH(k_amp_obs, (n + wpb - 1) / wpb, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a);
   CUDA_TRY(cudaGetLastError());
   return SMPLSIM_OK;
 }

@@ -140,6 +140,57 @@ class MotionLibB200:
                                                   env._stream()))
         env.gpu_launches += 1
 
+    # ------------------------------------------------------------------ AMP demonstration rows (amp.py, csrc/amp_kernels.cuh)
+    def set_amp_cfg(self, amp_cfg=None):
+        """The AMP observation ``amp_obs_demo`` produces (keys of ``amp.AMP_DEFAULTS``; ``HumanoidAmpB200`` sets its own)."""
+        from .amp import amp_c_cfg, amp_config
+        self.amp_cfg = amp_config(amp_cfg)
+        self._amp_ccfg, self._amp_keys = amp_c_cfg(self.env.model, self.amp_cfg)
+
+    def _amp_tables(self):
+        from .abi import SmplsimAmpTablesC, SmplsimMotionTablesC
+        if getattr(self, "_amp_tab", None) is None:
+            t = self.tables
+            self._amp_mtab = SmplsimMotionTablesC(
+                xpos=t["xpos"].data_ptr(), xquat=t["xquat"].data_ptr(), body_vel=t["body_vel"].data_ptr(), body_ang_vel=t["body_ang_vel"].data_ptr(),
+                motion_len=self._motion_lengths.data_ptr(), num_frames=self._motion_num_frames.data_ptr(), motion_dt=self._motion_dt.data_ptr(),
+                length_starts=self.length_starts.data_ptr(), num_motions=self.num_motions(), nbody=t["xpos"].shape[1] // 3)
+            self._amp_tab = SmplsimAmpTablesC(motion=C.addressof(self._amp_mtab), dof_pos=t["dof_pos"].data_ptr(), dof_vel=t["dof_vel"].data_ptr())
+        return self._amp_tab
+
+    def amp_obs_demo(self, n=None, motion_ids=None, motion_times=None, out=None):
+        """Demonstration AMP observations ``[n, K, F]``: row i holds frames ``t_i - k dt`` (k = 0..K-1, dt the env's control period) of
+        clip ``motion_ids[i]``, the nearest-frame rows of the tables.  Either ``n`` (clips from ``sample_motions``, times from
+        ``sample_time(ids, truncate_time=(K-1) dt) + (K-1) dt``, so no frame lies before the clip's start) or ``motion_ids`` (int32) and
+        ``motion_times`` (float32), ``[n]`` tensors on the env's device.  One kernel launch; nothing is allocated when ``out`` (float32,
+        contiguous) is given along with ids and times of those dtypes."""
+        if getattr(self, "amp_cfg", None) is None:
+            self.set_amp_cfg()
+        env, K = self.env, int(self.amp_cfg["num_amp_obs_steps"])
+        if motion_ids is None:
+            if n is None:
+                raise ValueError("give n or motion_ids / motion_times")
+            motion_ids = self.sample_motions(int(n))
+            span = (K - 1) * env.dt
+            motion_times = self.sample_time(motion_ids, truncate_time=span) + span
+        elif motion_times is None:
+            raise ValueError("motion_ids needs motion_times")
+        ids = motion_ids.to(env.device, torch.int32).contiguous()
+        tm = motion_times.to(env.device, torch.float32).contiguous()
+        m = ids.shape[0]
+        if tm.shape != (m,) or ids.dim() != 1:
+            raise ValueError(f"motion_ids and motion_times must be [n] tensors of one length, got {tuple(ids.shape)} / {tuple(tm.shape)}")
+        L = env._L()
+        F = L.smplsim_amp_obs_dim(env._h, C.byref(self._amp_ccfg))
+        if out is None:
+            out = torch.empty(m, K, F, dtype=torch.float32, device=env.device)
+        elif tuple(out.shape) != (m, K, F) or out.dtype != torch.float32 or not out.is_contiguous():
+            raise ValueError(f"out must be a contiguous float32 tensor of shape {(m, K, F)}")
+        env._check(L.smplsim_amp_demo(env._h, C.byref(self._amp_ccfg), C.byref(self._amp_tables()), ids.data_ptr(), tm.data_ptr(), m,
+                                      out.data_ptr() if m else None, env._stream()))
+        env.gpu_launches += 1
+        return out
+
     def inverse_dynamics(self, contact_wrench: bool = False):
         """``env.inverse`` over every frame of the library: ``qfrc_inverse [total_frames, nv]`` (and ``contact_wrench [total_frames,
         nbody, 6]``), indexed like the tables.  ``qfrc_inverse[:, 0:6]`` is the root residual force of each frame.  ``qacc`` is the
