@@ -188,7 +188,7 @@ typedef struct SmplsimCamera {
 typedef struct SmplsimHandle SmplsimHandle;
 
 const char* smplsim_last_error(void);
-int smplsim_version(void);   /* 280 = this header (270: before smplsim_amp_obs / smplsim_amp_demo; 260: before smplsim_imitation; 250: before smplsim_set_env_params; 240: before smplsim_ray / smplsim_render; 230: before smplsim_dynamics; 220: before smplsim_inverse;
+int smplsim_version(void);   /* 290 = this header (280: before smplsim_motion_blend and the interpolation / future-target fields; 270: before smplsim_amp_obs / smplsim_amp_demo; 260: before smplsim_imitation; 250: before smplsim_set_env_params; 240: before smplsim_ray / smplsim_render; 230: before smplsim_dynamics; 220: before smplsim_inverse;
                               * 210: before SmplsimAux.contact_wrench; 200: before SmplsimState.xfrc_applied; 100: before pid_* state and aux.status) */
 
 /* MjModel.from_xml_string + MjData + setup_humanoid_properties/setup_controller
@@ -340,6 +340,34 @@ int smplsim_motion_gather(SmplsimHandle* h, const int32_t* motion_ids_dev, const
                           const int32_t* length_starts_dev, int num_tables, const float* const* tables_dev,
                           const int32_t* widths, float* const* outs_dev, int32_t* frame_idx_dev, void* cuda_stream);
 
+/* MotionLibBaseTorch.get_motion_state (smpl_sim/smpllib/motion_lib_base_torch.py:434-499): the state of clip id at time t blended
+ * from the two frames around t, for n query rows.  Arguments as smplsim_motion_gather, plus kinds[k] (host, one SMPLSIM_BLEND_* per
+ * table), offset_dev[n,3] (or NULL) and the optional outputs frame0_dev / frame1_dev[n] (table rows, length_starts included) and
+ * blend_dev[n].  Frame rule (_calc_frame_blend, :528-538), every operation one float32 rounding as torch on the CPU:
+ *     phase = clip(t / len, 0, 1);  t = max(t, 0)
+ *     f0 = (int)(phase * (nf - 1));  f1 = min(f0 + 1, nf - 1);  b = clip((t - f0 dt) / dt, 0, 1)
+ * Value kinds, v0 / v1 = the rows f0 / f1 of a table:
+ *     LERP   (1 - b) v0 + b v1                                        (dof_pos, dof_vel, body_vel, body_ang_vel)
+ *     POS    LERP, then + offset[i] on every 3-group                    (rg_pos)
+ *     SLERP  every 4-group slerped (width a multiple of 4)              (rb_rot)
+ *     QPOS   LERP, columns 3-6 slerped, + offset[i] on columns 0-2      (qpos: this project's extension, the reference returns none)
+ *     ROW0   row f0 as it is                                            (motion_aa)
+ * slerp is torch_utils.slerp (smpl_sim/utils/torch_utils.py:405-426) with its quirks: q1 negated when q0.q1 < 0; the midpoint
+ * 0.5 q0 + 0.5 q1 when |sin(half angle)| < 0.001, whatever b; q0 when cos(half angle) >= 1; the result is not normalised.  Blended qvel
+ * rows (LERP of the qvel table) are, like QPOS, this project's extension.  Quaternions are wxyz; the formula does not depend on the order.
+ * SMPLSIM_EINVAL: a null argument, more than 16 tables, an unknown kind, SLERP on a width that is not a multiple of 4, POS on one that is
+ * not a multiple of 3, QPOS on one below 7. */
+#define SMPLSIM_BLEND_LERP 0
+#define SMPLSIM_BLEND_POS 1
+#define SMPLSIM_BLEND_SLERP 2
+#define SMPLSIM_BLEND_QPOS 3
+#define SMPLSIM_BLEND_ROW0 4
+int smplsim_motion_blend(SmplsimHandle* h, const int32_t* motion_ids_dev, const float* motion_times_dev, int n,
+                         const float* motion_len_dev, const int32_t* num_frames_dev, const float* motion_dt_dev,
+                         const int32_t* length_starts_dev, int num_tables, const float* const* tables_dev,
+                         const int32_t* widths, const int32_t* kinds, const float* offset_dev, float* const* outs_dev,
+                         int32_t* frame0_dev, int32_t* frame1_dev, float* blend_dev, void* cuda_stream);
+
 /* Motion-imitation task: every env tracks one clip of a motion library.  One launch, run after smplsim_step / smplsim_reset on the same
  * stream, writes the env's observation row, reward, flags and position error; the stepper itself runs as SMPLSIM_TASK_NONE.  The
  * reference ships no imitation task in its MuJoCo env layer (SURVEY.md 3.4), so the definitions are this project's, after the published
@@ -372,7 +400,16 @@ int smplsim_motion_gather(SmplsimHandle* h, const int32_t* motion_ids_dev, const
  *                  to qpos0, so it is no longer on its clip; aux.status NULL: not consulted);
  *     truncated  = t0 + (p + 1) dt > motion_len[m] (no next target) or p > episode_length (strict, quirk Q7).
  * mpjpe = mean_B |p^_b - p_b| in metres.  frames (may be NULL) receives the two table rows used, [N,2] = (now, next).
- * The means and the maximum are reduced in a fixed order: the outputs are bit-reproducible. */
+ * The means and the maximum are reduced in a fixed order: the outputs are bit-reproducible.
+ *
+ * Options (appended fields; their zero values give the task above):
+ *   interpolate = 1: ref(t) is the state smplsim_motion_blend gives for (m, t) instead of one row: positions and velocities lerped,
+ *     rotations slerped between the frames f0 and f1 of its frame rule.  The slerped q^_b are not renormalised (the reference's
+ *     slerp); q * v is evaluated as v (2 w^2 - 1) + 2 w (u x v) + 2 u (u . v) with u = xyz(q), which is the rotation for unit q.  The observation's targets, the reward, mpjpe and the
+ *     termination distance all use it; frames then reports the rows f0 of now and next.  Truncation is unchanged.
+ *   num_future = T >= 2: T targets, target k = 0..T-1 at fmaf(k, future_dt, t0 + (p + 1) dt); the row is [self obs | T x 24 J], frame
+ *     major, each block the 24 J words above against the current simulated state.  T = 0 or 1: one target.  The row is then
+ *     self_obs_dim + 24 J T wide (smplsim_imitation_obs_dim gives the one-target width). */
 typedef struct SmplsimImitationCfg {
   float k_pos, k_rot, k_vel, k_angvel;   /* defaults of the `im` cfg group: 100, 10, 0.1, 0.1 */
   float w_pos, w_rot, w_vel, w_angvel;   /*                                 0.5, 0.3, 0.1, 0.1 */
@@ -381,6 +418,9 @@ typedef struct SmplsimImitationCfg {
   int32_t self_obs_dim;                  /* must be the handle's self-observation width (the head of a smplsim_step observation row) */
   int32_t num_tracked;                   /* J, in [1, nbody] */
   const int32_t* tracked_bodies;         /* host array [num_tracked] of robot body indices (0 = root), or NULL */
+  int32_t interpolate;                   /* 0: the nearest-frame rows; 1: blended reference states (see above) */
+  int32_t num_future;                    /* T >= 0 targets per observation (0 and 1: one) */
+  float future_dt;                       /* >= 0 seconds between targets (PHC: 1 / trajSampleTimestepInv) */
 } SmplsimImitationCfg;
 /* Device tables of a motion library (the layout smplsim_motion_gather takes), read in place. */
 typedef struct SmplsimMotionTables {
@@ -395,7 +435,8 @@ typedef struct SmplsimMotionTables {
   int32_t num_motions;
   int32_t nbody;              /* bodies per table row; must be the handle's */
 } SmplsimMotionTables;
-/* Width of the observation row smplsim_imitation writes for num_tracked bodies: self-observation width + 24 num_tracked. */
+/* Width of the observation row smplsim_imitation writes for num_tracked bodies and one target: self-observation width + 24 num_tracked
+ * (T targets: self-observation width + 24 num_tracked T). */
 int smplsim_imitation_obs_dim(const SmplsimHandle* h, int num_tracked);
 /* For the envs whose mask byte is non-zero (mask_dev NULL: all): obs_dev[N, smplsim_imitation_obs_dim] and frames_dev; unless obs_only
  * (the call after a reset) also reward_dev[N], terminated_dev[N], truncated_dev[N], mpjpe_dev[N].  obs_only != 0 leaves those four
@@ -403,7 +444,8 @@ int smplsim_imitation_obs_dim(const SmplsimHandle* h, int num_tracked);
  * aux: xpos, xquat, body_linvel, body_angvel are read (required), status if non-NULL.  Works on every handle kind (SMPL, SMPL-X,
  * per-env shapes, self-collision); reads no handle scratch and writes no env state, so the stepper's results do not depend on it.
  * SMPLSIM_EINVAL: a null argument, num_tracked outside [1, nbody], a tracked body outside [0, nbody), tracked_bodies NULL with
- * num_tracked != nbody, tab->nbody != the handle's, num_motions < 1, self_obs_dim != the handle's. */
+ * num_tracked != nbody, tab->nbody != the handle's, num_motions < 1, self_obs_dim != the handle's, interpolate not 0 / 1, num_future < 0,
+ * future_dt < 0 or NaN. */
 int smplsim_imitation(SmplsimHandle* h, const SmplsimImitationCfg* cfg, const SmplsimMotionTables* tab, const int32_t* motion_ids_dev,
                       const float* motion_t0_dev, const int32_t* progress_dev, const SmplsimAux* aux, const float* self_obs_dev,
                       const uint8_t* mask_dev, int obs_only, float* obs_dev, float* reward_dev, uint8_t* terminated_dev,
@@ -444,6 +486,8 @@ typedef struct SmplsimAmpCfg {
   const int32_t* key_bodies;     /* host array [num_key_bodies] of robot body indices (0 = root); may be NULL when num_key_bodies = 0 */
   int32_t local_root_obs;        /* 0/1 */
   int32_t root_height_obs;       /* 0/1 */
+  int32_t interpolate;           /* 0: ref(t) as above; 1: the blended state of smplsim_motion_blend (frames f0 / f1 of its rule: root_rot
+                                  * slerped, root_pos, key_pos, velocities and the dof_pos exp-map triples lerped), in FILL_REF and demo rows */
 } SmplsimAmpCfg;
 /* The tables of ref(t): a motion library (SmplsimMotionTables, read in place) plus its joint tables. */
 typedef struct SmplsimAmpTables {
@@ -457,7 +501,7 @@ int smplsim_amp_obs_dim(const SmplsimHandle* h, const SmplsimAmpCfg* cfg);
  * written.  st: qpos, qvel (and progress for FILL_REF) are read; aux: xpos, xquat.  FILL_REF also reads tab, motion_ids_dev[N] and
  * motion_t0_dev[N] (the clip and the clip time of step 0, as smplsim_imitation); the other modes ignore them (they may be NULL).
  * SMPLSIM_EINVAL: a null required pointer, num_steps < 1, a bad key body, tab->motion->nbody != the handle's, num_motions < 1, an
- * unknown mode. */
+ * unknown mode, interpolate not 0 / 1. */
 int smplsim_amp_obs(SmplsimHandle* h, const SmplsimAmpCfg* cfg, const SmplsimState* st, const SmplsimAux* aux, const SmplsimAmpTables* tab,
                     const int32_t* motion_ids_dev, const float* motion_t0_dev, const uint8_t* mask_dev, int mode, float* amp_obs_dev,
                     void* cuda_stream);

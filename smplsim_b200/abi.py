@@ -57,7 +57,8 @@ class SmplsimImitationCfgC(C.Structure):
     _fields_ = [("k_pos", C.c_float), ("k_rot", C.c_float), ("k_vel", C.c_float), ("k_angvel", C.c_float),
                 ("w_pos", C.c_float), ("w_rot", C.c_float), ("w_vel", C.c_float), ("w_angvel", C.c_float),
                 ("termination_distance", C.c_float), ("episode_length", C.c_int32), ("self_obs_dim", C.c_int32),
-                ("num_tracked", C.c_int32), ("tracked_bodies", C.c_void_p)]
+                ("num_tracked", C.c_int32), ("tracked_bodies", C.c_void_p), ("interpolate", C.c_int32), ("num_future", C.c_int32),
+                ("future_dt", C.c_float)]
 
 
 class SmplsimMotionTablesC(C.Structure):
@@ -68,7 +69,7 @@ class SmplsimMotionTablesC(C.Structure):
 
 class SmplsimAmpCfgC(C.Structure):
     _fields_ = [("num_steps", C.c_int32), ("num_key_bodies", C.c_int32), ("key_bodies", C.c_void_p), ("local_root_obs", C.c_int32),
-                ("root_height_obs", C.c_int32)]
+                ("root_height_obs", C.c_int32), ("interpolate", C.c_int32)]
 
 
 class SmplsimAmpTablesC(C.Structure):
@@ -76,6 +77,7 @@ class SmplsimAmpTablesC(C.Structure):
 
 
 AMP_PUSH, AMP_FILL, AMP_FILL_REF = 0, 1, 2     # SMPLSIM_AMP_* modes of smplsim_amp_obs
+BLEND_LERP, BLEND_POS, BLEND_SLERP, BLEND_QPOS, BLEND_ROW0 = 0, 1, 2, 3, 4   # SMPLSIM_BLEND_* value kinds of smplsim_motion_blend
 
 
 def _get(node: Any, key: str, default=None):

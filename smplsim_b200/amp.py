@@ -31,6 +31,7 @@ AMP_DEFAULTS: Dict[str, Any] = dict(
     local_root_obs=True,                                    # phc_prim_iccv.yaml:51  localRootObs
     root_height_obs=True,                                   # phc_prim_iccv.yaml:52  rootHeightObs
     key_bodies=["R_Ankle", "L_Ankle", "R_Wrist", "L_Wrist"],  # phc_prim_iccv.yaml:53  keyBodies
+    interpolate=False,                                      # this project's: demo / MoCap-reset frames blended as get_motion_state
     disc_units=[1024, 512],                                 # im.yaml:38  network.disc.units
     disc_activation="relu",                                 # im.yaml:39  network.disc.activation
     lr=2e-5,                                                # im.yaml:59  learning_rate
@@ -71,7 +72,8 @@ def amp_c_cfg(model, amp_cfg: Dict[str, Any]):
         keys.append(int(x))
     arr = np.ascontiguousarray(np.asarray(keys, dtype=np.int32))
     c = SmplsimAmpCfgC(num_steps=int(amp_cfg["num_amp_obs_steps"]), num_key_bodies=len(keys), key_bodies=arr.ctypes.data if keys else None,
-                       local_root_obs=int(bool(amp_cfg["local_root_obs"])), root_height_obs=int(bool(amp_cfg["root_height_obs"])))
+                       local_root_obs=int(bool(amp_cfg["local_root_obs"])), root_height_obs=int(bool(amp_cfg["root_height_obs"])),
+                       interpolate=int(bool(amp_cfg["interpolate"])))
     return c, arr
 
 
@@ -254,7 +256,8 @@ class HumanoidAmpB200:
         b = self.batch
         if b._aux.xpos is None or b._aux.xquat is None:
             raise ValueError("HumanoidAmpB200 needs the batch's body poses (HumanoidBatchB200(..., with_aux=True))")
-        self.cfg = amp_config(amp_cfg)
+        # an imitation env's frame rule carries over to its AMP frames unless the caller sets the key
+        self.cfg = amp_config(dict({"interpolate": env.interpolate} if self.imitation else {}, **(amp_cfg or {})))
         self.num_envs, self.num_actions, self.device = env.num_envs, env.num_actions, env.device
         self.dt, self.max_episode_length = env.dt, env.max_episode_length
         self._ccfg, self._keys = amp_c_cfg(b.model, self.cfg)

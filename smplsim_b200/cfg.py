@@ -56,7 +56,10 @@ ENV_GROUPS: Dict[str, Dict[str, Any]] = {
     # weights w over (position, rotation, velocity, angular velocity); tracked_bodies: body names or indices, None = all
     "im": dict(_ENV_COMMON, task="HumanoidIm", state_init="MoCap", self_obs_v=2, create_vel_sensors=True, contact_bodies=list(_FEET),
                im_k_pos=100.0, im_k_rot=10.0, im_k_vel=0.1, im_k_angvel=0.1, im_w_pos=0.5, im_w_rot=0.3, im_w_vel=0.1, im_w_angvel=0.1,
-               termination_distance=0.25, tracked_bodies=None),
+               termination_distance=0.25, tracked_bodies=None,
+               # blended reference states (get_motion_state) instead of nearest frames; future targets per observation, 1 / inv s apart
+               # (PHC: numTrajSamples, trajSampleTimestepInv)
+               im_interpolate=False, num_traj_samples=1, traj_sample_timestep_inv=30),
 }
 # robot group -- smpl_sim/data/cfg/robot/{smpl,smplx}_humanoid.yaml
 _ROBOT_COMMON = dict(

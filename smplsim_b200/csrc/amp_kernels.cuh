@@ -63,14 +63,40 @@ __device__ __forceinline__ void amp_frame(const LHdr& H, const AmpArgs& a, int l
   for (int k = lane; k < a.nkey; k += 32) st3(out + ok + 3 * k, qrot_ref(hq, ld3(bx + 3 * a.key[k]) - root));
 }
 
-// ref(t) of clip id into out: the row motion_frame picks (the gather's nearest-frame rule, no blending)
+// ref(t) of clip id into out.  INTERP = 0: the row motion_frame picks (the gather's nearest-frame rule, no blending).  INTERP = 1: the
+// state get_motion_state blends from the frames f0 / f1 of motion_blend_frames, with k_motion_blend's rules (root rotation slerped;
+// root and key-body positions, velocities and the dof_pos exp-map triples lerped).  The blended dof_pos, dof_vel and body positions
+// are staged in the warp's shared-memory slot and framed by the same amp_frame.
+#define AMP_STAGE (2 * 3 * (LM_MAXB - 1) + 3 * LM_MAXB)   // floats per warp: dof_pos, dof_vel, body positions
+template <int INTERP>
 __device__ __forceinline__ void amp_ref_frame(const LHdr& H, const AmpArgs& a, int lane, int id, float t, float* out) {
+  if (INTERP) {
+    __shared__ float stage[8][AMP_STAGE];   // 8 warps per CTA (the launches' size)
+    float* sd = stage[threadIdx.x >> 5];
+    const int nd = a.nv - 6;
+    float *sv = sd + nd, *sx = sd + 2 * nd;
+    const MBlend m = motion_blend_frames(a.mlen[id], a.mdt[id], a.nframes[id], t);
+    const size_t r0 = (size_t)(a.starts[id] + m.f0), r1 = (size_t)(a.starts[id] + m.f1);
+    __syncwarp();   // the previous frame's reads of the slot are done
+    for (int i = lane; i < nd; i += 32) {
+      sd[i] = mb_lerp(a.tdof[r0 * nd + i], a.tdof[r1 * nd + i], m.b);
+      sv[i] = mb_lerp(a.tdofv[r0 * nd + i], a.tdofv[r1 * nd + i], m.b);
+    }
+    for (int i = lane; i < 3 * a.nb; i += 32) sx[i] = mb_lerp(a.txpos[r0 * a.nb * 3 + i], a.txpos[r1 * a.nb * 3 + i], m.b);
+    __syncwarp();
+    amp_frame(H, a, lane, ld3(sx), mb_slerp(amp_ldq(a.txquat + r0 * a.nb * 4), amp_ldq(a.txquat + r1 * a.nb * 4), m.b),
+              mb_lerp3(ld3(a.tvel + r0 * a.nb * 3), ld3(a.tvel + r1 * a.nb * 3), m.b),
+              mb_lerp3(ld3(a.tangvel + r0 * a.nb * 3), ld3(a.tangvel + r1 * a.nb * 3), m.b), sd, sv, sx, out);
+    return;
+  }
   const size_t r = (size_t)(a.starts[id] + motion_frame(a.mlen[id], a.mdt[id], a.nframes[id], t));
   const float* bx = a.txpos + r * a.nb * 3;
   amp_frame(H, a, lane, ld3(bx), amp_ldq(a.txquat + r * a.nb * 4), ld3(a.tvel + r * a.nb * 3), ld3(a.tangvel + r * a.nb * 3),
             a.tdof + r * (a.nv - 6), a.tdofv + r * (a.nv - 6), bx, out);
 }
 
+// INTERP: library frames blended (SmplsimAmpCfg.interpolate); <0> reads the nearest frame
+template <int INTERP>
 __global__ void __launch_bounds__(256) k_amp_obs(const float* __restrict__ gimg, AmpArgs a) {
   const LHdr& H = *(const LHdr*)gimg;   // the heading rule (upright_start) is the same for every body shape of a handle
   const int lane = threadIdx.x & 31;
@@ -81,7 +107,7 @@ __global__ void __launch_bounds__(256) k_amp_obs(const float* __restrict__ gimg,
   if (a.mode == AMP_DEMO) {
     const int id = min(max(a.ids[e], 0), a.nmotion - 1);
     const float t = a.t0[e];
-    for (int k = 0; k < K; k++) amp_ref_frame(H, a, lane, id, fmaf(-(float)k, a.dt, t), row + (size_t)k * F);
+    for (int k = 0; k < K; k++) amp_ref_frame<INTERP>(H, a, lane, id, fmaf(-(float)k, a.dt, t), row + (size_t)k * F);
     return;
   }
   if (a.mode == AMP_PUSH) {
@@ -116,5 +142,5 @@ __global__ void __launch_bounds__(256) k_amp_obs(const float* __restrict__ gimg,
   // AMP_FILL_REF: the env's clip behind the current time, t0 + (p - k) dt as one fused multiply-add (the time rule of k_imitation)
   const int id = min(max(a.ids[e], 0), a.nmotion - 1);
   const int p = a.progress[e];
-  for (int k = 1; k < K; k++) amp_ref_frame(H, a, lane, id, fmaf((float)(p - k), a.dt, a.t0[e]), row + (size_t)k * F);
+  for (int k = 1; k < K; k++) amp_ref_frame<INTERP>(H, a, lane, id, fmaf((float)(p - k), a.dt, a.t0[e]), row + (size_t)k * F);
 }

@@ -84,6 +84,107 @@ __global__ void k_motion_gather(GatherArgs a) {
   }
 }
 
+// get_motion_state (the torch motion library, motion_lib_base_torch.py:434-499): two frames around t and a blend weight instead of
+// one frame.  Every operation is one float32 rounding, as torch computes it on the CPU: no contraction, correctly rounded division.
+#ifdef SMPLSIM_EMU
+// the host build of these sources (the tests' SIMT emulator): one rounding per call, the empty asm keeps the compiler from fusing a
+// product into a neighbouring add (nvcc never fuses the device intrinsics)
+static inline float mb_host_rn(float r) {
+#if defined(__x86_64__)
+  __asm__("" : "+x"(r));
+#else
+  volatile float v = r;
+  r = v;
+#endif
+  return r;
+}
+static inline float __fadd_rn(float a, float b) { return mb_host_rn(a + b); }
+static inline float __fsub_rn(float a, float b) { return mb_host_rn(a - b); }
+static inline float __fmul_rn(float a, float b) { return mb_host_rn(a * b); }
+static inline float __fdiv_rn(float a, float b) { return mb_host_rn(a / b); }
+static inline float __fsqrt_rn(float a) { return mb_host_rn(sqrtf(a)); }
+#endif
+struct MBlend { int f0, f1; float b; };
+__device__ __forceinline__ MBlend motion_blend_frames(float len, float dt, int nf, float t) {   // _calc_frame_blend (:528-538)
+  const float phase = fminf(fmaxf(__fdiv_rn(t, len), 0.f), 1.f);
+  if (t < 0.f) t = 0.f;
+  MBlend m;
+  m.f0 = (int)__fmul_rn(phase, (float)(nf - 1));
+  m.f1 = min(m.f0 + 1, nf - 1);
+  m.b = fminf(fmaxf(__fdiv_rn(__fsub_rn(t, __fmul_rn((float)m.f0, dt)), dt), 0.f), 1.f);
+  return m;
+}
+// (1 - b) v0 + b v1
+__device__ __forceinline__ float mb_lerp(float v0, float v1, float b) { return __fadd_rn(__fmul_rn(__fsub_rn(1.f, b), v0), __fmul_rn(b, v1)); }
+__device__ __forceinline__ V3 mb_lerp3(V3 p, V3 q, float b) { return v3(mb_lerp(p.x, q.x, b), mb_lerp(p.y, q.y, b), mb_lerp(p.z, q.z, b)); }
+// torch_utils.slerp (smpl_sim/utils/torch_utils.py:405-426) with its quirks: q1 flipped when the dot product is negative, the plain
+// midpoint when |sin(half angle)| < 0.001 whatever the blend, q0 when cos(half angle) >= 1, no normalisation.  Component order free.
+__device__ __forceinline__ Q4 mb_slerp(Q4 q0, Q4 q1, float t) {
+  float c = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(q0.w, q1.w), __fmul_rn(q0.x, q1.x)), __fmul_rn(q0.y, q1.y)), __fmul_rn(q0.z, q1.z));
+  if (c < 0.f) { q1.w = -q1.w; q1.x = -q1.x; q1.y = -q1.y; q1.z = -q1.z; c = -c; }
+  if (c >= 1.f) return q0;
+  const float s = __fsqrt_rn(__fsub_rn(1.f, __fmul_rn(c, c)));
+  float ra = 0.5f, rb = 0.5f;
+  if (!(fabsf(s) < 0.001f)) {
+    const float ht = acosf(c);
+    ra = __fdiv_rn(sinf(__fmul_rn(__fsub_rn(1.f, t), ht)), s); rb = __fdiv_rn(sinf(__fmul_rn(t, ht)), s);
+  }
+  Q4 r;
+  r.w = __fadd_rn(__fmul_rn(ra, q0.w), __fmul_rn(rb, q1.w)); r.x = __fadd_rn(__fmul_rn(ra, q0.x), __fmul_rn(rb, q1.x));
+  r.y = __fadd_rn(__fmul_rn(ra, q0.y), __fmul_rn(rb, q1.y)); r.z = __fadd_rn(__fmul_rn(ra, q0.z), __fmul_rn(rb, q1.z));
+  return r;
+}
+__device__ __forceinline__ Q4 mb_ldq(const float* p) { Q4 q; q.w = p[0]; q.x = p[1]; q.y = p[2]; q.z = p[3]; return q; }
+__device__ __forceinline__ void mb_stq(float* p, Q4 q) { p[0] = q.w; p[1] = q.x; p[2] = q.y; p[3] = q.z; }
+
+// smplsim_motion_blend: per table a value kind (SMPLSIM_BLEND_*, include/smplsim.h)
+#define MB_LERP 0
+#define MB_POS 1
+#define MB_SLERP 2
+#define MB_QPOS 3
+#define MB_ROW0 4
+struct BlendArgs {
+  GatherArgs g;   // frame_idx unused
+  int kinds[SM_MAXTABLES];
+  const float* offset;   // [n, 3] or NULL
+  int32_t *frame0, *frame1; float* blend;
+};
+// a warp per query row, lanes over a table's columns (SLERP: over its quaternions)
+__global__ void k_motion_blend(BlendArgs a) {
+  const int lane = threadIdx.x & 31;
+  const int i = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (i >= a.g.n) return;
+  const int id = a.g.ids[i];
+  const MBlend m = motion_blend_frames(a.g.mlen[id], a.g.mdt[id], a.g.nframes[id], a.g.times[i]);
+  const size_t r0 = (size_t)(m.f0 + a.g.starts[id]), r1 = (size_t)(m.f1 + a.g.starts[id]);
+  if (lane == 0) {
+    if (a.frame0) a.frame0[i] = (int32_t)r0;
+    if (a.frame1) a.frame1[i] = (int32_t)r1;
+    if (a.blend) a.blend[i] = m.b;
+  }
+  float ox = 0.f, oy = 0.f, oz = 0.f;
+  if (a.offset) { ox = a.offset[3 * i]; oy = a.offset[3 * i + 1]; oz = a.offset[3 * i + 2]; }
+  for (int k = 0; k < a.g.ntab; k++) {
+    const int w = a.g.widths[k], kind = a.kinds[k];
+    const float *s0 = a.g.tables[k] + r0 * w, *s1 = a.g.tables[k] + r1 * w;
+    float* dst = a.g.outs[k] + (size_t)i * w;
+    if (kind == MB_SLERP) {
+      for (int q = lane; q < w / 4; q += 32) mb_stq(dst + 4 * q, mb_slerp(mb_ldq(s0 + 4 * q), mb_ldq(s1 + 4 * q), m.b));
+      continue;
+    }
+    for (int j = lane; j < w; j += 32) {
+      if (kind == MB_ROW0) { dst[j] = s0[j]; continue; }
+      if (kind == MB_QPOS && j >= 3 && j < 7) {   // the root quaternion: one lane slerps all four
+        if (j == 3) mb_stq(dst + 3, mb_slerp(mb_ldq(s0 + 3), mb_ldq(s1 + 3), m.b));
+        continue;
+      }
+      float v = mb_lerp(s0[j], s1[j], m.b);
+      if (a.offset && (kind == MB_POS || (kind == MB_QPOS && j < 3))) v = __fadd_rn(v, j % 3 == 0 ? ox : j % 3 == 1 ? oy : oz);
+      dst[j] = v;
+    }
+  }
+}
+
 // GAE (SURVEY.md 8 f2): learning_utils.estimate_advantages:198-218 as a reverse scan per env column of the [T,N] rollout;
 // thread per env, coalesced across envs at every t.
 __global__ void k_gae(const float* __restrict__ rew, const float* __restrict__ not_done, const float* __restrict__ not_dead,

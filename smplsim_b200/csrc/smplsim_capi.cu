@@ -67,7 +67,7 @@ struct DeviceGuard {   // every entry point runs on the handle's device and rest
 };
 
 extern "C" const char* smplsim_last_error(void) { return g_err.c_str(); }
-extern "C" int smplsim_version(void) { return 280; }   // 280: smplsim_amp_obs / smplsim_amp_demo; 270: smplsim_imitation; 260: smplsim_set_env_params; 250: smplsim_ray / smplsim_render; 240: smplsim_dynamics; 230: smplsim_inverse; 220: SmplsimAux.contact_wrench; 210: SmplsimState.xfrc_applied; 200: lane-chain kernels (ABI structs of 110)
+extern "C" int smplsim_version(void) { return 290; }   // 290: smplsim_motion_blend, blended / future imitation targets, blended AMP frames; 280: smplsim_amp_obs / smplsim_amp_demo; 270: smplsim_imitation; 260: smplsim_set_env_params; 250: smplsim_ray / smplsim_render; 240: smplsim_dynamics; 230: smplsim_inverse; 220: SmplsimAux.contact_wrench; 210: SmplsimState.xfrc_applied; 200: lane-chain kernels (ABI structs of 110)
 
 template <class C>
 static size_t cta_smem(const SmplsimHandle* h, int wpb) { return (size_t)h->img.hdr()->bytes + 16 + (size_t)wpb * C::EPW * C::total * 4; }
@@ -638,6 +638,36 @@ extern "C" int smplsim_motion_gather(SmplsimHandle* h, const int32_t* motion_ids
   return SMPLSIM_OK;
 }
 
+extern "C" int smplsim_motion_blend(SmplsimHandle* h, const int32_t* motion_ids_dev, const float* motion_times_dev, int n,
+                                    const float* motion_len_dev, const int32_t* num_frames_dev, const float* motion_dt_dev,
+                                    const int32_t* length_starts_dev, int num_tables, const float* const* tables_dev,
+                                    const int32_t* widths, const int32_t* kinds, const float* offset_dev, float* const* outs_dev,
+                                    int32_t* frame0_dev, int32_t* frame1_dev, float* blend_dev, void* stream) {
+  if (!motion_ids_dev || !motion_times_dev || !motion_len_dev || !num_frames_dev || !motion_dt_dev || !length_starts_dev || n < 0)
+    return fail(SMPLSIM_EINVAL, "smplsim_motion_blend: null argument");
+  if (num_tables < 0 || num_tables > SM_MAXTABLES) return fail(SMPLSIM_EINVAL, "smplsim_motion_blend: at most 16 tables");
+  if (num_tables > 0 && (!tables_dev || !widths || !kinds || !outs_dev)) return fail(SMPLSIM_EINVAL, "smplsim_motion_blend: null table list");
+  for (int k = 0; k < num_tables; k++) {
+    const int w = widths[k], kd = kinds[k];
+    if (w < 0) return fail(SMPLSIM_EINVAL, "smplsim_motion_blend: negative width");
+    if (kd < SMPLSIM_BLEND_LERP || kd > SMPLSIM_BLEND_ROW0) return fail(SMPLSIM_EINVAL, "smplsim_motion_blend: unknown kind");
+    if (kd == SMPLSIM_BLEND_SLERP && w % 4) return fail(SMPLSIM_EINVAL, "smplsim_motion_blend: SLERP needs a width that is a multiple of 4");
+    if (kd == SMPLSIM_BLEND_POS && w % 3) return fail(SMPLSIM_EINVAL, "smplsim_motion_blend: POS needs a width that is a multiple of 3");
+    if (kd == SMPLSIM_BLEND_QPOS && w < 7) return fail(SMPLSIM_EINVAL, "smplsim_motion_blend: QPOS needs a width of at least 7");
+  }
+  if (n == 0) return SMPLSIM_OK;
+  DeviceGuard guard(h ? h->device : 0);
+  BlendArgs a; std::memset(&a, 0, sizeof a);
+  a.g.ids = motion_ids_dev; a.g.times = motion_times_dev; a.g.mlen = motion_len_dev; a.g.nframes = num_frames_dev; a.g.mdt = motion_dt_dev;
+  a.g.starts = length_starts_dev; a.g.n = n; a.g.ntab = num_tables;
+  for (int k = 0; k < num_tables; k++) { a.g.tables[k] = tables_dev[k]; a.g.outs[k] = outs_dev[k]; a.g.widths[k] = widths[k]; a.kinds[k] = kinds[k]; }
+  a.offset = offset_dev; a.frame0 = frame0_dev; a.frame1 = frame1_dev; a.blend = blend_dev;
+  const int wpb = 8;
+  L_LAUNCH(k_motion_blend, (n + wpb - 1) / wpb, 32 * wpb, 0, (cudaStream_t)stream, a);
+  CUDA_TRY(cudaGetLastError());
+  return SMPLSIM_OK;
+}
+
 extern "C" int smplsim_imitation_obs_dim(const SmplsimHandle* h, int num_tracked) {
   return h && num_tracked >= 0 ? h->img.hdr()->self_obs_dim + 24 * num_tracked : SMPLSIM_EINVAL;
 }
@@ -661,6 +691,9 @@ extern "C" int smplsim_imitation(SmplsimHandle* h, const SmplsimImitationCfg* cf
   if (!aux->xpos || !aux->xquat || !aux->body_linvel || !aux->body_angvel) return fail(SMPLSIM_EINVAL, "smplsim_imitation: aux needs xpos, xquat, body_linvel, body_angvel");
   if (!motion_ids_dev || !motion_t0_dev || !progress_dev || !self_obs_dev || !obs_dev) return fail(SMPLSIM_EINVAL, "smplsim_imitation: null argument");
   if (!obs_only && (!reward_dev || !terminated_dev || !truncated_dev || !mpjpe_dev)) return fail(SMPLSIM_EINVAL, "smplsim_imitation: null reward / flag / mpjpe output");
+  if (cfg->interpolate != 0 && cfg->interpolate != 1) return fail(SMPLSIM_EINVAL, "smplsim_imitation: interpolate must be 0 or 1");
+  if (cfg->num_future < 0) return fail(SMPLSIM_EINVAL, "smplsim_imitation: num_future < 0");
+  if (!(cfg->future_dt >= 0.f)) return fail(SMPLSIM_EINVAL, "smplsim_imitation: future_dt < 0 or NaN");
   DeviceGuard guard(h->device);
   ImArgs a; std::memset(&a, 0, sizeof a);
   a.txpos = tab->xpos; a.txquat = tab->xquat; a.tvel = tab->body_vel; a.tangvel = tab->body_ang_vel;
@@ -674,8 +707,16 @@ extern "C" int smplsim_imitation(SmplsimHandle* h, const SmplsimImitationCfg* cf
   a.term_dist = cfg->termination_distance; a.dt = (float)h->ctrl_dt; a.episode_length = cfg->episode_length;
   a.n = h->num_envs; a.nb = H.nb; a.J = cfg->num_tracked; a.self_dim = H.self_obs_dim; a.self_stride = H.obs_dim; a.obs_only = obs_only ? 1 : 0;
   for (int j = 0; j < a.J; j++) a.body[j] = (unsigned char)(cfg->tracked_bodies ? cfg->tracked_bodies[j] : j);
-  const int wpb = 8;
-  L_LAUNCH(k_imitation, (a.n + wpb - 1) / wpb, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a);
+  a.T = std::max(cfg->num_future, 1); a.future_dt = cfg->future_dt;
+  const int wpb = 8, grid = (a.n + wpb - 1) / wpb;
+  const bool multi = a.T > 1;
+  if (cfg->interpolate) {
+    if (multi) L_LAUNCH((k_imitation<1, 1>), grid, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a);
+    else L_LAUNCH((k_imitation<1, 0>), grid, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a);
+  } else {
+    if (multi) L_LAUNCH((k_imitation<0, 1>), grid, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a);
+    else L_LAUNCH((k_imitation<0, 0>), grid, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a);
+  }
   CUDA_TRY(cudaGetLastError());
   return SMPLSIM_OK;
 }
@@ -690,6 +731,7 @@ static std::string amp_check(const SmplsimHandle* h, const SmplsimAmpCfg* cfg, i
   if (!h || !cfg) return "null handle / cfg";
   const LHdr& H = *h->img.hdr();
   if (cfg->num_steps < 1) return "num_steps < 1";
+  if (cfg->interpolate != 0 && cfg->interpolate != 1) return "interpolate must be 0 or 1";
   if (cfg->num_key_bodies < 0 || cfg->num_key_bodies > H.nb) return "num_key_bodies outside [0, nbody]";
   if (cfg->num_key_bodies > 0 && !cfg->key_bodies) return "key_bodies NULL with num_key_bodies > 0";
   for (int k = 0; k < cfg->num_key_bodies; k++)
@@ -747,7 +789,8 @@ extern "C" int smplsim_amp_obs(SmplsimHandle* h, const SmplsimAmpCfg* cfg, const
   a.qpos = st->qpos; a.qvel = st->qvel; a.xpos = aux->xpos; a.xquat = aux->xquat; a.out = amp_obs_dev;
   a.n = h->num_envs; a.mode = mode;
   const int wpb = 8;
-  L_LAUNCH(k_amp_obs, (a.n + wpb - 1) / wpb, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a);
+  if (cfg->interpolate) L_LAUNCH(k_amp_obs<1>, (a.n + wpb - 1) / wpb, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a);
+  else L_LAUNCH(k_amp_obs<0>, (a.n + wpb - 1) / wpb, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a);
   CUDA_TRY(cudaGetLastError());
   return SMPLSIM_OK;
 }
@@ -767,7 +810,8 @@ extern "C" int smplsim_amp_demo(SmplsimHandle* h, const SmplsimAmpCfg* cfg, cons
   amp_common(h, cfg, a);
   a.ids = motion_ids_dev; a.t0 = motion_times_dev; a.out = out_dev; a.n = n; a.mode = AMP_DEMO;
   const int wpb = 8;
-  L_LAUNCH(k_amp_obs, (n + wpb - 1) / wpb, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a);
+  if (cfg->interpolate) L_LAUNCH(k_amp_obs<1>, (n + wpb - 1) / wpb, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a);
+  else L_LAUNCH(k_amp_obs<0>, (n + wpb - 1) / wpb, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a);
   CUDA_TRY(cudaGetLastError());
   return SMPLSIM_OK;
 }

@@ -25,7 +25,9 @@ class HumanoidImB200:
     the clip time at which each env's episode started), ``mpjpe`` (metres, of the last step) and ``ref_frames`` (the two table rows the
     last call used: now, next).
 
-    ``cfg``: ``make_cfg(env="im")`` (gains ``im_k_*``, weights ``im_w_*``, ``termination_distance``, ``tracked_bodies``, ``episode_length``).
+    ``cfg``: ``make_cfg(env="im")`` (gains ``im_k_*``, weights ``im_w_*``, ``termination_distance``, ``tracked_bodies``, ``episode_length``;
+    ``im_interpolate``: blended reference states instead of nearest frames, in the task and in the reset state; ``num_traj_samples`` targets
+    per observation, ``1 / traj_sample_timestep_inv`` seconds apart).
     ``motion``: the library's tables (the dict ``synthetic_tables`` / ``amass_tables`` return), or a callable ``batch -> tables`` (the
     synthetic tables need the batch's kinematics), or a ``MotionLibB200`` built on ``batch``.
     ``tracked_bodies``: body names or indices (default ``cfg.env.tracked_bodies``, None = all bodies).
@@ -59,17 +61,23 @@ class HumanoidImB200:
         self.tracked_bodies = bodies
         self._bodies = np.ascontiguousarray(np.asarray(bodies, dtype=np.int32))
         L = b._L()
+        self.interpolate = bool(e.get("im_interpolate", False))
+        self.num_future = int(e.get("num_traj_samples", 1))
+        inv = float(e.get("traj_sample_timestep_inv", 30))
+        if self.num_future < 1 or not inv > 0:
+            raise ValueError(f"num_traj_samples must be >= 1 and traj_sample_timestep_inv > 0, got {self.num_future} / {inv}")
         self._icfg = SmplsimImitationCfgC(
             k_pos=float(e.im_k_pos), k_rot=float(e.im_k_rot), k_vel=float(e.im_k_vel), k_angvel=float(e.im_k_angvel),
             w_pos=float(e.im_w_pos), w_rot=float(e.im_w_rot), w_vel=float(e.im_w_vel), w_angvel=float(e.im_w_angvel),
             termination_distance=float(e.termination_distance), episode_length=self.max_episode_length, self_obs_dim=int(b.num_obs),
-            num_tracked=len(bodies), tracked_bodies=self._bodies.ctypes.data if len(bodies) else None)
+            num_tracked=len(bodies), tracked_bodies=self._bodies.ctypes.data if len(bodies) else None, interpolate=int(self.interpolate),
+            num_future=self.num_future, future_dt=1.0 / inv)
         self._tab = SmplsimMotionTablesC(
             xpos=lib.tables["xpos"].data_ptr(), xquat=lib.tables["xquat"].data_ptr(), body_vel=lib.tables["body_vel"].data_ptr(),
             body_ang_vel=lib.tables["body_ang_vel"].data_ptr(), motion_len=lib._motion_lengths.data_ptr(),
             num_frames=lib._motion_num_frames.data_ptr(), motion_dt=lib._motion_dt.data_ptr(), length_starts=lib.length_starts.data_ptr(),
             num_motions=lib.num_motions(), nbody=lib.tables["xpos"].shape[1] // 3)
-        self.num_obs = L.smplsim_imitation_obs_dim(b._h, len(bodies))
+        self.num_obs = b.num_obs + (L.smplsim_imitation_obs_dim(b._h, len(bodies)) - b.num_obs) * self.num_future
         f32 = dict(dtype=torch.float32, device=dv)
         u8 = dict(dtype=torch.uint8, device=dv)
         self.obs_buf = torch.zeros(N, max(self.num_obs, 0), **f32)
@@ -158,7 +166,10 @@ class HumanoidImB200:
             torch.where(sel, ids, self.motion_ids, out=self.motion_ids)
             torch.where(sel, t0, self.motion_start_times, out=self.motion_start_times)
         self._ids64.copy_(self.motion_ids)
-        lib.gather_into(("qpos", "qvel"), self.motion_ids, self.motion_start_times, (self._qpos0, self._qvel0))
+        if self.interpolate:   # the blended state at t0, so the reset observation shows no frame lag
+            lib.blend_into(("qpos", "qvel"), self.motion_ids, self.motion_start_times, (self._qpos0, self._qvel0))
+        else:
+            lib.gather_into(("qpos", "qvel"), self.motion_ids, self.motion_start_times, (self._qpos0, self._qvel0))
         b.reset(mask, init_mode=2, qpos0=self._qpos0, qvel0=self._qvel0)
         self._task(mask, obs_only=True)
         self._keep = mask

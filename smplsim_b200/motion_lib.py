@@ -18,7 +18,9 @@ import torch
 from .batched import HumanoidBatchB200
 
 TABLE_KEYS = ("qpos", "qvel", "xpos", "xquat", "body_vel", "body_ang_vel", "dof_pos", "dof_vel")
-OPTIONAL_KEYS = ("motion_aa",)          # per-frame axis-angle pose of the source clip (motion_lib_base.py:340-354 returns it)
+OPTIONAL_KEYS = ("motion_aa",)
+# value kind of each table in get_motion_state / blend_into (abi.BLEND_*: 0 LERP, 1 POS, 2 SLERP, 3 QPOS, 4 ROW0); the rest are LERP
+BLEND_KINDS = {"xpos": 1, "xquat": 2, "qpos": 3, "motion_aa": 4}          # per-frame axis-angle pose of the source clip (motion_lib_base.py:340-354 returns it)
 
 
 def _gauss1d(x, sigma):
@@ -140,6 +142,52 @@ class MotionLibB200:
                                                   env._stream()))
         env.gpu_launches += 1
 
+    # ------------------------------------------------------------------ blended states (csrc/aux_kernels.cuh k_motion_blend)
+    def get_motion_state(self, motion_ids: torch.Tensor, motion_times: torch.Tensor, offset=None):
+        """``MotionLibBaseTorch.get_motion_state`` (motion_lib_base_torch.py:434-499): the state at ``motion_times`` blended from the two
+        frames around it, positions / velocities / joint angles lerped, body rotations slerped (the reference's slerp, unnormalised).
+        ``offset [n, 3]`` (or None) is added to every body position.  The reference's keys, plus ``qpos`` (root quaternion slerped,
+        offset on the root position) and ``qvel`` (lerped), this project's extension, and ``frame_idx0`` / ``frame_idx1`` (table rows)
+        and ``blend``.  One kernel launch."""
+        dv = self.env.device
+        ids = motion_ids.to(dv, torch.int32).contiguous()
+        tm = motion_times.to(dv, torch.float32).contiguous()
+        n = ids.shape[0]
+        off = None if offset is None else torch.as_tensor(offset, dtype=torch.float32, device=dv).reshape(n, 3).contiguous()
+        outs = {k: torch.empty(n, self.tables[k].shape[1], dtype=torch.float32, device=dv) for k in self._keys}
+        f0, f1 = torch.empty(n, dtype=torch.int32, device=dv), torch.empty(n, dtype=torch.int32, device=dv)
+        blend = torch.empty(n, dtype=torch.float32, device=dv)
+        self.blend_into(self._keys, ids, tm, [outs[k] for k in self._keys], offset=off, frame_idx0=f0, frame_idx1=f1, blend=blend)
+        nb = self.env.model.nbody
+        xpos, xquat = outs["xpos"].view(n, nb, 3), outs["xquat"].view(n, nb, 4)
+        bv, bav = outs["body_vel"].view(n, nb, 3), outs["body_ang_vel"].view(n, nb, 3)
+        return dict(root_pos=xpos[:, 0], root_rot=xquat[:, 0], dof_pos=outs["dof_pos"], root_vel=bv[:, 0], root_ang_vel=bav[:, 0],
+                    dof_vel=outs["dof_vel"], motion_aa=outs.get("motion_aa"), rg_pos=xpos, rb_rot=xquat, body_vel=bv, body_ang_vel=bav,
+                    motion_bodies=self._motion_bodies[ids.long()], qpos=outs["qpos"], qvel=outs["qvel"], frame_idx0=f0, frame_idx1=f1,
+                    blend=blend)
+
+    def blend_into(self, keys, motion_ids: torch.Tensor, motion_times: torch.Tensor, outs, offset=None, kinds=None, frame_idx0=None,
+                   frame_idx1=None, blend=None):
+        """The blend of ``get_motion_state`` for the tables ``keys`` only, into the caller's ``outs`` (one ``[n, width]`` float32 tensor per
+        key): nothing is allocated.  ``kinds``: one ``abi.BLEND_*`` per key (default ``BLEND_KINDS``: ``xpos`` POS, ``xquat`` SLERP,
+        ``qpos`` QPOS, ``motion_aa`` ROW0, the rest LERP).  ``motion_ids`` int32 / ``motion_times`` float32 / ``offset`` float32 ``[n, 3]``,
+        contiguous, on the env's device; ``frame_idx0`` / ``frame_idx1`` int32 and ``blend`` float32 ``[n]`` outputs, or None."""
+        env, n = self.env, motion_ids.shape[0]
+        keys = tuple(keys)
+        kinds = tuple(BLEND_KINDS.get(k, 0) for k in keys) if kinds is None else tuple(int(x) for x in kinds)
+        ck = ("blend", keys, kinds)
+        if ck not in self._ptrs:
+            self._ptrs[ck] = ((C.c_void_p * len(keys))(*[self.tables[k].data_ptr() for k in keys]),
+                              (C.c_int32 * len(keys))(*[self.tables[k].shape[1] for k in keys]), (C.c_int32 * len(keys))(*kinds))
+        tabs, widths, ckinds = self._ptrs[ck]
+        optr = (C.c_void_p * len(keys))(*[o.data_ptr() for o in outs])
+        p = lambda t: None if t is None else t.data_ptr()  # noqa: E731
+        env._check(env._L().smplsim_motion_blend(env._h, motion_ids.data_ptr(), motion_times.data_ptr(), n, self._motion_lengths.data_ptr(),
+                                                 self._motion_num_frames.data_ptr(), self._motion_dt.data_ptr(), self.length_starts.data_ptr(),
+                                                 len(keys), tabs, widths, ckinds, p(offset), optr, p(frame_idx0), p(frame_idx1), p(blend),
+                                                 env._stream()))
+        env.gpu_launches += 1
+
     # ------------------------------------------------------------------ AMP demonstration rows (amp.py, csrc/amp_kernels.cuh)
     def set_amp_cfg(self, amp_cfg=None):
         """The AMP observation ``amp_obs_demo`` produces (keys of ``amp.AMP_DEFAULTS``; ``HumanoidAmpB200`` sets its own)."""
@@ -160,7 +208,7 @@ class MotionLibB200:
 
     def amp_obs_demo(self, n=None, motion_ids=None, motion_times=None, out=None):
         """Demonstration AMP observations ``[n, K, F]``: row i holds frames ``t_i - k dt`` (k = 0..K-1, dt the env's control period) of
-        clip ``motion_ids[i]``, the nearest-frame rows of the tables.  Either ``n`` (clips from ``sample_motions``, times from
+        clip ``motion_ids[i]``, the nearest-frame rows of the tables (blended states with the AMP key ``interpolate``).  Either ``n`` (clips from ``sample_motions``, times from
         ``sample_time(ids, truncate_time=(K-1) dt) + (K-1) dt``, so no frame lies before the clip's start) or ``motion_ids`` (int32) and
         ``motion_times`` (float32), ``[n]`` tensors on the env's device.  One kernel launch; nothing is allocated when ``out`` (float32,
         contiguous) is given along with ids and times of those dtypes."""
