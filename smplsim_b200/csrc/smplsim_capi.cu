@@ -99,18 +99,23 @@ static int pick_wpb(SmplsimHandle* h) {
   h->wpb = best;
   h->smem = cta_smem<C>(h, best);
   h->env_words = C::total;
-  if (cudaFuncSetAttribute(k_step5<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem) != cudaSuccess) return -1;
-  if (cudaFuncSetAttribute(k_step5<typename C::WithXfrc>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem) != cudaSuccess) return -1;
-  if (cudaFuncSetAttribute(k_step5<typename C::WithXfrcPrm>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem) != cudaSuccess) return -1;
-  if (cudaFuncSetAttribute(k_reset5<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem) != cudaSuccess) return -1;
-  if (cudaFuncSetAttribute(k_reset5<typename C::WithPrm>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem) != cudaSuccess) return -1;
-  if (cudaFuncSetAttribute(k_kin5<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem) != cudaSuccess) return -1;
+  // The shared-memory cap is an attribute of the kernel for the whole process, not of this handle: raise it to the device's
+  // opt-in limit rather than to this handle's need, so that a handle created later with smaller CTAs (fewer envs) does not
+  // lower the cap under the launches of a live handle with larger ones.  The lane kernels declare no static __shared__ (their
+  // only shared memory is the dynamic l_smem4), so the whole opt-in limit is a legal dynamic cap for each of them.
+  const int cap = h->max_smem;
+  if (cudaFuncSetAttribute(k_step5<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap) != cudaSuccess) return -1;
+  if (cudaFuncSetAttribute(k_step5<typename C::WithXfrc>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap) != cudaSuccess) return -1;
+  if (cudaFuncSetAttribute(k_step5<typename C::WithXfrcPrm>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap) != cudaSuccess) return -1;
+  if (cudaFuncSetAttribute(k_reset5<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap) != cudaSuccess) return -1;
+  if (cudaFuncSetAttribute(k_reset5<typename C::WithPrm>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap) != cudaSuccess) return -1;
+  if (cudaFuncSetAttribute(k_kin5<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap) != cudaSuccess) return -1;
   if constexpr (!C::SELFCOL) {
-    if (cudaFuncSetAttribute(k_inverse5<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem) != cudaSuccess) return -1;
-    if (cudaFuncSetAttribute(k_inverse5<typename C::WithPrm>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem) != cudaSuccess) return -1;
+    if (cudaFuncSetAttribute(k_inverse5<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap) != cudaSuccess) return -1;
+    if (cudaFuncSetAttribute(k_inverse5<typename C::WithPrm>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap) != cudaSuccess) return -1;
   }
-  if (cudaFuncSetAttribute(k_dyn5<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem) != cudaSuccess) return -1;
-  if (cudaFuncSetAttribute(k_dyn5<typename C::WithPrm>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem) != cudaSuccess) return -1;
+  if (cudaFuncSetAttribute(k_dyn5<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap) != cudaSuccess) return -1;
+  if (cudaFuncSetAttribute(k_dyn5<typename C::WithPrm>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap) != cudaSuccess) return -1;
   return best;
 }
 
