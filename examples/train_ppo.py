@@ -7,6 +7,7 @@ smplsim_gae (advantages), PPOLearner (AgentPPO.update_params semantics, gradient
     python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.1 examples/train_ppo.py --env getup
     python examples/train_ppo.py --env im --num-envs 4096      # motion imitation (HumanoidImB200) on synthetic clips
     python examples/train_ppo.py --env im --amp                # ... plus the AMP style reward (HumanoidAmpB200, AMPLearner)
+    python examples/train_ppo.py --env im --eval-every 5 --auto-pmcp hard   # score every clip every 5 epochs, train on the failed ones
 
 ``--horizon x --num-envs`` plays the role of ``learning.min_batch_size`` (51 200 in the reference yaml = 4096 envs x 12.5 steps)."""
 import argparse
@@ -33,7 +34,12 @@ def main():
     ap.add_argument("--units", type=int, nargs="+", default=[2048, 1536, 1024, 1024, 512, 512])   # data/cfg/learning/simple_mlp.yaml
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--amp", action="store_true", help="adversarial motion priors: discriminator reward mixed into the task reward")
+    ap.add_argument("--eval-every", type=int, default=0, help="--env im: evaluate the mean policy on every clip every E epochs (0: never)")
+    ap.add_argument("--auto-pmcp", default="off", choices=["off", "hard", "soft"],
+                    help="after each evaluation, sample training clips from the failed ones (the reference's auto_pmcp / auto_pmcp_soft)")
     a = ap.parse_args()
+    if (a.eval_every or a.auto_pmcp != "off") and (a.env != "im" or a.amp):
+        ap.error("--eval-every / --auto-pmcp need --env im without --amp")
     rank, world, local = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("LOCAL_RANK", 0))
     torch.cuda.set_device(local)
     dev = f"cuda:{local}"
@@ -80,6 +86,20 @@ def main():
             if amp_learner is not None:
                 print(f"  amp: task reward {float(env.extras['task_rew_buf'].mean()):.4f}  disc reward {float(env.disc_rew_buf.mean()):.4f}  "
                       f"disc_loss {info['disc_loss']:.4f}  acc agent {info['disc_agent_acc']:.3f} demo {info['disc_demo_acc']:.3f}", flush=True)
+        if a.eval_every and (ep + 1) % a.eval_every == 0:
+            with torch.no_grad():
+                policy.eval()
+                res = env.evaluate(lambda obs: policy.select_action(torch.clamp(obs, -5.0, 5.0), mean_action=True))
+            sampler.restart()                         # evaluate left every env flagged for reset
+            if a.auto_pmcp == "hard":
+                env.lib.update_hard_sampling_weight(res.failed_keys)
+            elif a.auto_pmcp == "soft":
+                env.lib.update_soft_sampling_weight(res.failed_keys)
+            if rank == 0:
+                s = res.summary()
+                print(f"  eval: {s['num_clips']} clips, {s['frames']} frames, success {s['success_rate']:.3f}, failed clips "
+                      f"{len(res.failed_keys)}  mpjpe_g {s['mpjpe_g']:.1f} mm  mpjpe_l {s['mpjpe_l']:.1f} mm  mpjpe_pa {s['mpjpe_pa']:.1f} mm  "
+                      f"vel {s['vel_dist']:.2f}  accel {s['accel_dist']:.2f}  rot {s['rot_error']:.3f} rad  (pmcp: {a.auto_pmcp})", flush=True)
     if world > 1:
         torch.distributed.destroy_process_group()
 

@@ -188,7 +188,7 @@ typedef struct SmplsimCamera {
 typedef struct SmplsimHandle SmplsimHandle;
 
 const char* smplsim_last_error(void);
-int smplsim_version(void);   /* 290 = this header (280: before smplsim_motion_blend and the interpolation / future-target fields; 270: before smplsim_amp_obs / smplsim_amp_demo; 260: before smplsim_imitation; 250: before smplsim_set_env_params; 240: before smplsim_ray / smplsim_render; 230: before smplsim_dynamics; 220: before smplsim_inverse;
+int smplsim_version(void);   /* 300 = this header (290: before smplsim_track_eval; 280: before smplsim_motion_blend and the interpolation / future-target fields; 270: before smplsim_amp_obs / smplsim_amp_demo; 260: before smplsim_imitation; 250: before smplsim_set_env_params; 240: before smplsim_ray / smplsim_render; 230: before smplsim_dynamics; 220: before smplsim_inverse;
                               * 210: before SmplsimAux.contact_wrench; 200: before SmplsimState.xfrc_applied; 100: before pid_* state and aux.status) */
 
 /* MjModel.from_xml_string + MjData + setup_humanoid_properties/setup_controller
@@ -450,6 +450,63 @@ int smplsim_imitation(SmplsimHandle* h, const SmplsimImitationCfg* cfg, const Sm
                       const float* motion_t0_dev, const int32_t* progress_dev, const SmplsimAux* aux, const float* self_obs_dev,
                       const uint8_t* mask_dev, int obs_only, float* obs_dev, float* reward_dev, uint8_t* terminated_dev,
                       uint8_t* truncated_dev, float* mpjpe_dev, int32_t* frames_dev, void* cuda_stream);
+
+/* Tracking evaluation: the per-frame metrics of the reference's smpl_eval (smpl_sim/smpllib/smpl_eval.py: compute_metrics_lite,
+ * compute_metrics_obj, p_mpjpe, compute_error_vel, compute_error_accel) for every env that tracks a clip, accumulated per env in one
+ * launch after each step's smplsim_imitation.  The reference scores recorded trajectories after the fact; here nothing but a [2, J, 3]
+ * difference history per env is kept.
+ *
+ * Eval bodies B = cfg->bodies (J = num_bodies >= 3 entries, NULL: all nbody bodies in order).  The root is the first eval body, B[0]
+ * (the reference's root_idx = 0); with a list that does not start at body 0, "root-relative" means relative to body B[0].
+ * Scored frame: the pair (the post-step state after step p, ref(t0 + p dt)) for p = progress[e], where ref is the reference pose
+ * smplsim_imitation's reward compares -- the same frame rule, nearest row or (interpolate = 1) the blended state -- and dt =
+ * cfg->dt, or the handle's control period (smplsim_imitation's) when cfg->dt = 0.  A caller runs it after every step from p = 1 on:
+ * the reset state (p = 0) is not scored.  Simulated poses: y_b = aux.xpos, q_b = aux.xquat; reference: x_b, q^_b.  Per scored frame,
+ * the f-th since the env's state was cleared (f = 0, 1, ...), with d_j = y_j - x_j and means over j in B:
+ *     mpjpe_g     mean |d_j|                                                           mm (x 1000, as the reference)
+ *     mpjpe_l     mean |(y_j - y_root) - (x_j - x_root)|                               mm
+ *     mpjpe_pa    p_mpjpe of the root-relative points: with x0 / y0 the points centred on their means, the proper rotation Q and scale
+ *                 s = lam / sum |y0|^2 maximising lam = sum x0 . Q y0 (the reference's sign_detR correction: never a reflection),
+ *                 mean |s Q y0_j - x0_j|; s = 0 when every y0 is zero (the reference divides by zero)   mm
+ *     vel_dist    mean |d_j^f - d_j^(f-1)|, f >= 1 only (compute_error_vel)            mm per frame
+ *     accel_dist  mean |d_j^f - 2 d_j^(f-1) + d_j^(f-2)|, f >= 2 only (compute_error_accel; not divided by dt)   mm per frame^2
+ *     rot_error   mean of th_j = 2 atan2(|xyz|, |w|) of q^_j (x) q_j^-1 (the rotvec norm of compute_metrics_obj; that function takes
+ *                 xyzw quaternions, these are wxyz)                                     rad
+ * Per env e with active[e] != 0 (the others are not read or written, frame_metrics rows included):
+ *     frame_metrics[e] (if non-NULL) = this frame's six values in the order above, NaN where undefined (vel f = 0, accel f <= 1);
+ *     sums[e, i] += value i (fp64) when defined; frames[e] = f + 1; prev_diff[e, f % 2] = d^f (slot f % 2 held d^(f-2));
+ *     if terminated[e] or truncated[e] (this step's flags, e.g. smplsim_imitation's): scoring ends with this frame, which is scored:
+ *     active[e] = 0, success[e] = truncated[e] && !terminated[e] (both set: failed).
+ * A clip's value of metric i is sums[e, i] / count_i with counts frames, frames, frames, frames - 1, frames - 2, frames; over a set of
+ * clips the frame-weighted mean (sum of sums / sum of counts) is compute_metrics_lite(..., concatenate=True)[k].mean().
+ * To start an env, the caller sets active = 1 and zeroes frames, sums and success (prev_diff needs no clearing).  Sums are lane partials in
+ * body-list order and an xor butterfly: the outputs are bit-reproducible.  Works on every handle kind; reads and writes no stepper state.
+ * SMPLSIM_EINVAL: a null argument or state array (frame_metrics may be NULL), num_bodies outside [3, nbody], an eval body outside
+ * [0, nbody), bodies NULL with num_bodies != nbody, tab->nbody != the handle's, num_motions < 1, interpolate not 0 / 1, dt < 0 or NaN. */
+#define SMPLSIM_TRACK_NMETRIC 6
+#define SMPLSIM_TRACK_MPJPE_G 0
+#define SMPLSIM_TRACK_MPJPE_L 1
+#define SMPLSIM_TRACK_MPJPE_PA 2
+#define SMPLSIM_TRACK_VEL_DIST 3
+#define SMPLSIM_TRACK_ACCEL_DIST 4
+#define SMPLSIM_TRACK_ROT_ERROR 5
+typedef struct SmplsimTrackEvalCfg {
+  int32_t num_bodies;            /* J in [3, nbody] (the Procrustes fit needs three points) */
+  const int32_t* bodies;         /* host array [num_bodies] of robot body indices (0 = root), or NULL */
+  int32_t interpolate;           /* 0: nearest-frame rows; 1: blended reference states (SmplsimImitationCfg.interpolate) */
+  float dt;                      /* seconds per step of the frame rule; 0: the handle's control period */
+} SmplsimTrackEvalCfg;
+typedef struct SmplsimTrackEvalState {
+  uint8_t* active;               /* [N]  1: scored this call */
+  float* prev_diff;              /* [N, 2, J, 3]  d of the last two scored frames */
+  int32_t* frames;               /* [N]  frames scored */
+  double* sums;                  /* [N, 6]  per-metric sums over the frames that define them */
+  uint8_t* success;              /* [N]  set when scoring ends by truncation alone */
+  float* frame_metrics;          /* [N, 6] or NULL: this call's values */
+} SmplsimTrackEvalState;
+int smplsim_track_eval(SmplsimHandle* h, const SmplsimTrackEvalCfg* cfg, const SmplsimMotionTables* tab, const int32_t* motion_ids_dev,
+                       const float* motion_t0_dev, const int32_t* progress_dev, const SmplsimAux* aux, const uint8_t* terminated_dev,
+                       const uint8_t* truncated_dev, const SmplsimTrackEvalState* state, void* cuda_stream);
 
 /* Adversarial motion priors (AMP): the discriminator's observation of an env's last K control steps and of a motion library's clips.
  * The per-frame feature is the reference's compute_humanoid_observations_smpl with has_smpl_params = False (smpl_sim/envs/nv/humanoid.py:

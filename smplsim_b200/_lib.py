@@ -65,6 +65,8 @@ _SYMBOLS = {
     "smplsim_imitation_obs_dim": (C.c_int, [C.c_void_p, C.c_int]),
     "smplsim_imitation": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                     C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "smplsim_track_eval": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                     C.c_void_p, C.c_void_p, C.c_void_p]),
     "smplsim_amp_obs_dim": (C.c_int, [C.c_void_p, C.c_void_p]),
     "smplsim_amp_obs": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                   C.c_void_p, C.c_void_p]),

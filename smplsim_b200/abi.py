@@ -67,6 +67,19 @@ class SmplsimMotionTablesC(C.Structure):
                 ("num_motions", C.c_int32), ("nbody", C.c_int32)]
 
 
+class SmplsimTrackEvalCfgC(C.Structure):
+    _fields_ = [("num_bodies", C.c_int32), ("bodies", C.c_void_p), ("interpolate", C.c_int32), ("dt", C.c_float)]
+
+
+class SmplsimTrackEvalStateC(C.Structure):
+    _fields_ = [("active", C.c_void_p), ("prev_diff", C.c_void_p), ("frames", C.c_void_p), ("sums", C.c_void_p), ("success", C.c_void_p),
+                ("frame_metrics", C.c_void_p)]
+
+
+# SMPLSIM_TRACK_* columns of SmplsimTrackEvalState.sums / frame_metrics
+TRACK_METRICS = ("mpjpe_g", "mpjpe_l", "mpjpe_pa", "vel_dist", "accel_dist", "rot_error")
+
+
 class SmplsimAmpCfgC(C.Structure):
     _fields_ = [("num_steps", C.c_int32), ("num_key_bodies", C.c_int32), ("key_bodies", C.c_void_p), ("local_root_obs", C.c_int32),
                 ("root_height_obs", C.c_int32), ("interpolate", C.c_int32)]

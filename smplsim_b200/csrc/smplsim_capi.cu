@@ -13,6 +13,7 @@
 
 #include "aux_kernels.cuh"
 #include "imitation_kernels.cuh"
+#include "track_eval_kernels.cuh"
 #include "amp_kernels.cuh"
 #include "render_kernels.cuh"
 
@@ -67,7 +68,7 @@ struct DeviceGuard {   // every entry point runs on the handle's device and rest
 };
 
 extern "C" const char* smplsim_last_error(void) { return g_err.c_str(); }
-extern "C" int smplsim_version(void) { return 290; }   // 290: smplsim_motion_blend, blended / future imitation targets, blended AMP frames; 280: smplsim_amp_obs / smplsim_amp_demo; 270: smplsim_imitation; 260: smplsim_set_env_params; 250: smplsim_ray / smplsim_render; 240: smplsim_dynamics; 230: smplsim_inverse; 220: SmplsimAux.contact_wrench; 210: SmplsimState.xfrc_applied; 200: lane-chain kernels (ABI structs of 110)
+extern "C" int smplsim_version(void) { return 300; }   // 300: smplsim_track_eval; 290: smplsim_motion_blend, blended / future imitation targets, blended AMP frames; 280: smplsim_amp_obs / smplsim_amp_demo; 270: smplsim_imitation; 260: smplsim_set_env_params; 250: smplsim_ray / smplsim_render; 240: smplsim_dynamics; 230: smplsim_inverse; 220: SmplsimAux.contact_wrench; 210: SmplsimState.xfrc_applied; 200: lane-chain kernels (ABI structs of 110)
 
 template <class C>
 static size_t cta_smem(const SmplsimHandle* h, int wpb) { return (size_t)h->img.hdr()->bytes + 16 + (size_t)wpb * C::EPW * C::total * 4; }
@@ -722,6 +723,47 @@ extern "C" int smplsim_imitation(SmplsimHandle* h, const SmplsimImitationCfg* cf
     if (multi) L_LAUNCH((k_imitation<0, 1>), grid, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a);
     else L_LAUNCH((k_imitation<0, 0>), grid, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a);
   }
+  CUDA_TRY(cudaGetLastError());
+  return SMPLSIM_OK;
+}
+
+// ------------------------------------------------------------------ tracking evaluation (track_eval_kernels.cuh)
+extern "C" int smplsim_track_eval(SmplsimHandle* h, const SmplsimTrackEvalCfg* cfg, const SmplsimMotionTables* tab, const int32_t* motion_ids_dev,
+                                  const float* motion_t0_dev, const int32_t* progress_dev, const SmplsimAux* aux, const uint8_t* terminated_dev,
+                                  const uint8_t* truncated_dev, const SmplsimTrackEvalState* state, void* stream) {
+  if (!h || !cfg || !tab || !aux || !state) return fail(SMPLSIM_EINVAL, "smplsim_track_eval: null handle / cfg / tables / aux / state");
+  const LHdr& H = *h->img.hdr();
+  if (cfg->num_bodies < 3 || cfg->num_bodies > H.nb) return fail(SMPLSIM_EINVAL, "smplsim_track_eval: num_bodies outside [3, nbody]");
+  if (!cfg->bodies && cfg->num_bodies != H.nb) return fail(SMPLSIM_EINVAL, "smplsim_track_eval: bodies NULL needs num_bodies == nbody");
+  if (cfg->bodies)
+    for (int j = 0; j < cfg->num_bodies; j++)
+      if (cfg->bodies[j] < 0 || cfg->bodies[j] >= H.nb) return fail(SMPLSIM_EINVAL, "smplsim_track_eval: eval body out of range [0, nbody)");
+  if (tab->nbody != H.nb) return fail(SMPLSIM_EINVAL, "smplsim_track_eval: the tables' nbody is not the handle's");
+  if (tab->num_motions < 1) return fail(SMPLSIM_EINVAL, "smplsim_track_eval: num_motions < 1");
+  if (!tab->xpos || !tab->xquat || !tab->body_vel || !tab->body_ang_vel || !tab->motion_len || !tab->num_frames || !tab->motion_dt || !tab->length_starts)
+    return fail(SMPLSIM_EINVAL, "smplsim_track_eval: null motion table");
+  if (!aux->xpos || !aux->xquat) return fail(SMPLSIM_EINVAL, "smplsim_track_eval: aux needs xpos, xquat");
+  if (!motion_ids_dev || !motion_t0_dev || !progress_dev || !terminated_dev || !truncated_dev) return fail(SMPLSIM_EINVAL, "smplsim_track_eval: null argument");
+  if (!state->active || !state->prev_diff || !state->frames || !state->sums || !state->success)
+    return fail(SMPLSIM_EINVAL, "smplsim_track_eval: null state array");
+  if (cfg->interpolate != 0 && cfg->interpolate != 1) return fail(SMPLSIM_EINVAL, "smplsim_track_eval: interpolate must be 0 or 1");
+  if (!(cfg->dt >= 0.f)) return fail(SMPLSIM_EINVAL, "smplsim_track_eval: dt < 0 or NaN");
+  DeviceGuard guard(h->device);
+  TeArgs t; std::memset(&t, 0, sizeof t);
+  ImArgs& a = t.im;
+  a.txpos = tab->xpos; a.txquat = tab->xquat; a.tvel = tab->body_vel; a.tangvel = tab->body_ang_vel;
+  a.mlen = tab->motion_len; a.nframes = tab->num_frames; a.mdt = tab->motion_dt; a.starts = tab->length_starts; a.nmotion = tab->num_motions;
+  a.ids = motion_ids_dev; a.t0 = motion_t0_dev; a.progress = progress_dev;
+  a.xpos = aux->xpos; a.xquat = aux->xquat;
+  a.dt = cfg->dt > 0.f ? cfg->dt : (float)h->ctrl_dt;
+  a.n = h->num_envs; a.nb = H.nb; a.J = cfg->num_bodies;
+  for (int j = 0; j < a.J; j++) a.body[j] = (unsigned char)(cfg->bodies ? cfg->bodies[j] : j);
+  t.terminated = terminated_dev; t.truncated = truncated_dev;
+  t.active = state->active; t.prev_diff = state->prev_diff; t.frames = state->frames; t.sums = state->sums; t.success = state->success;
+  t.frame_metrics = state->frame_metrics;
+  const int wpb = 8, grid = (a.n + wpb - 1) / wpb;
+  if (cfg->interpolate) L_LAUNCH(k_track_eval<1>, grid, 32 * wpb, 0, (cudaStream_t)stream, t);
+  else L_LAUNCH(k_track_eval<0>, grid, 32 * wpb, 0, (cudaStream_t)stream, t);
   CUDA_TRY(cudaGetLastError());
   return SMPLSIM_OK;
 }

@@ -4,16 +4,20 @@
 CUDA kernel per call (``smplsim_imitation``, csrc/imitation_kernels.cuh) that reads the library's tables in place: tracking
 observation, reward, early termination, truncation at the clip's end and the mean per-joint position error.  The definitions are
 stated in include/smplsim.h and DESIGN.md 2; the reference ships no imitation task in its MuJoCo env layer (SURVEY.md 3.4), they
-follow the published PHC formulation.  Envs that finish are put back on a reference frame of a newly drawn clip (MoCap init)."""
+follow the published PHC formulation.  Envs that finish are put back on a reference frame of a newly drawn clip (MoCap init).
+``HumanoidImB200.evaluate`` scores a policy on every clip of the library with the reference's smpl_eval metrics (``smplsim_track_eval``,
+csrc/track_eval_kernels.cuh) and reports the failed clips that PMCP sampling takes."""
 from __future__ import annotations
 
 import ctypes as C
-from typing import Any, Callable, Optional, Sequence, Union
+import math
+from dataclasses import dataclass
+from typing import Any, Callable, Dict, List, Optional, Sequence, Union
 
 import numpy as np
 import torch
 
-from .abi import SmplsimImitationCfgC, SmplsimMotionTablesC
+from .abi import TRACK_METRICS, SmplsimImitationCfgC, SmplsimMotionTablesC, SmplsimTrackEvalCfgC, SmplsimTrackEvalStateC
 from .batched import HumanoidBatchB200, _ptr
 from .motion_lib import MotionLibB200
 
@@ -116,9 +120,9 @@ class HumanoidImB200:
     def gpu_launches(self) -> int:
         return self.batch.gpu_launches
 
-    def _task(self, mask: Optional[torch.Tensor], obs_only: bool):
+    def _task(self, mask: Optional[torch.Tensor], obs_only: bool, icfg: Optional[SmplsimImitationCfgC] = None):
         b = self.batch
-        b._check(b._L().smplsim_imitation(b._h, C.byref(self._icfg), C.byref(self._tab), _ptr(self.motion_ids), _ptr(self.motion_start_times),
+        b._check(b._L().smplsim_imitation(b._h, C.byref(self._icfg if icfg is None else icfg), C.byref(self._tab), _ptr(self.motion_ids), _ptr(self.motion_start_times),
                                           _ptr(b.progress_buf), C.byref(b._aux), _ptr(b.obs_buf), _ptr(mask), int(obs_only),
                                           _ptr(self.obs_buf), _ptr(self.rew_buf), _ptr(self.terminate_buf), _ptr(self.truncate_buf),
                                           _ptr(self.mpjpe), _ptr(self.ref_frames), b._stream()))
@@ -183,3 +187,134 @@ class HumanoidImB200:
         """Early terminations per clip since construction (float64 ``[num_motions]``), the argument of
         ``MotionLibB200.update_sampling_prob``: clips that fail more are drawn more (PMCP).  ``clip_episodes`` holds the episode counts."""
         return self.clip_terminations.clone()
+
+    # ------------------------------------------------------------------ evaluation (csrc/track_eval_kernels.cuh)
+    def clip_steps(self, motion_ids: Optional[Sequence[int]] = None) -> np.ndarray:
+        """Steps an episode started at clip time 0 runs before truncation ends it at the clip's end: the first p >= 1 with
+        t0 + (p + 1) dt > motion_len in float32 (the task kernel's rule, one rounding), from the host copy of the clip lengths."""
+        lens = self.lib._motion_lengths.cpu().numpy()
+        ids = np.arange(len(lens)) if motion_ids is None else np.asarray(motion_ids, dtype=np.int64)
+        dt = np.float64(np.float32(self.dt))
+        out = np.empty(len(ids), dtype=np.int64)
+        for i, m in enumerate(ids):
+            L = lens[m]
+            p = max(1, int(L / dt) - 2)
+            while np.float32((p + 1) * dt) <= L:
+                p += 1
+            out[i] = p
+        return out
+
+    def evaluate(self, policy: Callable[[torch.Tensor], torch.Tensor], motion_ids: Optional[Sequence[int]] = None,
+                 termination_distance: Optional[float] = None, eval_bodies: Optional[Sequence] = None) -> "TrackingEval":
+        """Run ``policy(obs) -> actions`` (clipped to [-1, 1], as ``BatchedSampler`` does; called under ``torch.no_grad``) on every clip of
+        ``motion_ids`` (default: the whole library) from clip time 0 to its end, and score it with the metrics of the reference's
+        smpl_eval (include/smplsim.h, smplsim_track_eval).  Clips go to envs in waves of ``num_envs``: one masked ``reset`` per wave, then
+        a step count fixed up front from the host copy of the clip lengths (``clip_steps``), each step the physics step, the task kernel
+        and the evaluation kernel, with no host sync.  A clip fails when it terminates early (``termination_distance``, default the cfg's)
+        and succeeds when it reaches its end; the episode length is raised to the longest clip for the call.
+        ``eval_bodies``: names or indices, at least 3, the first is the root (default: all bodies).
+
+        Training state is left alone: ``clip_episodes`` / ``clip_terminations`` and the sampling weights do not change.  The env's
+        buffers (observation, reward, flags, clips, start times) hold the last evaluation step, and ``reset_buf`` is set for every env,
+        so the next ``reset_done()`` puts every env on a freshly drawn clip.  A ``BatchedSampler`` that caches its observation is
+        restarted with ``sampler.restart()``."""
+        b, lib, N, dv = self.batch, self.lib, self.num_envs, self.device
+        K = lib.num_motions()
+        ids = np.arange(K, dtype=np.int64) if motion_ids is None else np.asarray(
+            motion_ids.cpu() if isinstance(motion_ids, torch.Tensor) else motion_ids, dtype=np.int64).reshape(-1)
+        if ids.size == 0 or ids.min() < 0 or ids.max() >= K:
+            raise ValueError(f"motion_ids must be a non-empty list of clips in [0, {K})")
+        nb = self.model.nbody
+        bodies = list(range(nb)) if eval_bodies is None else [self._body_index(x) for x in eval_bodies]
+        ebodies = np.ascontiguousarray(np.asarray(bodies, dtype=np.int32))
+        J, M = len(bodies), ids.size
+        tcfg = SmplsimTrackEvalCfgC(num_bodies=J, bodies=ebodies.ctypes.data if J else None, interpolate=int(self.interpolate), dt=0.0)
+        steps = self.clip_steps(ids)
+        icfg = SmplsimImitationCfgC()
+        C.memmove(C.byref(icfg), C.byref(self._icfg), C.sizeof(icfg))
+        if termination_distance is not None:
+            icfg.termination_distance = float(termination_distance)
+        icfg.episode_length = max(int(icfg.episode_length), int(steps.max()))
+        active = torch.zeros(N, dtype=torch.uint8, device=dv)
+        frames = torch.zeros(N, dtype=torch.int32, device=dv)
+        success = torch.zeros(N, dtype=torch.uint8, device=dv)
+        sums = torch.zeros(N, len(TRACK_METRICS), dtype=torch.float64, device=dv)
+        prev = torch.zeros(N, 2, J, 3, dtype=torch.float32, device=dv)
+        st = SmplsimTrackEvalStateC(active=_ptr(active), prev_diff=_ptr(prev), frames=_ptr(frames), sums=_ptr(sums), success=_ptr(success))
+        L = b._L()
+
+        def score():
+            b._check(L.smplsim_track_eval(b._h, C.byref(tcfg), C.byref(self._tab), _ptr(self.motion_ids), _ptr(self.motion_start_times),
+                                          _ptr(b.progress_buf), C.byref(b._aux), _ptr(self.terminate_buf), _ptr(self.truncate_buf), C.byref(st),
+                                          b._stream()))
+            b.gpu_launches += 1
+
+        score()            # argument check up front (no env is active: nothing is read or written)
+        out_frames = torch.zeros(M, dtype=torch.int32, device=dv)
+        out_success = torch.zeros(M, dtype=torch.uint8, device=dv)
+        out_sums = torch.zeros(M, len(TRACK_METRICS), dtype=torch.float64, device=dv)
+        left = torch.zeros(M, dtype=torch.uint8, device=dv)
+        all_ids = torch.as_tensor(ids, dtype=torch.int32).to(dv)
+        zero_t = torch.zeros(N, dtype=torch.float32, device=dv)
+        with torch.no_grad():
+            for w0 in range(0, M, N):
+                c = min(N, M - w0)
+                mask = torch.zeros(N, dtype=torch.uint8, device=dv)
+                mask[:c] = 1
+                wid = torch.zeros(N, dtype=torch.int32, device=dv)
+                wid[:c] = all_ids[w0:w0 + c]
+                self.reset(mask, motion_ids=wid, motion_times=zero_t)
+                active.copy_(mask); frames.zero_(); sums.zero_(); success.zero_()
+                for _ in range(int(steps[w0:w0 + c].max())):
+                    b.step(torch.clamp(policy(self.obs_buf), -1.0, 1.0))
+                    self._task(None, obs_only=False, icfg=icfg)
+                    score()
+                out_frames[w0:w0 + c] = frames[:c]
+                out_success[w0:w0 + c] = success[:c]
+                out_sums[w0:w0 + c] = sums[:c]
+                left[w0:w0 + c] = active[:c]
+        self.reset_buf.fill_(1)
+        if bool(left.any()):
+            raise RuntimeError("evaluate: a clip was still being scored after its step count (clip_steps disagrees with the task kernel)")
+        keys = [str(k) for k in np.asarray(lib._motion_data_keys)[ids]]
+        return TrackingEval(motion_ids=torch.as_tensor(ids), keys=keys, frames=out_frames.cpu().long(), success=out_success.cpu().bool(),
+                            sums=out_sums.cpu())
+
+
+@dataclass
+class TrackingEval:
+    """Per-clip results of ``HumanoidImB200.evaluate``, on the host.  ``motion_ids`` / ``keys``: the clips in the order evaluated;
+    ``frames``: scored frames; ``success``: the clip reached its end without early termination; ``sums [M, 6]``: per-metric sums over
+    the frames that define the metric (columns ``abi.TRACK_METRICS``: mpjpe_g, mpjpe_l, mpjpe_pa in mm, vel_dist in mm per frame,
+    accel_dist in mm per frame^2, rot_error in rad).  ``metrics[name]``: the clip's mean (NaN for a clip without such a frame);
+    ``failed_keys``: the library's motion keys of the failed clips, the argument of ``MotionLibB200.update_hard_sampling_weight`` /
+    ``update_soft_sampling_weight``."""
+    motion_ids: torch.Tensor
+    keys: List[str]
+    frames: torch.Tensor
+    success: torch.Tensor
+    sums: torch.Tensor
+
+    @property
+    def counts(self) -> torch.Tensor:
+        """``[M, 6]`` frames that define each metric: velocity needs two scored frames, acceleration three."""
+        f = self.frames.double()
+        return torch.stack([f, f, f, (f - 1).clamp(min=0), (f - 2).clamp(min=0), f], 1)
+
+    @property
+    def metrics(self) -> Dict[str, torch.Tensor]:
+        m = self.sums / self.counts
+        return {k: m[:, i] for i, k in enumerate(TRACK_METRICS)}
+
+    @property
+    def failed_keys(self) -> List[str]:
+        return [k for k, ok in zip(self.keys, self.success.tolist()) if not ok]
+
+    def summary(self, successful_only: bool = False) -> Dict[str, float]:
+        """Frame-weighted means over all clips (or the successful ones only): ``compute_metrics_lite(..., concatenate=True)[k].mean()``
+        of the reference over the same frames; plus ``success_rate`` (over all clips), ``num_clips`` and ``frames`` of the set."""
+        sel = self.success if successful_only else torch.ones_like(self.success)
+        s, n = self.sums[sel].sum(0), self.counts[sel].sum(0)
+        out = {k: float(s[i] / n[i]) if n[i] > 0 else math.nan for i, k in enumerate(TRACK_METRICS)}
+        out.update(success_rate=float(self.success.double().mean()), num_clips=int(sel.sum()), frames=int(self.frames[sel].sum()))
+        return out

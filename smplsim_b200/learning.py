@@ -52,6 +52,11 @@ class BatchedSampler:
         self.obs_clip = obs_clip
         self._obs = None
 
+    def restart(self):
+        """Forget the cached observation: the next ``sample`` starts with ``env.reset()`` (after the env was used elsewhere, e.g. by
+        ``HumanoidImB200.evaluate``)."""
+        self._obs = None
+
     def _pre(self, obs):
         return torch.clamp(obs, -self.obs_clip, self.obs_clip) if self.obs_clip else obs
 
