@@ -8,6 +8,7 @@ smplsim_gae (advantages), PPOLearner (AgentPPO.update_params semantics, gradient
     python examples/train_ppo.py --env im --num-envs 4096      # motion imitation (HumanoidImB200) on synthetic clips
     python examples/train_ppo.py --env im --amp                # ... plus the AMP style reward (HumanoidAmpB200, AMPLearner)
     python examples/train_ppo.py --env im --eval-every 5 --auto-pmcp hard   # score every clip every 5 epochs, train on the failed ones
+    python examples/train_ppo.py --env im_recovery             # imitation with fall / recovery episodes, far targets pulled in, power penalty
 
 ``--horizon x --num-envs`` plays the role of ``learning.min_batch_size`` (51 200 in the reference yaml = 4096 envs x 12.5 steps)."""
 import argparse
@@ -27,7 +28,7 @@ from smplsim_b200.ppo import PolicyGaussian, PPOLearner, Value  # noqa: E402
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--env", default="speed", choices=["speed", "reach", "getup", "im"])
+    ap.add_argument("--env", default="speed", choices=["speed", "reach", "getup", "im", "im_recovery"])
     ap.add_argument("--num-envs", type=int, default=4096, help="envs on THIS GPU")
     ap.add_argument("--horizon", type=int, default=16)
     ap.add_argument("--epochs", type=int, default=5)
@@ -38,18 +39,19 @@ def main():
     ap.add_argument("--auto-pmcp", default="off", choices=["off", "hard", "soft"],
                     help="after each evaluation, sample training clips from the failed ones (the reference's auto_pmcp / auto_pmcp_soft)")
     a = ap.parse_args()
-    if (a.eval_every or a.auto_pmcp != "off") and (a.env != "im" or a.amp):
-        ap.error("--eval-every / --auto-pmcp need --env im without --amp")
+    im = a.env in ("im", "im_recovery")
+    if (a.eval_every or a.auto_pmcp != "off") and (not im or a.amp):
+        ap.error("--eval-every / --auto-pmcp need --env im or im_recovery without --amp")
     rank, world, local = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("LOCAL_RANK", 0))
     torch.cuda.set_device(local)
     dev = f"cuda:{local}"
     if world > 1:
         torch.distributed.init_process_group("nccl", device_id=torch.device(dev))
     torch.manual_seed(a.seed)                         # identical initial weights on every rank
-    if a.env == "im":     # every env tracks a clip of the library; the synthetic clips stand in for an AMASS table (motion_loader.py)
+    if im:                # every env tracks a clip of the library; the synthetic clips stand in for an AMASS table (motion_loader.py)
         from smplsim_b200.imitation import HumanoidImB200
         from smplsim_b200.motion_lib import synthetic_tables
-        env = HumanoidImB200(make_cfg(env="im"), lambda b: synthetic_tables(b, num_clips=64, frames=300), num_envs=a.num_envs, device=dev,
+        env = HumanoidImB200(make_cfg(env=a.env), lambda b: synthetic_tables(b, num_clips=64, frames=300), num_envs=a.num_envs, device=dev,
                              seed=a.seed, rank=rank)
     else:
         env = HumanoidBatchB200(make_cfg(env=a.env), num_envs=a.num_envs, device=dev, seed=a.seed, rank=rank, with_aux=a.amp)
@@ -57,7 +59,7 @@ def main():
     if a.amp:             # the demonstrations: the imitation env's library, or synthetic clips for the other tasks
         from smplsim_b200.amp import HumanoidAmpB200
         from smplsim_b200.motion_lib import MotionLibB200, synthetic_tables
-        lib = None if a.env == "im" else MotionLibB200(env, synthetic_tables(env, num_clips=64, frames=300))
+        lib = None if im else MotionLibB200(env, synthetic_tables(env, num_clips=64, frames=300))
         env = HumanoidAmpB200(env, lib)
         amp_learner = env.make_learner()
     policy = PolicyGaussian(env.num_obs, env.num_actions, a.units, "silu", -2.5, True).to(dev)
@@ -69,6 +71,7 @@ def main():
         policy.eval()                                 # to_test during sampling: RunningNorm frozen (agents/agent.py:123)
         return policy.select_action(obs, generator=gen)
 
+    im_env = (env.env if a.amp else env) if im else None
     sampler = BatchedSampler(env, act)
     for ep in range(a.epochs):
         t0 = time.time()
@@ -86,6 +89,10 @@ def main():
             if amp_learner is not None:
                 print(f"  amp: task reward {float(env.extras['task_rew_buf'].mean()):.4f}  disc reward {float(env.disc_rew_buf.mean()):.4f}  "
                       f"disc_loss {info['disc_loss']:.4f}  acc agent {info['disc_agent_acc']:.3f} demo {info['disc_demo_acc']:.3f}", flush=True)
+            if im_env is not None and im_env.fail_states:
+                c = im_env.reset_counts.tolist()
+                print(f"  resets so far: mocap {c[1]}  fall {c[2]}  recovery {c[3]}  envs in a recovery window now "
+                      f"{int((im_env.recovery > 0).sum())}", flush=True)
         if a.eval_every and (ep + 1) % a.eval_every == 0:
             with torch.no_grad():
                 policy.eval()

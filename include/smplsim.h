@@ -451,6 +451,47 @@ int smplsim_imitation(SmplsimHandle* h, const SmplsimImitationCfg* cfg, const Sm
                       const uint8_t* mask_dev, int obs_only, float* obs_dev, float* reward_dev, uint8_t* terminated_dev,
                       uint8_t* truncated_dev, float* mpjpe_dev, int32_t* frames_dev, void* cuda_stream);
 
+/* Fail-state recovery for the imitation task, after PHC / ASE: an env that has fallen or drifted off its clip is asked to get up and
+ * walk back to it instead of being ended.  The reference ships the settings (phc_*_iccv.yaml: zero_out_far, recoverySteps,
+ * power_reward, power_coefficient) but not the code behind them, so the definitions are this project's.  Symbols as above; td =
+ * termination_distance; the root is body 0 whether or not it is tracked; p_root is the simulated root position.
+ *
+ * Zero-out-far (zero_out_far = 1), for each observation target block and for the reward's now-frame separately, on the reference pose
+ * the frame rule gives (nearest row or blended):
+ *     d = |p^_root - p_root| (before any change);
+ *     d > far_distance: p^_root <- p_root + (p^_root - p_root) far_distance / d   (body 0's target, wherever it is used);
+ *     d > td: every tracked body b targets the root: p^_b = the (pulled-in) p^_root, q^_b = q^_root, v^_b - v_b = w^_b - w_b = 0.
+ *   The 24 J words keep their layout.
+ * Point goal: g = |xy(p^_root - p_root)| against the UNMODIFIED now-frame root; every call writes goal_dist[e] = g for the envs it
+ *   touches (obs_only calls included).  With zero-out-far on and d_now > td the reward is
+ *     r = clamp((goal_dist_prev - g) / dt, 0, 1)   (goal_dist_prev: the value before this call; 1 m/s of approach earns the maximum)
+ *   instead of the tracking reward.  mpjpe and the termination distance always use the unmodified reference.
+ * Recovery window (recovery non-NULL): at a full call with recovery[e] > 0 the distance rule of terminated is not applied (aux.status
+ *   bits 1 / 2 / 4 still terminate), then recovery[e] -= 1.  Truncation is unchanged.
+ * Power: power = sum_j |ctrl[e, j] qvel[e, 6 + j]| over the actuators j (ctrl = aux.ctrl, the torque of the last substep; qvel = the
+ *   post-step qvel: Isaac's dof_force x dof_vel).  power_coefficient > 0: r -= power_coefficient power when p > 3 (the first three steps
+ *   are exempt).  Full calls write power[e] whenever power is non-NULL.
+ * Sums are lane partials in body / actuator order followed by an xor butterfly, as above: bit-reproducible.
+ * Every field zero / NULL gives exactly smplsim_imitation, through the same kernel. */
+typedef struct SmplsimImitationRecovery {
+  int32_t zero_out_far;        /* 0 / 1 */
+  float far_distance;          /* metres, > 0 when zero_out_far (PHC: 3) */
+  float power_coefficient;     /* >= 0 (PHC: 0.00005) */
+  int32_t pad_;
+  int32_t* recovery;           /* device [N] steps left in the recovery window, or NULL */
+  float* goal_dist;            /* device [N] point-goal distance, read and written; required with zero_out_far */
+  const float* qvel;           /* device [N, nv] (SmplsimState.qvel); required when power_coefficient > 0 or power is non-NULL */
+  float* power;                /* device [N], or NULL */
+} SmplsimImitationRecovery;
+/* smplsim_imitation with the recovery fields above.  SMPLSIM_EINVAL: as smplsim_imitation, and rec NULL, zero_out_far not 0 / 1,
+ * far_distance <= 0 or NaN with zero_out_far, goal_dist NULL with zero_out_far, power_coefficient < 0 or NaN, qvel or aux.ctrl NULL
+ * when the power is asked for. */
+int smplsim_imitation_recovery(SmplsimHandle* h, const SmplsimImitationCfg* cfg, const SmplsimImitationRecovery* rec,
+                               const SmplsimMotionTables* tab, const int32_t* motion_ids_dev, const float* motion_t0_dev,
+                               const int32_t* progress_dev, const SmplsimAux* aux, const float* self_obs_dev, const uint8_t* mask_dev,
+                               int obs_only, float* obs_dev, float* reward_dev, uint8_t* terminated_dev, uint8_t* truncated_dev,
+                               float* mpjpe_dev, int32_t* frames_dev, void* cuda_stream);
+
 /* Tracking evaluation: the per-frame metrics of the reference's smpl_eval (smpl_sim/smpllib/smpl_eval.py: compute_metrics_lite,
  * compute_metrics_obj, p_mpjpe, compute_error_vel, compute_error_accel) for every env that tracks a clip, accumulated per env in one
  * launch after each step's smplsim_imitation.  The reference scores recorded trajectories after the fact; here nothing but a [2, J, 3]

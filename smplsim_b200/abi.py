@@ -61,6 +61,11 @@ class SmplsimImitationCfgC(C.Structure):
                 ("future_dt", C.c_float)]
 
 
+class SmplsimImitationRecoveryC(C.Structure):
+    _fields_ = [("zero_out_far", C.c_int32), ("far_distance", C.c_float), ("power_coefficient", C.c_float), ("pad_", C.c_int32),
+                ("recovery", C.c_void_p), ("goal_dist", C.c_void_p), ("qvel", C.c_void_p), ("power", C.c_void_p)]
+
+
 class SmplsimMotionTablesC(C.Structure):
     _fields_ = [("xpos", C.c_void_p), ("xquat", C.c_void_p), ("body_vel", C.c_void_p), ("body_ang_vel", C.c_void_p),
                 ("motion_len", C.c_void_p), ("num_frames", C.c_void_p), ("motion_dt", C.c_void_p), ("length_starts", C.c_void_p),

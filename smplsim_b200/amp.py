@@ -245,7 +245,9 @@ class HumanoidAmpB200:
       disc_reward_w * r_d``; ``extras["task_rew_buf"]`` / ``extras["disc_rew_buf"]`` hold the two parts.  The step's AMP rows (before any
       reset) are kept for ``drain_amp_obs``.  In stream order, no host sync.
     - ``reset(env_ids, ...)`` / ``reset_done()``: the env's reset, then the history of the same envs filled: the current frame in every
-      slot, or for an imitation env the current frame and the clip's frames behind the reset time (MoCap init)."""
+      slot, or for an imitation env the current frame and the clip's frames behind the reset time (MoCap init).  With an imitation env's
+      fail-state recovery on, by ``reset_kind``: MoCap envs from the clip, fall envs from their state, recovery envs untouched (their state
+      and history continue)."""
 
     def __init__(self, env, motion_lib=None, amp_cfg: Optional[Dict[str, Any]] = None, discriminator: Optional[AMPDiscriminator] = None):
         from .imitation import HumanoidImB200
@@ -327,7 +329,15 @@ class HumanoidAmpB200:
             return self.obs_buf
         mask = self._mask(env_ids)
         out = self.env.reset(mask, *args, **kw)
-        self._amp(mask, AMP_FILL_REF if self.imitation else AMP_FILL)
+        if self.imitation and self.env.fail_states:    # by kind: MoCap from the clip, fall from the state; recovery envs continue
+            from .imitation import RESET_FALL, RESET_MOCAP
+            kind = self.env.reset_kind
+            mocap, fall = (kind == RESET_MOCAP).to(torch.uint8), (kind == RESET_FALL).to(torch.uint8)
+            self._amp(mocap, AMP_FILL_REF)
+            self._amp(fall, AMP_FILL)
+            mask = (mocap, fall)
+        else:
+            self._amp(mask, AMP_FILL_REF if self.imitation else AMP_FILL)
         self._keep_mask = mask
         return out
 

@@ -59,8 +59,15 @@ ENV_GROUPS: Dict[str, Dict[str, Any]] = {
                termination_distance=0.25, tracked_bodies=None,
                # blended reference states (get_motion_state) instead of nearest frames; future targets per observation, 1 / inv s apart
                # (PHC: numTrajSamples, trajSampleTimestepInv)
-               im_interpolate=False, num_traj_samples=1, traj_sample_timestep_inv=30),
+               im_interpolate=False, num_traj_samples=1, traj_sample_timestep_inv=30,
+               # fail-state recovery (PHC: fallInitProb, recoveryEpisodeProb, recoverySteps, zero_out_far, power_coefficient): all off
+               fall_init_prob=0.0, recovery_episode_prob=0.0, recovery_steps=90, zero_out_far=False, far_distance=3.0,
+               power_coefficient=0.0),
 }
+# imitation with fail-state recovery: the recovery keys of the reference's phc_kp_mcp_iccv.yaml (the other keys of that file are the
+# Isaac side's: observation v7, PNN / MCP policies, hybrid init)
+ENV_GROUPS["im_recovery"] = dict(ENV_GROUPS["im"], fall_init_prob=0.3, recovery_episode_prob=0.5, recovery_steps=90, zero_out_far=True,
+                                 far_distance=3.0, power_reward=True, power_coefficient=0.00005)
 # robot group -- smpl_sim/data/cfg/robot/{smpl,smplx}_humanoid.yaml
 _ROBOT_COMMON = dict(
     has_upright_start=False, has_shape_obs=False, has_weight_obs=False, has_shape_variation=False, has_mesh=False,

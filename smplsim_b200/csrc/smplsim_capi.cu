@@ -678,10 +678,11 @@ extern "C" int smplsim_imitation_obs_dim(const SmplsimHandle* h, int num_tracked
   return h && num_tracked >= 0 ? h->img.hdr()->self_obs_dim + 24 * num_tracked : SMPLSIM_EINVAL;
 }
 
-extern "C" int smplsim_imitation(SmplsimHandle* h, const SmplsimImitationCfg* cfg, const SmplsimMotionTables* tab, const int32_t* motion_ids_dev,
-                                 const float* motion_t0_dev, const int32_t* progress_dev, const SmplsimAux* aux, const float* self_obs_dev,
-                                 const uint8_t* mask_dev, int obs_only, float* obs_dev, float* reward_dev, uint8_t* terminated_dev,
-                                 uint8_t* truncated_dev, float* mpjpe_dev, int32_t* frames_dev, void* stream) {
+// smplsim_imitation (rec NULL) and smplsim_imitation_recovery
+static int imitation(SmplsimHandle* h, const SmplsimImitationCfg* cfg, const SmplsimImitationRecovery* rc, const SmplsimMotionTables* tab,
+                     const int32_t* motion_ids_dev, const float* motion_t0_dev, const int32_t* progress_dev, const SmplsimAux* aux,
+                     const float* self_obs_dev, const uint8_t* mask_dev, int obs_only, float* obs_dev, float* reward_dev,
+                     uint8_t* terminated_dev, uint8_t* truncated_dev, float* mpjpe_dev, int32_t* frames_dev, void* stream) {
   if (!h || !cfg || !tab || !aux) return fail(SMPLSIM_EINVAL, "smplsim_imitation: null handle / cfg / tables / aux");
   const LHdr& H = *h->img.hdr();
   if (cfg->num_tracked < 1 || cfg->num_tracked > H.nb) return fail(SMPLSIM_EINVAL, "smplsim_imitation: num_tracked outside [1, nbody]");
@@ -700,6 +701,14 @@ extern "C" int smplsim_imitation(SmplsimHandle* h, const SmplsimImitationCfg* cf
   if (cfg->interpolate != 0 && cfg->interpolate != 1) return fail(SMPLSIM_EINVAL, "smplsim_imitation: interpolate must be 0 or 1");
   if (cfg->num_future < 0) return fail(SMPLSIM_EINVAL, "smplsim_imitation: num_future < 0");
   if (!(cfg->future_dt >= 0.f)) return fail(SMPLSIM_EINVAL, "smplsim_imitation: future_dt < 0 or NaN");
+  SmplsimImitationRecovery r; std::memset(&r, 0, sizeof r);
+  if (rc) r = *rc;
+  if (r.zero_out_far != 0 && r.zero_out_far != 1) return fail(SMPLSIM_EINVAL, "smplsim_imitation: zero_out_far must be 0 or 1");
+  if (r.zero_out_far && !(r.far_distance > 0.f)) return fail(SMPLSIM_EINVAL, "smplsim_imitation: far_distance <= 0 or NaN with zero_out_far");
+  if (r.zero_out_far && !r.goal_dist) return fail(SMPLSIM_EINVAL, "smplsim_imitation: zero_out_far needs goal_dist");
+  if (!(r.power_coefficient >= 0.f)) return fail(SMPLSIM_EINVAL, "smplsim_imitation: power_coefficient < 0 or NaN");
+  const bool power = r.power_coefficient > 0.f || r.power;
+  if (power && (!r.qvel || !aux->ctrl)) return fail(SMPLSIM_EINVAL, "smplsim_imitation: the power needs qvel and aux.ctrl");
   DeviceGuard guard(h->device);
   ImArgs a; std::memset(&a, 0, sizeof a);
   a.txpos = tab->xpos; a.txquat = tab->xquat; a.tvel = tab->body_vel; a.tangvel = tab->body_ang_vel;
@@ -714,17 +723,48 @@ extern "C" int smplsim_imitation(SmplsimHandle* h, const SmplsimImitationCfg* cf
   a.n = h->num_envs; a.nb = H.nb; a.J = cfg->num_tracked; a.self_dim = H.self_obs_dim; a.self_stride = H.obs_dim; a.obs_only = obs_only ? 1 : 0;
   for (int j = 0; j < a.J; j++) a.body[j] = (unsigned char)(cfg->tracked_bodies ? cfg->tracked_bodies[j] : j);
   a.T = std::max(cfg->num_future, 1); a.future_dt = cfg->future_dt;
+  ImRec rk; std::memset(&rk, 0, sizeof rk);
+  rk.zof = r.zero_out_far; rk.far = r.far_distance; rk.power_k = r.power_coefficient; rk.nu = H.nu; rk.nv = H.nv;
+  rk.recovery = r.recovery; rk.goal = r.goal_dist; rk.qvel = r.qvel; rk.ctrl = aux->ctrl; rk.power = r.power;
   const int wpb = 8, grid = (a.n + wpb - 1) / wpb;
   const bool multi = a.T > 1;
-  if (cfg->interpolate) {
-    if (multi) L_LAUNCH((k_imitation<1, 1>), grid, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a);
-    else L_LAUNCH((k_imitation<1, 0>), grid, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a);
+  // fail-state recovery runs in its own instances, so that with every recovery field zero the task is the one before it existed
+  const bool rec = r.zero_out_far || power || r.recovery || r.goal_dist;
+  if (rec) {
+    if (cfg->interpolate) {
+      if (multi) L_LAUNCH((k_imitation<1, 1, 1>), grid, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a, rk);
+      else L_LAUNCH((k_imitation<1, 0, 1>), grid, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a, rk);
+    } else {
+      if (multi) L_LAUNCH((k_imitation<0, 1, 1>), grid, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a, rk);
+      else L_LAUNCH((k_imitation<0, 0, 1>), grid, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a, rk);
+    }
+  } else if (cfg->interpolate) {
+    if (multi) L_LAUNCH((k_imitation<1, 1, 0>), grid, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a, rk);
+    else L_LAUNCH((k_imitation<1, 0, 0>), grid, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a, rk);
   } else {
-    if (multi) L_LAUNCH((k_imitation<0, 1>), grid, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a);
-    else L_LAUNCH((k_imitation<0, 0>), grid, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a);
+    if (multi) L_LAUNCH((k_imitation<0, 1, 0>), grid, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a, rk);
+    else L_LAUNCH((k_imitation<0, 0, 0>), grid, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a, rk);
   }
   CUDA_TRY(cudaGetLastError());
   return SMPLSIM_OK;
+}
+
+extern "C" int smplsim_imitation(SmplsimHandle* h, const SmplsimImitationCfg* cfg, const SmplsimMotionTables* tab, const int32_t* motion_ids_dev,
+                                 const float* motion_t0_dev, const int32_t* progress_dev, const SmplsimAux* aux, const float* self_obs_dev,
+                                 const uint8_t* mask_dev, int obs_only, float* obs_dev, float* reward_dev, uint8_t* terminated_dev,
+                                 uint8_t* truncated_dev, float* mpjpe_dev, int32_t* frames_dev, void* stream) {
+  return imitation(h, cfg, nullptr, tab, motion_ids_dev, motion_t0_dev, progress_dev, aux, self_obs_dev, mask_dev, obs_only, obs_dev, reward_dev,
+                   terminated_dev, truncated_dev, mpjpe_dev, frames_dev, stream);
+}
+
+extern "C" int smplsim_imitation_recovery(SmplsimHandle* h, const SmplsimImitationCfg* cfg, const SmplsimImitationRecovery* rec,
+                                          const SmplsimMotionTables* tab, const int32_t* motion_ids_dev, const float* motion_t0_dev,
+                                          const int32_t* progress_dev, const SmplsimAux* aux, const float* self_obs_dev, const uint8_t* mask_dev,
+                                          int obs_only, float* obs_dev, float* reward_dev, uint8_t* terminated_dev, uint8_t* truncated_dev,
+                                          float* mpjpe_dev, int32_t* frames_dev, void* stream) {
+  if (!rec) return fail(SMPLSIM_EINVAL, "smplsim_imitation_recovery: null recovery fields");
+  return imitation(h, cfg, rec, tab, motion_ids_dev, motion_t0_dev, progress_dev, aux, self_obs_dev, mask_dev, obs_only, obs_dev, reward_dev,
+                   terminated_dev, truncated_dev, mpjpe_dev, frames_dev, stream);
 }
 
 // ------------------------------------------------------------------ tracking evaluation (track_eval_kernels.cuh)

@@ -4,7 +4,9 @@
 CUDA kernel per call (``smplsim_imitation``, csrc/imitation_kernels.cuh) that reads the library's tables in place: tracking
 observation, reward, early termination, truncation at the clip's end and the mean per-joint position error.  The definitions are
 stated in include/smplsim.h and DESIGN.md 2; the reference ships no imitation task in its MuJoCo env layer (SURVEY.md 3.4), they
-follow the published PHC formulation.  Envs that finish are put back on a reference frame of a newly drawn clip (MoCap init).
+follow the published PHC formulation.  Envs that finish are put back on a reference frame of a newly drawn clip (MoCap init), or, with
+fail-state recovery on, on a fallen state of a bank built at construction (fall episode) or left where they fell with a new clip to walk
+back to (recovery episode; ``smplsim_imitation_recovery``).
 ``HumanoidImB200.evaluate`` scores a policy on every clip of the library with the reference's smpl_eval metrics (``smplsim_track_eval``,
 csrc/track_eval_kernels.cuh) and reports the failed clips that PMCP sampling takes."""
 from __future__ import annotations
@@ -17,9 +19,13 @@ from typing import Any, Callable, Dict, List, Optional, Sequence, Union
 import numpy as np
 import torch
 
-from .abi import TRACK_METRICS, SmplsimImitationCfgC, SmplsimMotionTablesC, SmplsimTrackEvalCfgC, SmplsimTrackEvalStateC
+from .abi import (TRACK_METRICS, SmplsimImitationCfgC, SmplsimImitationRecoveryC, SmplsimMotionTablesC, SmplsimTrackEvalCfgC,
+                  SmplsimTrackEvalStateC)
 from .batched import HumanoidBatchB200, _ptr
 from .motion_lib import MotionLibB200
+
+RESET_NONE, RESET_MOCAP, RESET_FALL, RESET_RECOVERY = 0, 1, 2, 3     # values of HumanoidImB200.reset_kind
+FALL_BANK_ROUNDS = 8                                                # fallen states kept per env
 
 
 class HumanoidImB200:
@@ -31,7 +37,13 @@ class HumanoidImB200:
 
     ``cfg``: ``make_cfg(env="im")`` (gains ``im_k_*``, weights ``im_w_*``, ``termination_distance``, ``tracked_bodies``, ``episode_length``;
     ``im_interpolate``: blended reference states instead of nearest frames, in the task and in the reset state; ``num_traj_samples`` targets
-    per observation, ``1 / traj_sample_timestep_inv`` seconds apart).
+    per observation, ``1 / traj_sample_timestep_inv`` seconds apart).  Fail-state recovery (``make_cfg(env="im_recovery")``, the
+    values of PHC's settings; all off in ``im``): ``zero_out_far`` / ``far_distance`` (far targets pulled in to the root and the
+    point-goal reward), ``power_coefficient`` (with ``power_reward``: the power penalty), ``fall_init_prob`` / ``recovery_episode_prob``
+    / ``recovery_steps`` (the reset policy of ``reset``).  With ``fall_init_prob > 0`` the constructor runs the stepper's Fall reset over
+    all envs ``FALL_BANK_ROUNDS`` times and keeps the states (``fall_qpos [8, N, nq]``, ``fall_qvel``), so it overwrites the batch's
+    state (every env's ``reset_buf`` is set after construction anyway).  ``extras`` holds ``power``, ``recovery`` (steps left in the
+    window without distance termination) and ``goal_dist`` (point-goal distance); they stay zero while recovery is off.
     ``motion``: the library's tables (the dict ``synthetic_tables`` / ``amass_tables`` return), or a callable ``batch -> tables`` (the
     synthetic tables need the batch's kinematics), or a ``MotionLibB200`` built on ``batch``.
     ``tracked_bodies``: body names or indices (default ``cfg.env.tracked_bodies``, None = all bodies).
@@ -70,6 +82,16 @@ class HumanoidImB200:
         inv = float(e.get("traj_sample_timestep_inv", 30))
         if self.num_future < 1 or not inv > 0:
             raise ValueError(f"num_traj_samples must be >= 1 and traj_sample_timestep_inv > 0, got {self.num_future} / {inv}")
+        self.fall_init_prob, self.recovery_episode_prob = float(e.get("fall_init_prob", 0.0)), float(e.get("recovery_episode_prob", 0.0))
+        self.recovery_steps = int(e.get("recovery_steps", 90))
+        zof, far = bool(e.get("zero_out_far", False)), float(e.get("far_distance", 3.0))
+        pk = float(e.get("power_coefficient", 0.0)) if bool(e.get("power_reward", False)) else 0.0
+        for k, x in (("fall_init_prob", self.fall_init_prob), ("recovery_episode_prob", self.recovery_episode_prob)):
+            if not 0.0 <= x <= 1.0:
+                raise ValueError(f"{k} must be in [0, 1], got {x}")
+        if self.recovery_steps < 0:
+            raise ValueError(f"recovery_steps must be >= 0, got {self.recovery_steps}")
+        self.fail_states = self.fall_init_prob > 0 or self.recovery_episode_prob > 0     # reset() draws the episode kind
         self._icfg = SmplsimImitationCfgC(
             k_pos=float(e.im_k_pos), k_rot=float(e.im_k_rot), k_vel=float(e.im_k_vel), k_angvel=float(e.im_k_angvel),
             w_pos=float(e.im_w_pos), w_rot=float(e.im_w_rot), w_vel=float(e.im_w_vel), w_angvel=float(e.im_w_angvel),
@@ -94,7 +116,17 @@ class HumanoidImB200:
         self.motion_ids = torch.zeros(N, dtype=torch.int32, device=dv)
         self.motion_start_times = torch.zeros(N, **f32)
         self.ref_frames = torch.zeros(N, 2, dtype=torch.int32, device=dv)
-        self.extras = {"terminate": self.terminate_buf, "sim_warning": b.status, "mpjpe": self.mpjpe}
+        self.recovery = torch.zeros(N, dtype=torch.int32, device=dv)
+        self.goal_dist = torch.zeros(N, **f32)
+        self.power = torch.zeros(N, **f32)
+        self.reset_kind = torch.zeros(N, **u8)
+        self.reset_counts = torch.zeros(4, dtype=torch.int64, device=dv)   # resets of each kind since construction, by RESET_*
+        self.extras = {"terminate": self.terminate_buf, "sim_warning": b.status, "mpjpe": self.mpjpe, "power": self.power,
+                       "recovery": self.recovery, "goal_dist": self.goal_dist}
+        # the recovery fields (None: the plain task); the kernel checks them with the rest at the first call below
+        self._rec = SmplsimImitationRecoveryC(zero_out_far=int(zof), far_distance=far, power_coefficient=pk, recovery=_ptr(self.recovery),
+                                              goal_dist=_ptr(self.goal_dist), qvel=_ptr(b.qvel), power=_ptr(self.power)) \
+            if (self.fail_states or zof or pk > 0) else None
         # reference state of a reset (gathered rows of the qpos / qvel tables) and per-clip statistics
         self._qpos0 = torch.zeros(N, m.nq, **f32)
         self._qvel0 = torch.zeros(N, m.nv, **f32)
@@ -105,6 +137,15 @@ class HumanoidImB200:
         self.clip_episodes = torch.zeros(K, dtype=torch.float64, device=dv)       # episodes that ended on each clip
         self.clip_terminations = torch.zeros(K, dtype=torch.float64, device=dv)   # ... of which by early termination
         self._task(None, obs_only=True)      # argument check up front (a bad tracked body is refused here, not at the first step)
+        self.fall_qpos = self.fall_qvel = None
+        if self.fall_init_prob > 0:          # the fall-state bank: column e holds states of env e's own body and parameters
+            self.fall_qpos = torch.zeros(FALL_BANK_ROUNDS, N, m.nq, **f32)
+            self.fall_qvel = torch.zeros(FALL_BANK_ROUNDS, N, m.nv, **f32)
+            for r in range(FALL_BANK_ROUNDS):
+                b.reset(None, init_mode=1)
+                self.fall_qpos[r].copy_(b.qpos)
+                self.fall_qvel[r].copy_(b.qvel)
+            self._env_index = torch.arange(N, device=dv)
 
     def _body_index(self, x):
         m = self.batch.model
@@ -120,12 +161,17 @@ class HumanoidImB200:
     def gpu_launches(self) -> int:
         return self.batch.gpu_launches
 
-    def _task(self, mask: Optional[torch.Tensor], obs_only: bool, icfg: Optional[SmplsimImitationCfgC] = None):
-        b = self.batch
-        b._check(b._L().smplsim_imitation(b._h, C.byref(self._icfg if icfg is None else icfg), C.byref(self._tab), _ptr(self.motion_ids), _ptr(self.motion_start_times),
-                                          _ptr(b.progress_buf), C.byref(b._aux), _ptr(b.obs_buf), _ptr(mask), int(obs_only),
-                                          _ptr(self.obs_buf), _ptr(self.rew_buf), _ptr(self.terminate_buf), _ptr(self.truncate_buf),
-                                          _ptr(self.mpjpe), _ptr(self.ref_frames), b._stream()))
+    def _task(self, mask: Optional[torch.Tensor], obs_only: bool, icfg: Optional[SmplsimImitationCfgC] = None, recovery: bool = True):
+        """One task launch; ``recovery=False`` runs the plain task even when fail-state recovery is on (``evaluate``)."""
+        b, L = self.batch, self.batch._L()
+        head = (b._h, C.byref(self._icfg if icfg is None else icfg))
+        tail = (C.byref(self._tab), _ptr(self.motion_ids), _ptr(self.motion_start_times), _ptr(b.progress_buf), C.byref(b._aux), _ptr(b.obs_buf),
+                _ptr(mask), int(obs_only), _ptr(self.obs_buf), _ptr(self.rew_buf), _ptr(self.terminate_buf), _ptr(self.truncate_buf),
+                _ptr(self.mpjpe), _ptr(self.ref_frames), b._stream())
+        if recovery and self._rec is not None:
+            b._check(L.smplsim_imitation_recovery(*head, C.byref(self._rec), *tail))
+        else:
+            b._check(L.smplsim_imitation(*head, *tail))
         b.gpu_launches += 1
 
     def step(self, actions: torch.Tensor):
@@ -145,7 +191,18 @@ class HumanoidImB200:
         """Put the envs ``env_ids`` (None = all; an index tensor or a uint8 / bool mask) on a reference frame: a clip from
         ``lib.sample_motions`` and a start time from ``lib.sample_time`` (at least one control period before the clip's end), or the
         caller's ``motion_ids`` / ``motion_times`` (full ``[num_envs]`` tensors; rows outside ``env_ids`` are ignored).  Masked and in
-        stream order: the other envs keep their state, observation row, clip and start time."""
+        stream order: the other envs keep their state, observation row, clip and start time.
+
+        With ``fall_init_prob`` or ``recovery_episode_prob`` above 0, a call without ``motion_ids`` / ``motion_times`` (the one
+        ``reset_done`` makes) draws each selected env's episode kind on the device, without a host sync: an env whose ``terminate_buf``
+        is set becomes a recovery episode with probability ``recovery_episode_prob`` (its physics state is kept, ``progress_buf`` = 0);
+        of the others, a fall episode with probability ``fall_init_prob`` (restored from a row of its own column of the fall-state bank);
+        the rest are MoCap resets.  Every selected env gets a new clip and start time; recovery and fall episodes start a window of
+        ``recovery_steps`` full steps without distance termination (``recovery``), MoCap resets clear it.  ``reset_kind`` records the
+        kind (``RESET_*``; 0 for envs outside the selection) and ``reset_counts`` adds it up.  An explicit ``motion_ids`` / ``motion_times`` call is a MoCap reset."""
+        return self._reset(env_ids, motion_ids, motion_times, recovery=True)
+
+    def _reset(self, env_ids, motion_ids, motion_times, recovery: bool):
         b, lib, N, dv = self.batch, self.lib, self.num_envs, self.device
         mask = None
         if env_ids is not None:
@@ -174,9 +231,28 @@ class HumanoidImB200:
             lib.blend_into(("qpos", "qvel"), self.motion_ids, self.motion_start_times, (self._qpos0, self._qvel0))
         else:
             lib.gather_into(("qpos", "qvel"), self.motion_ids, self.motion_start_times, (self._qpos0, self._qvel0))
-        b.reset(mask, init_mode=2, qpos0=self._qpos0, qvel0=self._qvel0)
-        self._task(mask, obs_only=True)
-        self._keep = mask
+        phys = mask
+        if self.fail_states:
+            sel = torch.ones(N, dtype=torch.bool, device=dv) if mask is None else mask.bool()
+            kind = torch.full((N,), RESET_MOCAP, dtype=torch.uint8, device=dv)
+            if motion_ids is None and motion_times is None:
+                u = torch.rand(2, N, generator=lib._gen, device=dv)
+                rec = sel & self.terminate_buf.bool() & (u[0] < self.recovery_episode_prob)
+                fall = sel & ~rec & (u[1] < self.fall_init_prob)
+                if self.fall_qpos is not None:     # a bank row per env, from its own column
+                    row = torch.randint(0, FALL_BANK_ROUNDS, (N,), generator=lib._gen, device=dv)
+                    torch.where(fall[:, None], self.fall_qpos[row, self._env_index], self._qpos0, out=self._qpos0)
+                    torch.where(fall[:, None], self.fall_qvel[row, self._env_index], self._qvel0, out=self._qvel0)
+                kind.masked_fill_(fall, RESET_FALL).masked_fill_(rec, RESET_RECOVERY)
+                self.progress_buf.masked_fill_(rec, 0)
+                phys = (sel & ~rec).to(torch.uint8)
+            torch.where(sel, kind, torch.zeros_like(kind), out=self.reset_kind)
+            self.reset_counts.scatter_add_(0, self.reset_kind.long(), sel.long())
+            steps = torch.where(kind == RESET_MOCAP, 0, self.recovery_steps).to(torch.int32)
+            torch.where(sel, steps, self.recovery, out=self.recovery)
+        b.reset(phys, init_mode=2, qpos0=self._qpos0, qvel0=self._qvel0)
+        self._task(mask, obs_only=True, recovery=recovery)
+        self._keep = (mask, phys)
         return self.obs_buf
 
     def reset_done(self):
@@ -211,7 +287,8 @@ class HumanoidImB200:
         smpl_eval (include/smplsim.h, smplsim_track_eval).  Clips go to envs in waves of ``num_envs``: one masked ``reset`` per wave, then
         a step count fixed up front from the host copy of the clip lengths (``clip_steps``), each step the physics step, the task kernel
         and the evaluation kernel, with no host sync.  A clip fails when it terminates early (``termination_distance``, default the cfg's)
-        and succeeds when it reaches its end; the episode length is raised to the longest clip for the call.
+        and succeeds when it reaches its end; the episode length is raised to the longest clip for the call.  Fail-state recovery plays
+        no part: the plain task scores every step, and the resets are MoCap resets that clear the recovery counters.
         ``eval_bodies``: names or indices, at least 3, the first is the root (default: all bodies).
 
         Training state is left alone: ``clip_episodes`` / ``clip_terminations`` and the sampling weights do not change.  The env's
@@ -263,11 +340,11 @@ class HumanoidImB200:
                 mask[:c] = 1
                 wid = torch.zeros(N, dtype=torch.int32, device=dv)
                 wid[:c] = all_ids[w0:w0 + c]
-                self.reset(mask, motion_ids=wid, motion_times=zero_t)
+                self._reset(mask, wid, zero_t, recovery=False)
                 active.copy_(mask); frames.zero_(); sums.zero_(); success.zero_()
                 for _ in range(int(steps[w0:w0 + c].max())):
                     b.step(torch.clamp(policy(self.obs_buf), -1.0, 1.0))
-                    self._task(None, obs_only=False, icfg=icfg)
+                    self._task(None, obs_only=False, icfg=icfg, recovery=False)
                     score()
                 out_frames[w0:w0 + c] = frames[:c]
                 out_success[w0:w0 + c] = success[:c]
