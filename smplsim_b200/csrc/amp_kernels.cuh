@@ -14,7 +14,7 @@
 #define AMP_DEMO 3       // caller rows (motion id, time): ref(t - k dt) in slot k
 
 struct AmpArgs {
-  // motion library: per-frame tables [total_frames, nb * {3, 4, 3, 3} | nv - 6 | nv - 6] and per-clip rows (FILL_REF, DEMO)
+  // motion library (motion_clip, ImRow): per-frame tables [total_frames, nb * {3, 4, 3, 3} | nv - 6 | nv - 6] and per-clip rows (FILL_REF, DEMO)
   const float *txpos, *txquat, *tvel, *tangvel, *tdof, *tdofv;
   const float* mlen; const int32_t* nframes; const float* mdt; const int32_t* starts;
   // per env (per row in DEMO)
@@ -26,12 +26,6 @@ struct AmpArgs {
   unsigned char key[LM_MAXB];
 };
 
-__device__ __forceinline__ Q4 amp_ldq(const float* p) { Q4 q; q.w = p[0]; q.x = p[1]; q.y = p[2]; q.z = p[3]; return q; }
-__device__ __forceinline__ void amp_st6(float* p, Q4 q) {   // quat_to_tan_norm: [q * (1,0,0), q * (0,0,1)]
-  st3(p, qrot_ref(q, v3(1.f, 0.f, 0.f)));
-  st3(p + 3, qrot_ref(q, v3(0.f, 0.f, 1.f)));
-}
-
 // One AMP frame into out[0, F).  root_vel / root_ang_vel are world-frame; dof / dofv hold nv - 6 values; bx is the [nb, 3] body
 // position row the key bodies are read from.
 __device__ __forceinline__ void amp_frame(const LHdr& H, const AmpArgs& a, int lane, V3 root, Q4 rq, V3 rv, V3 rw, const float* dof,
@@ -41,7 +35,7 @@ __device__ __forceinline__ void amp_frame(const LHdr& H, const AmpArgs& a, int l
   const int o = a.root_h, od = o + 12, ov = od + 6 * (a.nb - 1), ok = ov + (a.nv - 6);
   if (lane == 0) {
     if (a.root_h) out[0] = root.z;
-    amp_st6(out + o, a.local_root ? qmul(hq, rq) : rq);
+    st_tan_norm(out + o, a.local_root ? qmul(hq, rq) : rq);
     st3(out + o + 6, qrot_ref(hq, rv));
     st3(out + o + 9, qrot_ref(hq, rw));
   }
@@ -57,7 +51,7 @@ __device__ __forceinline__ void amp_frame(const LHdr& H, const AmpArgs& a, int l
       q.w = cosf(0.5f * w); q.x = ax.x * s; q.y = ax.y * s; q.z = ax.z * s;
       q = qnormalize(q);                                               // ... and the quaternion
     }
-    amp_st6(out + od + 6 * j, q);
+    st_tan_norm(out + od + 6 * j, q);
   }
   for (int i = lane; i < a.nv - 6; i += 32) out[ov + i] = dofv[i];
   for (int k = lane; k < a.nkey; k += 32) st3(out + ok + 3 * k, qrot_ref(hq, ld3(bx + 3 * a.key[k]) - root));
@@ -70,29 +64,26 @@ __device__ __forceinline__ void amp_frame(const LHdr& H, const AmpArgs& a, int l
 #define AMP_STAGE (2 * 3 * (LM_MAXB - 1) + 3 * LM_MAXB)   // floats per warp: dof_pos, dof_vel, body positions
 template <int INTERP>
 __device__ __forceinline__ void amp_ref_frame(const LHdr& H, const AmpArgs& a, int lane, int id, float t, float* out) {
+  const ImFrame f = im_frame<INTERP>(a.mlen[id], a.mdt[id], a.nframes[id], a.starts[id], t);
+  const ImRow r0(a, f.f0);
+  const int nd = a.nv - 6;
   if (INTERP) {
     __shared__ float stage[8][AMP_STAGE];   // 8 warps per CTA (the launches' size)
     float* sd = stage[threadIdx.x >> 5];
-    const int nd = a.nv - 6;
     float *sv = sd + nd, *sx = sd + 2 * nd;
-    const MBlend m = motion_blend_frames(a.mlen[id], a.mdt[id], a.nframes[id], t);
-    const size_t r0 = (size_t)(a.starts[id] + m.f0), r1 = (size_t)(a.starts[id] + m.f1);
+    const ImRow r1(a, f.f1);
     __syncwarp();   // the previous frame's reads of the slot are done
     for (int i = lane; i < nd; i += 32) {
-      sd[i] = mb_lerp(a.tdof[r0 * nd + i], a.tdof[r1 * nd + i], m.b);
-      sv[i] = mb_lerp(a.tdofv[r0 * nd + i], a.tdofv[r1 * nd + i], m.b);
+      sd[i] = mb_lerp(a.tdof[f.f0 * nd + i], a.tdof[f.f1 * nd + i], f.b);
+      sv[i] = mb_lerp(a.tdofv[f.f0 * nd + i], a.tdofv[f.f1 * nd + i], f.b);
     }
-    for (int i = lane; i < 3 * a.nb; i += 32) sx[i] = mb_lerp(a.txpos[r0 * a.nb * 3 + i], a.txpos[r1 * a.nb * 3 + i], m.b);
+    for (int i = lane; i < 3 * a.nb; i += 32) sx[i] = mb_lerp(r0.p[i], r1.p[i], f.b);
     __syncwarp();
-    amp_frame(H, a, lane, ld3(sx), mb_slerp(amp_ldq(a.txquat + r0 * a.nb * 4), amp_ldq(a.txquat + r1 * a.nb * 4), m.b),
-              mb_lerp3(ld3(a.tvel + r0 * a.nb * 3), ld3(a.tvel + r1 * a.nb * 3), m.b),
-              mb_lerp3(ld3(a.tangvel + r0 * a.nb * 3), ld3(a.tangvel + r1 * a.nb * 3), m.b), sd, sv, sx, out);
+    amp_frame(H, a, lane, ld3(sx), mb_slerp(mb_ldq(r0.q), mb_ldq(r1.q), f.b), mb_lerp3(ld3(r0.v), ld3(r1.v), f.b),
+              mb_lerp3(ld3(r0.w), ld3(r1.w), f.b), sd, sv, sx, out);
     return;
   }
-  const size_t r = (size_t)(a.starts[id] + motion_frame(a.mlen[id], a.mdt[id], a.nframes[id], t));
-  const float* bx = a.txpos + r * a.nb * 3;
-  amp_frame(H, a, lane, ld3(bx), amp_ldq(a.txquat + r * a.nb * 4), ld3(a.tvel + r * a.nb * 3), ld3(a.tangvel + r * a.nb * 3),
-            a.tdof + r * (a.nv - 6), a.tdofv + r * (a.nv - 6), bx, out);
+  amp_frame(H, a, lane, ld3(r0.p), mb_ldq(r0.q), ld3(r0.v), ld3(r0.w), a.tdof + f.f0 * nd, a.tdofv + f.f0 * nd, r0.p, out);
 }
 
 // INTERP: library frames blended (SmplsimAmpCfg.interpolate); <0> reads the nearest frame
@@ -105,7 +96,7 @@ __global__ void __launch_bounds__(256) k_amp_obs(const float* __restrict__ gimg,
   const int K = a.K, F = a.F;
   float* row = a.out + (size_t)e * K * F;
   if (a.mode == AMP_DEMO) {
-    const int id = min(max(a.ids[e], 0), a.nmotion - 1);
+    const int id = motion_clip(a, a.ids[e]);
     const float t = a.t0[e];
     for (int k = 0; k < K; k++) amp_ref_frame<INTERP>(H, a, lane, id, fmaf(-(float)k, a.dt, t), row + (size_t)k * F);
     return;
@@ -127,7 +118,7 @@ __global__ void __launch_bounds__(256) k_amp_obs(const float* __restrict__ gimg,
   {   // the simulated frame at slot 0: post-step state; MuJoCo's root angular velocity is body-frame, rotated to world here
     const float *qp = a.qpos + (size_t)e * a.nv + (size_t)e, *qv = a.qvel + (size_t)e * a.nv;   // qpos rows are nv + 1 wide
     const float* bx = a.xpos + (size_t)e * a.nb * 3;
-    const Q4 rq = amp_ldq(a.xquat + (size_t)e * a.nb * 4);
+    const Q4 rq = mb_ldq(a.xquat + (size_t)e * a.nb * 4);
     amp_frame(H, a, lane, ld3(bx), rq, ld3(qv), qrot_ref(rq, ld3(qv + 3)), qp + 7, qv + 6, bx, row);
   }
   if (a.mode == AMP_PUSH) return;
@@ -140,7 +131,7 @@ __global__ void __launch_bounds__(256) k_amp_obs(const float* __restrict__ gimg,
     return;
   }
   // AMP_FILL_REF: the env's clip behind the current time, t0 + (p - k) dt as one fused multiply-add (the time rule of k_imitation)
-  const int id = min(max(a.ids[e], 0), a.nmotion - 1);
+  const int id = motion_clip(a, a.ids[e]);
   const int p = a.progress[e];
   for (int k = 1; k < K; k++) amp_ref_frame<INTERP>(H, a, lane, id, fmaf((float)(p - k), a.dt, a.t0[e]), row + (size_t)k * F);
 }

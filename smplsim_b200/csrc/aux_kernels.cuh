@@ -136,6 +136,39 @@ __device__ __forceinline__ Q4 mb_slerp(Q4 q0, Q4 q1, float t) {
 }
 __device__ __forceinline__ Q4 mb_ldq(const float* p) { Q4 q; q.w = p[0]; q.x = p[1]; q.y = p[2]; q.z = p[3]; return q; }
 __device__ __forceinline__ void mb_stq(float* p, Q4 q) { p[0] = q.w; p[1] = q.x; p[2] = q.y; p[3] = q.z; }
+// quat_to_tan_norm: [q * (1,0,0), q * (0,0,1)], a rotation as the observations hold it (the rule of pack_self_obs)
+__device__ __forceinline__ void st_tan_norm(float* p, Q4 q) {
+  st3(p, qrot_ref(q, v3(1.f, 0.f, 0.f)));
+  st3(p + 3, qrot_ref(q, v3(0.f, 0.f, 1.f)));
+}
+
+// The motion library as the per-env task kernels (imitation, tracking evaluation, AMP) read it, from the fields their arguments share:
+// per-frame body tables txpos / txquat / tvel / tangvel [total_frames, nb * {3, 4, 3, 3}], per-clip rows mlen / nframes / mdt / starts
+// and nmotion clips.  The fields stay flat in each argument struct: nested in a struct of their own they cost k_imitation<0, 1, 0>
+// 16 registers (a CTA fewer per SM) and a fifth of its time.
+// motion_clip: a caller's clip id, clamped to the library
+template <class A>
+__device__ __forceinline__ int motion_clip(const A& a, int id) { return min(max(id, 0), a.nmotion - 1); }
+// The reference pose of a clip at one time.  ImFrame: its table row f0 and, with INTERP, the next row f1 and the blend weight of
+// get_motion_state (motion_blend_frames); without, the one row of motion_frame.
+struct ImFrame { size_t f0, f1; float b; };
+template <int INTERP>
+__device__ __forceinline__ ImFrame im_frame(float len, float mdt, int nf, int start, float t) {
+  ImFrame f;
+  if (INTERP) {
+    const MBlend m = motion_blend_frames(len, mdt, nf, t);
+    f.f0 = (size_t)(start + m.f0); f.f1 = (size_t)(start + m.f1); f.b = m.b;
+  } else {
+    f.f0 = f.f1 = (size_t)(start + motion_frame(len, mdt, nf, t)); f.b = 0.f;
+  }
+  return f;
+}
+// the body tables' row r of the library in a (with a.nb bodies)
+struct ImRow {
+  const float *p, *q, *v, *w;
+  template <class A>
+  __device__ __forceinline__ ImRow(const A& a, size_t r) : p(a.txpos + r * a.nb * 3), q(a.txquat + r * a.nb * 4), v(a.tvel + r * a.nb * 3), w(a.tangvel + r * a.nb * 3) {}
+};
 
 // smplsim_motion_blend: per table a value kind (SMPLSIM_BLEND_*, include/smplsim.h)
 #define MB_LERP 0

@@ -678,6 +678,19 @@ extern "C" int smplsim_imitation_obs_dim(const SmplsimHandle* h, int num_tracked
   return h && num_tracked >= 0 ? h->img.hdr()->self_obs_dim + 24 * num_tracked : SMPLSIM_EINVAL;
 }
 
+// a motion library's tables against the handle, into the kernel arguments a (ImArgs, AmpArgs); "" when they are good, else the reason
+// (SMPLSIM_EINVAL)
+template <class A>
+static std::string motion_tables(const LHdr& H, const SmplsimMotionTables* tab, A& a) {
+  if (tab->nbody != H.nb) return "the tables' nbody is not the handle's";
+  if (tab->num_motions < 1) return "num_motions < 1";
+  if (!tab->xpos || !tab->xquat || !tab->body_vel || !tab->body_ang_vel || !tab->motion_len || !tab->num_frames || !tab->motion_dt || !tab->length_starts)
+    return "null motion table";
+  a.txpos = tab->xpos; a.txquat = tab->xquat; a.tvel = tab->body_vel; a.tangvel = tab->body_ang_vel;
+  a.mlen = tab->motion_len; a.nframes = tab->num_frames; a.mdt = tab->motion_dt; a.starts = tab->length_starts; a.nmotion = tab->num_motions;
+  return "";
+}
+
 // smplsim_imitation (rec NULL) and smplsim_imitation_recovery
 static int imitation(SmplsimHandle* h, const SmplsimImitationCfg* cfg, const SmplsimImitationRecovery* rc, const SmplsimMotionTables* tab,
                      const int32_t* motion_ids_dev, const float* motion_t0_dev, const int32_t* progress_dev, const SmplsimAux* aux,
@@ -690,11 +703,11 @@ static int imitation(SmplsimHandle* h, const SmplsimImitationCfg* cfg, const Smp
   if (cfg->tracked_bodies)
     for (int j = 0; j < cfg->num_tracked; j++)
       if (cfg->tracked_bodies[j] < 0 || cfg->tracked_bodies[j] >= H.nb) return fail(SMPLSIM_EINVAL, "smplsim_imitation: tracked body out of range [0, nbody)");
-  if (tab->nbody != H.nb) return fail(SMPLSIM_EINVAL, "smplsim_imitation: the tables' nbody is not the handle's");
-  if (tab->num_motions < 1) return fail(SMPLSIM_EINVAL, "smplsim_imitation: num_motions < 1");
+  // every table check, NULL tables included, precedes the self_obs_dim check: a call with both wrong reports the tables
+  ImArgs a; std::memset(&a, 0, sizeof a);
+  const std::string why = motion_tables(H, tab, a);
+  if (!why.empty()) return fail(SMPLSIM_EINVAL, "smplsim_imitation: " + why);
   if (cfg->self_obs_dim != H.self_obs_dim) return fail(SMPLSIM_EINVAL, "smplsim_imitation: self_obs_dim is not the handle's self-observation width");
-  if (!tab->xpos || !tab->xquat || !tab->body_vel || !tab->body_ang_vel || !tab->motion_len || !tab->num_frames || !tab->motion_dt || !tab->length_starts)
-    return fail(SMPLSIM_EINVAL, "smplsim_imitation: null motion table");
   if (!aux->xpos || !aux->xquat || !aux->body_linvel || !aux->body_angvel) return fail(SMPLSIM_EINVAL, "smplsim_imitation: aux needs xpos, xquat, body_linvel, body_angvel");
   if (!motion_ids_dev || !motion_t0_dev || !progress_dev || !self_obs_dev || !obs_dev) return fail(SMPLSIM_EINVAL, "smplsim_imitation: null argument");
   if (!obs_only && (!reward_dev || !terminated_dev || !truncated_dev || !mpjpe_dev)) return fail(SMPLSIM_EINVAL, "smplsim_imitation: null reward / flag / mpjpe output");
@@ -710,9 +723,6 @@ static int imitation(SmplsimHandle* h, const SmplsimImitationCfg* cfg, const Smp
   const bool power = r.power_coefficient > 0.f || r.power;
   if (power && (!r.qvel || !aux->ctrl)) return fail(SMPLSIM_EINVAL, "smplsim_imitation: the power needs qvel and aux.ctrl");
   DeviceGuard guard(h->device);
-  ImArgs a; std::memset(&a, 0, sizeof a);
-  a.txpos = tab->xpos; a.txquat = tab->xquat; a.tvel = tab->body_vel; a.tangvel = tab->body_ang_vel;
-  a.mlen = tab->motion_len; a.nframes = tab->num_frames; a.mdt = tab->motion_dt; a.starts = tab->length_starts; a.nmotion = tab->num_motions;
   a.ids = motion_ids_dev; a.t0 = motion_t0_dev; a.progress = progress_dev; a.mask = mask_dev;
   a.xpos = aux->xpos; a.xquat = aux->xquat; a.linvel = aux->body_linvel; a.angvel = aux->body_angvel; a.status = aux->status;
   a.self_obs = self_obs_dev; a.obs = obs_dev; a.reward = reward_dev; a.mpjpe = mpjpe_dev; a.terminated = terminated_dev; a.truncated = truncated_dev;
@@ -726,25 +736,14 @@ static int imitation(SmplsimHandle* h, const SmplsimImitationCfg* cfg, const Smp
   ImRec rk; std::memset(&rk, 0, sizeof rk);
   rk.zof = r.zero_out_far; rk.far = r.far_distance; rk.power_k = r.power_coefficient; rk.nu = H.nu; rk.nv = H.nv;
   rk.recovery = r.recovery; rk.goal = r.goal_dist; rk.qvel = r.qvel; rk.ctrl = aux->ctrl; rk.power = r.power;
-  const int wpb = 8, grid = (a.n + wpb - 1) / wpb;
-  const bool multi = a.T > 1;
-  // fail-state recovery runs in its own instances, so that with every recovery field zero the task is the one before it existed
+  // [interpolate][more than one target][recovery]; fail-state recovery runs in its own instances, so that with every recovery field
+  // zero the task is the one before it existed
+  static void (*const kernels[2][2][2])(const float*, ImArgs, ImRec) = {
+      {{k_imitation<0, 0, 0>, k_imitation<0, 0, 1>}, {k_imitation<0, 1, 0>, k_imitation<0, 1, 1>}},
+      {{k_imitation<1, 0, 0>, k_imitation<1, 0, 1>}, {k_imitation<1, 1, 0>, k_imitation<1, 1, 1>}}};
   const bool rec = r.zero_out_far || power || r.recovery || r.goal_dist;
-  if (rec) {
-    if (cfg->interpolate) {
-      if (multi) L_LAUNCH((k_imitation<1, 1, 1>), grid, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a, rk);
-      else L_LAUNCH((k_imitation<1, 0, 1>), grid, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a, rk);
-    } else {
-      if (multi) L_LAUNCH((k_imitation<0, 1, 1>), grid, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a, rk);
-      else L_LAUNCH((k_imitation<0, 0, 1>), grid, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a, rk);
-    }
-  } else if (cfg->interpolate) {
-    if (multi) L_LAUNCH((k_imitation<1, 1, 0>), grid, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a, rk);
-    else L_LAUNCH((k_imitation<1, 0, 0>), grid, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a, rk);
-  } else {
-    if (multi) L_LAUNCH((k_imitation<0, 1, 0>), grid, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a, rk);
-    else L_LAUNCH((k_imitation<0, 0, 0>), grid, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a, rk);
-  }
+  const int wpb = 8, grid = (a.n + wpb - 1) / wpb;
+  L_LAUNCH(kernels[cfg->interpolate][a.T > 1][rec], grid, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a, rk);
   CUDA_TRY(cudaGetLastError());
   return SMPLSIM_OK;
 }
@@ -778,10 +777,10 @@ extern "C" int smplsim_track_eval(SmplsimHandle* h, const SmplsimTrackEvalCfg* c
   if (cfg->bodies)
     for (int j = 0; j < cfg->num_bodies; j++)
       if (cfg->bodies[j] < 0 || cfg->bodies[j] >= H.nb) return fail(SMPLSIM_EINVAL, "smplsim_track_eval: eval body out of range [0, nbody)");
-  if (tab->nbody != H.nb) return fail(SMPLSIM_EINVAL, "smplsim_track_eval: the tables' nbody is not the handle's");
-  if (tab->num_motions < 1) return fail(SMPLSIM_EINVAL, "smplsim_track_eval: num_motions < 1");
-  if (!tab->xpos || !tab->xquat || !tab->body_vel || !tab->body_ang_vel || !tab->motion_len || !tab->num_frames || !tab->motion_dt || !tab->length_starts)
-    return fail(SMPLSIM_EINVAL, "smplsim_track_eval: null motion table");
+  TeArgs t; std::memset(&t, 0, sizeof t);
+  ImArgs& a = t.im;
+  const std::string why = motion_tables(H, tab, a);
+  if (!why.empty()) return fail(SMPLSIM_EINVAL, "smplsim_track_eval: " + why);
   if (!aux->xpos || !aux->xquat) return fail(SMPLSIM_EINVAL, "smplsim_track_eval: aux needs xpos, xquat");
   if (!motion_ids_dev || !motion_t0_dev || !progress_dev || !terminated_dev || !truncated_dev) return fail(SMPLSIM_EINVAL, "smplsim_track_eval: null argument");
   if (!state->active || !state->prev_diff || !state->frames || !state->sums || !state->success)
@@ -789,10 +788,6 @@ extern "C" int smplsim_track_eval(SmplsimHandle* h, const SmplsimTrackEvalCfg* c
   if (cfg->interpolate != 0 && cfg->interpolate != 1) return fail(SMPLSIM_EINVAL, "smplsim_track_eval: interpolate must be 0 or 1");
   if (!(cfg->dt >= 0.f)) return fail(SMPLSIM_EINVAL, "smplsim_track_eval: dt < 0 or NaN");
   DeviceGuard guard(h->device);
-  TeArgs t; std::memset(&t, 0, sizeof t);
-  ImArgs& a = t.im;
-  a.txpos = tab->xpos; a.txquat = tab->xquat; a.tvel = tab->body_vel; a.tangvel = tab->body_ang_vel;
-  a.mlen = tab->motion_len; a.nframes = tab->num_frames; a.mdt = tab->motion_dt; a.starts = tab->length_starts; a.nmotion = tab->num_motions;
   a.ids = motion_ids_dev; a.t0 = motion_t0_dev; a.progress = progress_dev;
   a.xpos = aux->xpos; a.xquat = aux->xquat;
   a.dt = cfg->dt > 0.f ? cfg->dt : (float)h->ctrl_dt;
@@ -831,14 +826,10 @@ static std::string amp_check(const SmplsimHandle* h, const SmplsimAmpCfg* cfg, i
 }
 static std::string amp_tables(const LHdr& H, const SmplsimAmpTables* tab, AmpArgs& a) {
   if (!tab || !tab->motion) return "null motion tables";
-  const SmplsimMotionTables* m = tab->motion;
-  if (m->nbody != H.nb) return "the tables' nbody is not the handle's";
-  if (m->num_motions < 1) return "num_motions < 1";
-  if (!m->xpos || !m->xquat || !m->body_vel || !m->body_ang_vel || !m->motion_len || !m->num_frames || !m->motion_dt || !m->length_starts ||
-      !tab->dof_pos || !tab->dof_vel)
-    return "null motion table";
-  a.txpos = m->xpos; a.txquat = m->xquat; a.tvel = m->body_vel; a.tangvel = m->body_ang_vel; a.tdof = tab->dof_pos; a.tdofv = tab->dof_vel;
-  a.mlen = m->motion_len; a.nframes = m->num_frames; a.mdt = m->motion_dt; a.starts = m->length_starts; a.nmotion = m->num_motions;
+  const std::string why = motion_tables(H, tab->motion, a);
+  if (!why.empty()) return why;
+  if (!tab->dof_pos || !tab->dof_vel) return "null motion table";
+  a.tdof = tab->dof_pos; a.tdofv = tab->dof_vel;
   return "";
 }
 static void amp_common(const SmplsimHandle* h, const SmplsimAmpCfg* cfg, AmpArgs& a) {

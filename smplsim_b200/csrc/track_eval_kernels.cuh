@@ -94,7 +94,7 @@ __global__ void __launch_bounds__(256) k_track_eval(TeArgs t) {
   const int e = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (e >= a.n || !t.active[e]) return;   // warp-uniform
   const int nb = a.nb, J = a.J;
-  const int id = min(max(a.ids[e], 0), a.nmotion - 1);
+  const int id = motion_clip(a, a.ids[e]);
   const float len = a.mlen[id], mdt = a.mdt[id], t0 = a.t0[e];
   const int nf = a.nframes[id], start = a.starts[id], p = a.progress[e];
   const ImRef<INTERP> ref(a, im_frame<INTERP>(len, mdt, nf, start, fmaf((float)p, a.dt, t0)));   // the row k_imitation's reward compares
@@ -118,7 +118,7 @@ __global__ void __launch_bounds__(256) k_track_eval(TeArgs t) {
       if (f >= 1) { const V3 dv = d - ld3(d1 + 3 * j); sv += sqrtf(dot(dv, dv)); }
       if (f >= 2) { const V3 da = (d - ld3(d1 + 3 * j)) - (ld3(d1 + 3 * j) - ld3(d2 + 3 * j)); sa += sqrtf(dot(da, da)); }
       st3(d2 + 3 * j, d);
-      const Q4 dq = qmul(ref.quat(b), im_conj(im_ldq(xq + 4 * b)));
+      const Q4 dq = qmul(ref.quat(b), im_conj(mb_ldq(xq + 4 * b)));
       sr += 2.0f * atan2f(sqrtf(dq.x * dq.x + dq.y * dq.y + dq.z * dq.z), fabsf(dq.w));
     }
   }

@@ -19,8 +19,7 @@ from typing import Any, Callable, Dict, List, Optional, Sequence, Union
 import numpy as np
 import torch
 
-from .abi import (TRACK_METRICS, SmplsimImitationCfgC, SmplsimImitationRecoveryC, SmplsimMotionTablesC, SmplsimTrackEvalCfgC,
-                  SmplsimTrackEvalStateC)
+from .abi import TRACK_METRICS, SmplsimImitationCfgC, SmplsimImitationRecoveryC, SmplsimTrackEvalCfgC, SmplsimTrackEvalStateC
 from .batched import HumanoidBatchB200, _ptr
 from .motion_lib import MotionLibB200
 
@@ -98,11 +97,7 @@ class HumanoidImB200:
             termination_distance=float(e.termination_distance), episode_length=self.max_episode_length, self_obs_dim=int(b.num_obs),
             num_tracked=len(bodies), tracked_bodies=self._bodies.ctypes.data if len(bodies) else None, interpolate=int(self.interpolate),
             num_future=self.num_future, future_dt=1.0 / inv)
-        self._tab = SmplsimMotionTablesC(
-            xpos=lib.tables["xpos"].data_ptr(), xquat=lib.tables["xquat"].data_ptr(), body_vel=lib.tables["body_vel"].data_ptr(),
-            body_ang_vel=lib.tables["body_ang_vel"].data_ptr(), motion_len=lib._motion_lengths.data_ptr(),
-            num_frames=lib._motion_num_frames.data_ptr(), motion_dt=lib._motion_dt.data_ptr(), length_starts=lib.length_starts.data_ptr(),
-            num_motions=lib.num_motions(), nbody=lib.tables["xpos"].shape[1] // 3)
+        self._tab = lib.c_tables
         self.num_obs = b.num_obs + (L.smplsim_imitation_obs_dim(b._h, len(bodies)) - b.num_obs) * self.num_future
         f32 = dict(dtype=torch.float32, device=dv)
         u8 = dict(dtype=torch.uint8, device=dv)

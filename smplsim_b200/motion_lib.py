@@ -15,6 +15,7 @@ from typing import Dict
 import numpy as np
 import torch
 
+from .abi import SmplsimAmpTablesC, SmplsimMotionTablesC
 from .batched import HumanoidBatchB200
 
 TABLE_KEYS = ("qpos", "qvel", "xpos", "xquat", "body_vel", "body_ang_vel", "dof_pos", "dof_vel")
@@ -102,6 +103,12 @@ class MotionLibB200:
         self.curr_failed_keys = []
         self._gen = torch.Generator(device=dv)
         self._gen.manual_seed(int(getattr(env, "seed", 0)) & 0x7FFFFFFF)
+        # the tables as the imitation, evaluation and AMP entry points take them; they point into the tensors above
+        t = self.tables
+        self.c_tables = SmplsimMotionTablesC(
+            xpos=t["xpos"].data_ptr(), xquat=t["xquat"].data_ptr(), body_vel=t["body_vel"].data_ptr(), body_ang_vel=t["body_ang_vel"].data_ptr(),
+            motion_len=self._motion_lengths.data_ptr(), num_frames=self._motion_num_frames.data_ptr(), motion_dt=self._motion_dt.data_ptr(),
+            length_starts=self.length_starts.data_ptr(), num_motions=K, nbody=t["xpos"].shape[1] // 3)
 
     def num_motions(self):
         return int(self._motion_lengths.shape[0])
@@ -196,14 +203,9 @@ class MotionLibB200:
         self._amp_ccfg, self._amp_keys = amp_c_cfg(self.env.model, self.amp_cfg)
 
     def _amp_tables(self):
-        from .abi import SmplsimAmpTablesC, SmplsimMotionTablesC
         if getattr(self, "_amp_tab", None) is None:
             t = self.tables
-            self._amp_mtab = SmplsimMotionTablesC(
-                xpos=t["xpos"].data_ptr(), xquat=t["xquat"].data_ptr(), body_vel=t["body_vel"].data_ptr(), body_ang_vel=t["body_ang_vel"].data_ptr(),
-                motion_len=self._motion_lengths.data_ptr(), num_frames=self._motion_num_frames.data_ptr(), motion_dt=self._motion_dt.data_ptr(),
-                length_starts=self.length_starts.data_ptr(), num_motions=self.num_motions(), nbody=t["xpos"].shape[1] // 3)
-            self._amp_tab = SmplsimAmpTablesC(motion=C.addressof(self._amp_mtab), dof_pos=t["dof_pos"].data_ptr(), dof_vel=t["dof_vel"].data_ptr())
+            self._amp_tab = SmplsimAmpTablesC(motion=C.addressof(self.c_tables), dof_pos=t["dof_pos"].data_ptr(), dof_vel=t["dof_vel"].data_ptr())
         return self._amp_tab
 
     def amp_obs_demo(self, n=None, motion_ids=None, motion_times=None, out=None):
