@@ -83,6 +83,25 @@ static long count_blocks(const SmplsimHandle* h, long per) {
   return b;
 }
 
+// The lane kernels a handle of class C may launch.  pick_wpb raises the shared-memory cap of every entry and the launches take their
+// kernel from here, so that no instance runs under the default cap.
+struct LaneKernels {
+  void (*step[3])(const float*, int, LStepArgs, const float*, float*);   // [0 plain, 1 external wrench, 2 wrench + parameter records]
+  void (*reset[2])(const float*, int, LResetArgs);                      // [parameter records]
+  void (*kin)(const float*, int, LKinArgs);
+  void (*inverse[2])(const float*, int, LInvArgs);                      // [parameter records]
+  void (*dyn[2])(const float*, int, LDynArgs);                          // [parameter records]
+};
+template <class C>
+static LaneKernels lane_kernels() {
+  typedef typename C::WithPrm P;
+  LaneKernels k = {{k_step5<C>, k_step5<typename C::WithXfrc>, k_step5<typename C::WithXfrcPrm>}, {k_reset5<C>, k_reset5<P>}, k_kin5<C>, {}, {}};
+  // a self-collision class has no inverse instances (smplsim_inverse refuses such handles): NULL entries, so that none is compiled
+  if constexpr (!C::SELFCOL) { k.inverse[0] = k_inverse5<C>; k.inverse[1] = k_inverse5<P>; }
+  k.dyn[0] = k_dyn5<C>; k.dyn[1] = k_dyn5<P>;
+  return k;
+}
+
 // warps per CTA: fewest waves over the SMs first, then the fewest warps (an SM issues faster for few resident warps)
 template <class C>
 static int pick_wpb(SmplsimHandle* h) {
@@ -104,95 +123,31 @@ static int pick_wpb(SmplsimHandle* h) {
   // opt-in limit rather than to this handle's need, so that a handle created later with smaller CTAs (fewer envs) does not
   // lower the cap under the launches of a live handle with larger ones.  The lane kernels declare no static __shared__ (their
   // only shared memory is the dynamic l_smem4), so the whole opt-in limit is a legal dynamic cap for each of them.
-  const int cap = h->max_smem;
-  if (cudaFuncSetAttribute(k_step5<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap) != cudaSuccess) return -1;
-  if (cudaFuncSetAttribute(k_step5<typename C::WithXfrc>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap) != cudaSuccess) return -1;
-  if (cudaFuncSetAttribute(k_step5<typename C::WithXfrcPrm>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap) != cudaSuccess) return -1;
-  if (cudaFuncSetAttribute(k_reset5<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap) != cudaSuccess) return -1;
-  if (cudaFuncSetAttribute(k_reset5<typename C::WithPrm>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap) != cudaSuccess) return -1;
-  if (cudaFuncSetAttribute(k_kin5<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap) != cudaSuccess) return -1;
-  if constexpr (!C::SELFCOL) {
-    if (cudaFuncSetAttribute(k_inverse5<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap) != cudaSuccess) return -1;
-    if (cudaFuncSetAttribute(k_inverse5<typename C::WithPrm>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap) != cudaSuccess) return -1;
-  }
-  if (cudaFuncSetAttribute(k_dyn5<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap) != cudaSuccess) return -1;
-  if (cudaFuncSetAttribute(k_dyn5<typename C::WithPrm>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap) != cudaSuccess) return -1;
+  auto raise = [cap = h->max_smem](auto... k) {   // in order, stopping at the first failure
+    return ((!k || cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, cap) == cudaSuccess) && ...);
+  };
+  const LaneKernels K = lane_kernels<C>();
+  if (!raise(K.step[0], K.step[1], K.step[2], K.reset[0], K.reset[1], K.kin, K.inverse[0], K.inverse[1], K.dyn[0], K.dyn[1])) return -1;
   return best;
 }
 
-// step and mj_step: the instance with the external-wrench code compiled in only when the caller passes xfrc_applied (same layout,
-// shared memory and CTA size; without a wrench the kernel is the one without that code).  The contact wrench output is a run-time
-// argument of every instance (NULL: not written).  While the handle has per-env parameter records, the instance with both the
-// parameter reads and the wrench code runs (its wrench pointer may be NULL).
-template <class C>
-static void run_step(SmplsimHandle* h, const LStepArgs& a, const float* xfrc, float* cwrench, cudaStream_t st) {
-  int wpb = h->wpb, per = wpb * C::EPW, grid = h->nblocks ? h->nblocks : (a.n + per - 1) / per;
-  if (h->prm) L_LAUNCH(k_step5<typename C::WithXfrcPrm>, grid, 32 * wpb, h->smem, st, h->dimg, h->img.hdr()->bytes, a, xfrc, cwrench);
-  else if (xfrc) L_LAUNCH(k_step5<typename C::WithXfrc>, grid, 32 * wpb, h->smem, st, h->dimg, h->img.hdr()->bytes, a, xfrc, cwrench);
-  else L_LAUNCH(k_step5<C>, grid, 32 * wpb, h->smem, st, h->dimg, h->img.hdr()->bytes, a, nullptr, cwrench);
+// One launch of a lane kernel over `rows` envs, or over the handle's CTAs when it groups envs by body shape
+template <class C, class K, class... A>
+static void lane_launch(const SmplsimHandle* h, K kern, int rows, cudaStream_t st, const A&... args) {
+  const int per = h->wpb * C::EPW, grid = h->nblocks ? h->nblocks : (rows + per - 1) / per;
+  L_LAUNCH(kern, grid, 32 * h->wpb, h->smem, st, h->dimg, h->img.hdr()->bytes, args...);
 }
-template <class C>
-static void run_reset(SmplsimHandle* h, const LResetArgs& a, float* cwrench, cudaStream_t st) {
-  int wpb = h->wpb, per = wpb * C::EPW, grid = h->nblocks ? h->nblocks : (a.n + per - 1) / per;
-  if (h->prm) L_LAUNCH(k_reset5<typename C::WithPrm>, grid, 32 * wpb, h->smem, st, h->dimg, h->img.hdr()->bytes, a);
-  else L_LAUNCH(k_reset5<C>, grid, 32 * wpb, h->smem, st, h->dimg, h->img.hdr()->bytes, a);
-  if (cwrench) {
-    const int row = 6 * h->img.hdr()->nb;
-    L_LAUNCH(k_zero_wrench, (int)(((long)a.n * row + 255) / 256), 256, 0, st, cwrench, a.mask, a.n, row);
-  }
-}
-template <class C>
-static void run_kin(SmplsimHandle* h, const LKinArgs& a, cudaStream_t st) {
-  int wpb = h->wpb, per = wpb * C::EPW;
-  L_LAUNCH(k_kin5<C>, h->nblocks ? h->nblocks : (a.n + per - 1) / per, 32 * wpb, h->smem, st, h->dimg, h->img.hdr()->bytes, a);
-}
-// inverse dynamics: instances without the geom-geom rows only (smplsim_inverse refuses self-collision handles).  One shape: launches of
-// at most num_envs rows (the handle's scratch rows), in order on the caller's stream; per-env shapes: n == num_envs, one launch.
-// Per-env parameter records: n == num_envs, one launch of the instance that reads them (row i = env i).
-template <class C>
-static void run_inverse(SmplsimHandle* h, const LInvArgs& a, cudaStream_t st) {
-  if constexpr (!C::SELFCOL) {
-    const LHdr& H = *h->img.hdr();
-    const int wpb = h->wpb, per = wpb * C::EPW;
-    if (h->prm) {
-      L_LAUNCH(k_inverse5<typename C::WithPrm>, h->nblocks ? h->nblocks : (a.n + per - 1) / per, 32 * wpb, h->smem, st, h->dimg, H.bytes, a);
-      return;
-    }
-    if (h->nblocks) {
-      L_LAUNCH(k_inverse5<C>, h->nblocks, 32 * wpb, h->smem, st, h->dimg, H.bytes, a);
-      return;
-    }
-    for (int r0 = 0; r0 < a.n; r0 += h->num_envs) {
-      LInvArgs c = a;
-      c.n = std::min(h->num_envs, a.n - r0);
-      c.qpos += (size_t)r0 * (H.nv + 1); c.qvel += (size_t)r0 * H.nv; c.qacc += (size_t)r0 * H.nv; c.qfrc += (size_t)r0 * H.nv;
-      if (c.cwrench) c.cwrench += (size_t)r0 * H.nb * 6;
-      L_LAUNCH(k_inverse5<C>, (c.n + per - 1) / per, 32 * wpb, h->smem, st, h->dimg, H.bytes, c);
-    }
-  }
-}
-// mass matrix / bias / Jacobians: every instance (no contact rows).  Chunked as the inverse.
-template <class C>
-static void run_dynamics(SmplsimHandle* h, const LDynArgs& a, cudaStream_t st) {
-  const LHdr& H = *h->img.hdr();
-  const int wpb = h->wpb, per = wpb * C::EPW;
-  if (h->prm) {
-    L_LAUNCH(k_dyn5<typename C::WithPrm>, h->nblocks ? h->nblocks : (a.n + per - 1) / per, 32 * wpb, h->smem, st, h->dimg, H.bytes, a);
-    return;
-  }
-  if (h->nblocks) {
-    L_LAUNCH(k_dyn5<C>, h->nblocks, 32 * wpb, h->smem, st, h->dimg, H.bytes, a);
-    return;
-  }
+// inverse / dynamics on n caller rows of state.  One shape without parameter records: launches of at most num_envs rows (the
+// handle's scratch rows), in order on the caller's stream, `advance` moving every row pointer of a chunk to its first row.  Otherwise
+// (env_rows holds n == num_envs) one launch, of the instance that reads the records while the handle has them (row i = env i).
+template <class C, class A, class F>
+static void state_rows(const SmplsimHandle* h, void (*const kern[2])(const float*, int, A), const A& a, F advance, cudaStream_t st) {
+  if (h->prm || h->nblocks) return lane_launch<C>(h, kern[h->prm ? 1 : 0], a.n, st, a);
   for (int r0 = 0; r0 < a.n; r0 += h->num_envs) {
-    LDynArgs c = a;
+    A c = a;
     c.n = std::min(h->num_envs, a.n - r0);
-    c.qpos += (size_t)r0 * (H.nv + 1);
-    if (c.qvel) c.qvel += (size_t)r0 * H.nv;
-    if (c.qM) c.qM += (size_t)r0 * H.nv * H.nv;
-    if (c.bias) c.bias += (size_t)r0 * H.nv;
-    if (c.jac) c.jac += (size_t)r0 * c.njac * 6 * H.nv;
-    L_LAUNCH(k_dyn5<C>, (c.n + per - 1) / per, 32 * wpb, h->smem, st, h->dimg, H.bytes, c);
+    advance(c, (size_t)r0);
+    lane_launch<C>(h, kern[0], c.n, st, c);
   }
 }
 // dispatch over (model class, self-collision)
@@ -270,17 +225,14 @@ static int create_impl(const SmplsimModelDesc* s, int nmodels, const int32_t* en
   if (e == cudaSuccess) e = cudaDeviceGetAttribute(&h->nsm, cudaDevAttrMultiProcessorCount, cuda_device);
 #endif
   if (e != cudaSuccess) { delete h; return fail(SMPLSIM_ECUDA, std::string("smplsim_create: ") + cudaGetErrorString(e)); }
-  int ok = 0;
-  L_DISPATCH(h, ok = pick_wpb<C_>(h));
+  int ok = 0, per = 1;   // the class constants: warps per CTA (and its shared memory, in h), envs per CTA, scratch words per env
+  size_t gs = 0, pw = 0;
+  L_DISPATCH(h, ok = pick_wpb<C_>(h); per = h->wpb * C_::EPW; gs = C_::GSCRW; pw = C_::PFLW);
   if (ok <= 0) { delete h; return fail(SMPLSIM_EUNSUPPORTED, "per-env rows exceed shared memory"); }
-  size_t gs = 0;
-  L_DISPATCH(h, gs = (size_t)C_::GSCRW);
   e = cudaMalloc(&h->dimg, (size_t)H.bytes * nmodels);
   if (e == cudaSuccess) e = cudaMemcpy(h->dimg, h->img.bytes.data(), H.bytes, cudaMemcpyHostToDevice);
   for (int k = 1; k < nmodels && e == cudaSuccess; k++) e = cudaMemcpy((char*)h->dimg + (size_t)H.bytes * k, more[k - 1].bytes.data(), H.bytes, cudaMemcpyHostToDevice);
   if (e == cudaSuccess && !h->env_model.empty()) {   // envs grouped by shape into whole CTAs (empty slots: -1)
-    int per = 1;
-    L_DISPATCH(h, per = h->wpb * C_::EPW);
     std::vector<int> slot_env, blk_img;
     for (int k = 0; k < nmodels; k++) {
       int fill = 0;
@@ -302,8 +254,6 @@ static int create_impl(const SmplsimModelDesc* s, int nmodels, const int32_t* en
   }
   if (e == cudaSuccess) e = cudaMalloc(&h->gscr, gs * (size_t)num_envs * 4 + 16);
   if (e == cudaSuccess) e = cudaMalloc(&h->gsens, (size_t)6 * H.nb * num_envs * 4);
-  size_t pw = 0;
-  L_DISPATCH(h, pw = (size_t)C_::PFLW);
   if (e == cudaSuccess) e = cudaMalloc(&h->gpfl, pw * num_envs * 4);
   if (e == cudaSuccess) e = cudaMemset(h->gpfl, 0, pw * num_envs * 4);
   if (e == cudaSuccess && cfg->self_collision) e = cudaMalloc(&h->gbody, (size_t)10 * H.nb * num_envs * 4);
@@ -338,26 +288,41 @@ extern "C" int smplsim_warps_per_block(const SmplsimHandle* h) { return h ? h->w
 extern "C" int smplsim_kernel_version(const SmplsimHandle* h) { return h ? 5 : SMPLSIM_EINVAL; }
 extern "C" int smplsim_schedule_steps(const SmplsimHandle* h) { return h ? h->img.hdr()->T : SMPLSIM_EINVAL; }
 
-static LState lane_state(const SmplsimState* st) {   // the rows before xfrc_applied, in the same order
-  static_assert(sizeof(LState) == offsetof(SmplsimState, xfrc_applied), "LState must mirror SmplsimState up to xfrc_applied");
-  LState s;
-  std::memcpy(&s, st, sizeof s);
-  return s;
-}
-static LAux lane_aux(const SmplsimAux* aux) {   // the rows before contact_wrench, in the same order (all NULL without aux)
-  static_assert(sizeof(LAux) == offsetof(SmplsimAux, contact_wrench), "LAux must mirror SmplsimAux up to contact_wrench");
-  LAux x;
-  std::memset(&x, 0, sizeof x);
-  if (aux) std::memcpy(&x, aux, sizeof x);
-  return x;
-}
 static float* aux_wrench(const SmplsimAux* aux) { return aux ? aux->contact_wrench : nullptr; }
 static bool state_ok(const SmplsimState* st) {
   return st && st->qpos && st->qvel && st->qpos_fwd && st->qvel_fwd && st->qacc_warm && st->task_target && st->task_change_step &&
          st->progress && st->recovery && st->rng_counter;
 }
-static int want_sens(const SmplsimHandle* h, const SmplsimAux* aux) {
-  return (h->img.hdr()->cfg.self_obs_v == 2 || (aux && (aux->body_linvel || aux->body_angvel))) ? 1 : 0;
+// the arguments step, mj_step and reset share (LStepArgs, LResetArgs): state and side-output rows, the handle's scratch, every env
+template <class A>
+static A lane_args(const SmplsimHandle* h, const SmplsimState* st, const SmplsimAux* aux) {
+  static_assert(sizeof(LState) == offsetof(SmplsimState, xfrc_applied), "LState must mirror SmplsimState up to xfrc_applied");
+  static_assert(sizeof(LAux) == offsetof(SmplsimAux, contact_wrench), "LAux must mirror SmplsimAux up to contact_wrench");
+  A a; std::memset(&a, 0, sizeof a);
+  std::memcpy(&a.st, st, sizeof a.st);     // the rows before xfrc_applied, in the same order
+  if (aux) std::memcpy(&a.aux, aux, sizeof a.aux);   // the rows before contact_wrench, in the same order (all NULL without aux)
+  a.gscr = h->gscr; a.gpfl = h->gpfl; a.gbody = h->gbody; a.n = h->num_envs; a.map = h->map();
+  const bool sens = h->img.hdr()->cfg.self_obs_v == 2 || (aux && (aux->body_linvel || aux->body_angvel));
+  a.gsens = sens ? h->gsens : nullptr;
+  return a;
+}
+// step and mj_step: the instance with the external-wrench code compiled in only when the caller passes xfrc_applied (same layout,
+// shared memory and CTA size; without a wrench the kernel is the one without that code).  The contact wrench output is a run-time
+// argument of every instance (NULL: not written).  While the handle has per-env parameter records, the instance with both the
+// parameter reads and the wrench code runs (its wrench pointer may be NULL).
+static int lane_step(const SmplsimHandle* h, const LStepArgs& a, const SmplsimState* st, const SmplsimAux* aux, void* stream) {
+  const float* xfrc = st->xfrc_applied;
+  L_DISPATCH(h, lane_launch<C_>(h, lane_kernels<C_>().step[h->prm ? 2 : xfrc ? 1 : 0], a.n, (cudaStream_t)stream, a, xfrc, aux_wrench(aux)));
+  CUDA_TRY(cudaGetLastError());
+  return SMPLSIM_OK;
+}
+// calls on n caller rows: with per-env body shapes, and for the kernels that read them (prm) per-env parameter records, row i is env i
+static int env_rows(const SmplsimHandle* h, int n, const char* fn, bool prm) {
+  if (h->nblocks && n != h->num_envs)
+    return fail(SMPLSIM_EINVAL, std::string(fn) + ": with per-env body shapes n must be the handle's num_envs (row i uses env i's shape)");
+  if (prm && h->prm && n != h->num_envs)
+    return fail(SMPLSIM_EINVAL, std::string(fn) + ": with per-env parameters n must be the handle's num_envs (row i uses env i's parameters)");
+  return SMPLSIM_OK;
 }
 
 extern "C" int smplsim_step(SmplsimHandle* h, const SmplsimState* st, const float* action_dev, float* obs_dev, float* reward_dev,
@@ -366,26 +331,18 @@ extern "C" int smplsim_step(SmplsimHandle* h, const SmplsimState* st, const floa
   if (h->img.hdr()->cfg.control_mode == SMPLSIM_CTRL_SIMPLE_PID && (!st->pid_integral || !st->pid_last_error))
     return fail(SMPLSIM_EINVAL, "smplsim_step: control_mode simple_pid needs state.pid_integral / pid_last_error");
   DeviceGuard guard(h->device);
-  LStepArgs a; std::memset(&a, 0, sizeof a);
-  a.st = lane_state(st); a.aux = lane_aux(aux);
+  LStepArgs a = lane_args<LStepArgs>(h, st, aux);
   a.action = action_dev; a.obs = obs_dev; a.reward = reward_dev; a.terminated = terminated_dev; a.truncated = truncated_dev;
-  a.gscr = h->gscr; a.gpfl = h->gpfl; a.gbody = h->gbody; a.n = h->num_envs; a.nsub = h->img.hdr()->cfg.nsubsteps; a.mode = 0; a.map = h->map();
-  a.gsens = want_sens(h, aux) ? h->gsens : nullptr;
-  L_DISPATCH(h, run_step<C_>(h, a, st->xfrc_applied, aux_wrench(aux), (cudaStream_t)stream));
-  CUDA_TRY(cudaGetLastError());
-  return SMPLSIM_OK;
+  a.nsub = h->img.hdr()->cfg.nsubsteps; a.mode = 0;
+  return lane_step(h, a, st, aux, stream);
 }
 
 extern "C" int smplsim_mj_step(SmplsimHandle* h, const SmplsimState* st, const float* ctrl_dev, int nsub, const SmplsimAux* aux, void* stream) {
   if (!h || !state_ok(st) || !ctrl_dev || nsub < 1) return fail(SMPLSIM_EINVAL, "smplsim_mj_step: bad argument");
   DeviceGuard guard(h->device);
-  LStepArgs a; std::memset(&a, 0, sizeof a);
-  a.st = lane_state(st); a.aux = lane_aux(aux);
-  a.action = ctrl_dev; a.gscr = h->gscr; a.gpfl = h->gpfl; a.gbody = h->gbody; a.n = h->num_envs; a.nsub = nsub; a.mode = 1; a.map = h->map();
-  a.gsens = want_sens(h, aux) ? h->gsens : nullptr;
-  L_DISPATCH(h, run_step<C_>(h, a, st->xfrc_applied, aux_wrench(aux), (cudaStream_t)stream));
-  CUDA_TRY(cudaGetLastError());
-  return SMPLSIM_OK;
+  LStepArgs a = lane_args<LStepArgs>(h, st, aux);
+  a.action = ctrl_dev; a.nsub = nsub; a.mode = 1;
+  return lane_step(h, a, st, aux, stream);
 }
 
 extern "C" int smplsim_reset(SmplsimHandle* h, const SmplsimState* st, const uint8_t* mask_dev, int init_mode, const float* qpos0_dev,
@@ -397,11 +354,13 @@ extern "C" int smplsim_reset(SmplsimHandle* h, const SmplsimState* st, const uin
   if (mode < 0 || mode > 2) return fail(SMPLSIM_EINVAL, "smplsim_reset: init_mode");
   if (mode == SMPLSIM_INIT_MOCAP && (!qpos0_dev || !qvel0_dev)) return fail(SMPLSIM_EINVAL, "smplsim_reset: MoCap init needs qpos0/qvel0");
   DeviceGuard guard(h->device);
-  LResetArgs a; std::memset(&a, 0, sizeof a);
-  a.st = lane_state(st); a.aux = lane_aux(aux);
-  a.mask = mask_dev; a.qpos0 = qpos0_dev; a.qvel0 = qvel0_dev; a.obs = obs_dev; a.gscr = h->gscr; a.gpfl = h->gpfl; a.gbody = h->gbody; a.n = h->num_envs; a.init_mode = mode; a.map = h->map();
-  a.gsens = want_sens(h, aux) ? h->gsens : nullptr;
-  L_DISPATCH(h, run_reset<C_>(h, a, aux_wrench(aux), (cudaStream_t)stream));
+  LResetArgs a = lane_args<LResetArgs>(h, st, aux);
+  a.mask = mask_dev; a.qpos0 = qpos0_dev; a.qvel0 = qvel0_dev; a.obs = obs_dev; a.init_mode = mode;
+  L_DISPATCH(h, lane_launch<C_>(h, lane_kernels<C_>().reset[h->prm ? 1 : 0], a.n, (cudaStream_t)stream, a));
+  if (float* cw = aux_wrench(aux)) {   // the reset runs no constraint solve: zero wrench rows for the envs it resets
+    const int row = 6 * h->img.hdr()->nb;
+    L_LAUNCH(k_zero_wrench, (int)(((long)a.n * row + 255) / 256), 256, 0, (cudaStream_t)stream, cw, a.mask, a.n, row);
+  }
   CUDA_TRY(cudaGetLastError());
   return SMPLSIM_OK;
 }
@@ -410,9 +369,9 @@ extern "C" int smplsim_kinematics(SmplsimHandle* h, const float* qpos_dev, float
   if (!h || !qpos_dev || !xpos_dev || !xquat_dev || n < 0) return fail(SMPLSIM_EINVAL, "smplsim_kinematics: bad argument");
   if (n == 0) return SMPLSIM_OK;
   DeviceGuard guard(h->device);
-  if (h->nblocks && n != h->num_envs) return fail(SMPLSIM_EINVAL, "smplsim_kinematics: with per-env body shapes n must be the handle's num_envs (row i uses env i's shape)");
+  if (int rc = env_rows(h, n, "smplsim_kinematics", false)) return rc;
   LKinArgs a; a.qpos = qpos_dev; a.xpos = xpos_dev; a.xquat = xquat_dev; a.n = n; a.map = h->map();
-  L_DISPATCH(h, run_kin<C_>(h, a, (cudaStream_t)stream));
+  L_DISPATCH(h, lane_launch<C_>(h, lane_kernels<C_>().kin, n, (cudaStream_t)stream, a));
   CUDA_TRY(cudaGetLastError());
   return SMPLSIM_OK;
 }
@@ -424,13 +383,17 @@ extern "C" int smplsim_inverse(SmplsimHandle* h, const float* qpos_dev, const fl
     return fail(SMPLSIM_EUNSUPPORTED, "smplsim_inverse: the inverse does not build geom-geom contacts (handle created with self_collision = 1)");
   if (n == 0) return SMPLSIM_OK;   // nothing is read: empty tensors may come as NULL
   if (!qpos_dev || !qvel_dev || !qacc_dev || !qfrc_inverse_dev) return fail(SMPLSIM_EINVAL, "smplsim_inverse: null argument");
-  if (h->nblocks && n != h->num_envs) return fail(SMPLSIM_EINVAL, "smplsim_inverse: with per-env body shapes n must be the handle's num_envs (row i uses env i's shape)");
-  if (h->prm && n != h->num_envs) return fail(SMPLSIM_EINVAL, "smplsim_inverse: with per-env parameters n must be the handle's num_envs (row i uses env i's parameters)");
+  if (int rc = env_rows(h, n, "smplsim_inverse", true)) return rc;
   DeviceGuard guard(h->device);
   LInvArgs a; std::memset(&a, 0, sizeof a);
   a.qpos = qpos_dev; a.qvel = qvel_dev; a.qacc = qacc_dev; a.qfrc = qfrc_inverse_dev; a.cwrench = contact_wrench_dev; a.gscr = h->gscr; a.n = n;
   a.map = h->map();
-  L_DISPATCH(h, run_inverse<C_>(h, a, (cudaStream_t)stream));
+  const size_t nv = h->img.hdr()->nv, nb = h->img.hdr()->nb;
+  auto advance = [nv, nb](LInvArgs& c, size_t r) {
+    c.qpos += r * (nv + 1); c.qvel += r * nv; c.qacc += r * nv; c.qfrc += r * nv;
+    if (c.cwrench) c.cwrench += r * nb * 6;
+  };
+  L_DISPATCH(h, state_rows<C_>(h, lane_kernels<C_>().inverse, a, advance, (cudaStream_t)stream));
   CUDA_TRY(cudaGetLastError());
   return SMPLSIM_OK;
 }
@@ -448,15 +411,22 @@ extern "C" int smplsim_dynamics(SmplsimHandle* h, const float* qpos_dev, const f
   if (njac > 0 && !jac_dev) return fail(SMPLSIM_EINVAL, "smplsim_dynamics: njac > 0 needs jac_dev");
   if (!qM_dev && !qfrc_bias_dev && !njac) return fail(SMPLSIM_EINVAL, "smplsim_dynamics: no output requested");
   if (!qpos_dev) return fail(SMPLSIM_EINVAL, "smplsim_dynamics: null qpos");
-  if (h->nblocks && n != h->num_envs) return fail(SMPLSIM_EINVAL, "smplsim_dynamics: with per-env body shapes n must be the handle's num_envs (row i uses env i's shape)");
-  if (h->prm && n != h->num_envs) return fail(SMPLSIM_EINVAL, "smplsim_dynamics: with per-env parameters n must be the handle's num_envs (row i uses env i's parameters)");
+  if (int rc = env_rows(h, n, "smplsim_dynamics", true)) return rc;
   DeviceGuard guard(h->device);
   LDynArgs a; std::memset(&a, 0, sizeof a);
   a.qpos = qpos_dev; a.qvel = qvel_dev; a.qM = qM_dev; a.bias = qfrc_bias_dev; a.jac = njac ? jac_dev : nullptr; a.gscr = h->gscr; a.n = n;
   a.njac = njac;
   for (int j = 0; j < njac; j++) a.jb[j] = (unsigned char)jac_body[j];
   a.map = h->map();
-  L_DISPATCH(h, run_dynamics<C_>(h, a, (cudaStream_t)stream));
+  const size_t nv = H.nv;
+  auto advance = [nv](LDynArgs& c, size_t r) {
+    c.qpos += r * (nv + 1);
+    if (c.qvel) c.qvel += r * nv;
+    if (c.qM) c.qM += r * nv * nv;
+    if (c.bias) c.bias += r * nv;
+    if (c.jac) c.jac += r * c.njac * 6 * nv;
+  };
+  L_DISPATCH(h, state_rows<C_>(h, lane_kernels<C_>().dyn, a, advance, (cudaStream_t)stream));
   CUDA_TRY(cudaGetLastError());
   return SMPLSIM_OK;
 }
@@ -488,7 +458,7 @@ extern "C" int smplsim_ray(SmplsimHandle* h, const float* xpos_dev, const float*
   if (nray <= 0) return fail(SMPLSIM_EINVAL, "smplsim_ray: nray <= 0");
   if (!dist_dev && !geomid_dev) return fail(SMPLSIM_EINVAL, "smplsim_ray: no output requested");
   if (!xpos_dev || !xquat_dev || !pnt_dev || !vec_dev) return fail(SMPLSIM_EINVAL, "smplsim_ray: null argument");
-  if (h->nblocks && n != h->num_envs) return fail(SMPLSIM_EINVAL, "smplsim_ray: with per-env body shapes n must be the handle's num_envs (row i uses env i's shape)");
+  if (int rc = env_rows(h, n, "smplsim_ray", false)) return rc;
   const long grid = (long)n * ((nray + R_THREADS - 1) / R_THREADS);
   if (grid > 0x7fffffffL) return fail(SMPLSIM_EINVAL, "smplsim_ray: n x nray too large for one launch");
   DeviceGuard guard(h->device);
@@ -513,7 +483,7 @@ extern "C" int smplsim_render(SmplsimHandle* h, const float* xpos_dev, const flo
   if (width <= 0 || height <= 0) return fail(SMPLSIM_EINVAL, "smplsim_render: width / height <= 0");
   if (!depth_dev && !seg_dev && !rgb_dev) return fail(SMPLSIM_EINVAL, "smplsim_render: no output requested");
   if (!xpos_dev || !xquat_dev) return fail(SMPLSIM_EINVAL, "smplsim_render: null xpos / xquat");
-  if (h->nblocks && n != h->num_envs) return fail(SMPLSIM_EINVAL, "smplsim_render: with per-env body shapes n must be the handle's num_envs (row i uses env i's shape)");
+  if (int rc = env_rows(h, n, "smplsim_render", false)) return rc;
   const bool prm = h->prm && cam->mode == SMPLSIM_CAM_TRACKCOM;   // the robot COM with the env's mass scales
   if (prm && n != h->num_envs) return fail(SMPLSIM_EINVAL, "smplsim_render: a TRACKCOM camera with per-env parameters needs n == num_envs (row i uses env i's masses)");
   const int tiles_x = (width + R_CTA_W - 1) / R_CTA_W, tiles = tiles_x * ((height + R_CTA_H - 1) / R_CTA_H);
@@ -796,9 +766,9 @@ extern "C" int smplsim_track_eval(SmplsimHandle* h, const SmplsimTrackEvalCfg* c
   t.terminated = terminated_dev; t.truncated = truncated_dev;
   t.active = state->active; t.prev_diff = state->prev_diff; t.frames = state->frames; t.sums = state->sums; t.success = state->success;
   t.frame_metrics = state->frame_metrics;
+  static void (*const kernels[2])(TeArgs) = {k_track_eval<0>, k_track_eval<1>};   // [interpolate]
   const int wpb = 8, grid = (a.n + wpb - 1) / wpb;
-  if (cfg->interpolate) L_LAUNCH(k_track_eval<1>, grid, 32 * wpb, 0, (cudaStream_t)stream, t);
-  else L_LAUNCH(k_track_eval<0>, grid, 32 * wpb, 0, (cudaStream_t)stream, t);
+  L_LAUNCH(kernels[cfg->interpolate], grid, 32 * wpb, 0, (cudaStream_t)stream, t);
   CUDA_TRY(cudaGetLastError());
   return SMPLSIM_OK;
 }
@@ -832,6 +802,7 @@ static std::string amp_tables(const LHdr& H, const SmplsimAmpTables* tab, AmpArg
   a.tdof = tab->dof_pos; a.tdofv = tab->dof_vel;
   return "";
 }
+static void (*const amp_kernels[2])(const float*, AmpArgs) = {k_amp_obs<0>, k_amp_obs<1>};   // [interpolate]
 static void amp_common(const SmplsimHandle* h, const SmplsimAmpCfg* cfg, AmpArgs& a) {
   const LHdr& H = *h->img.hdr();
   a.K = cfg->num_steps; a.F = amp_dim(H, cfg); a.nb = H.nb; a.nv = H.nv; a.nkey = cfg->num_key_bodies;
@@ -867,8 +838,7 @@ extern "C" int smplsim_amp_obs(SmplsimHandle* h, const SmplsimAmpCfg* cfg, const
   a.qpos = st->qpos; a.qvel = st->qvel; a.xpos = aux->xpos; a.xquat = aux->xquat; a.out = amp_obs_dev;
   a.n = h->num_envs; a.mode = mode;
   const int wpb = 8;
-  if (cfg->interpolate) L_LAUNCH(k_amp_obs<1>, (a.n + wpb - 1) / wpb, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a);
-  else L_LAUNCH(k_amp_obs<0>, (a.n + wpb - 1) / wpb, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a);
+  L_LAUNCH(amp_kernels[cfg->interpolate], (a.n + wpb - 1) / wpb, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a);
   CUDA_TRY(cudaGetLastError());
   return SMPLSIM_OK;
 }
@@ -888,8 +858,7 @@ extern "C" int smplsim_amp_demo(SmplsimHandle* h, const SmplsimAmpCfg* cfg, cons
   amp_common(h, cfg, a);
   a.ids = motion_ids_dev; a.t0 = motion_times_dev; a.out = out_dev; a.n = n; a.mode = AMP_DEMO;
   const int wpb = 8;
-  if (cfg->interpolate) L_LAUNCH(k_amp_obs<1>, (n + wpb - 1) / wpb, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a);
-  else L_LAUNCH(k_amp_obs<0>, (n + wpb - 1) / wpb, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a);
+  L_LAUNCH(amp_kernels[cfg->interpolate], (n + wpb - 1) / wpb, 32 * wpb, 0, (cudaStream_t)stream, h->dimg, a);
   CUDA_TRY(cudaGetLastError());
   return SMPLSIM_OK;
 }
