@@ -244,6 +244,47 @@ int smplsim_kinematics(SmplsimHandle* h, const float* qpos_dev, float* xpos_dev,
 int smplsim_inverse(SmplsimHandle* h, const float* qpos_dev, const float* qvel_dev, const float* qacc_dev,
                     float* qfrc_inverse_dev, float* contact_wrench_dev, int n, void* cuda_stream);
 
+/* mujoco.mj_forward on n caller rows: qpos[n,nq], qvel[n,nv], ctrl[n,nu] (raw joint torques, not clamped, as smplsim_mj_step takes
+ * them) and qacc_warmstart[n,nv] (NULL: zeros) -> qacc[n,nv] (required); contact_mask[n], solver_iter[n], status[n] (bits 1 - 16 as in
+ * SmplsimAux.status) and contact_wrench[n,nbody,6] (as SmplsimAux.contact_wrench) each NULL: not written.  The pass is the first
+ * substep's of smplsim_mj_step without the integration, from empty working-set memory: at an env's own state, ctrl and warm start it
+ * gives that substep's qacc up to the solver's tolerance (the step carries the working set of its previous call).  No auto-reset: a row
+ * with a non-finite input or qacc gets its status bits and unspecified values in that row only.  Takes no xfrc_applied and writes no
+ * per-env state (a later smplsim_step is unaffected).  Row rules of smplsim_inverse: single shape, any n >= 0 (launched in pieces of at
+ * most num_envs rows on the stream); per-env shapes or parameter records: n == num_envs, row i uses env i; self_collision = 1:
+ * SMPLSIM_EUNSUPPORTED. */
+int smplsim_forward(SmplsimHandle* h, const float* qpos_dev, const float* qvel_dev, const float* ctrl_dev, const float* qacc_warmstart_dev,
+                    int n, float* qacc_dev, uint64_t* contact_mask_dev, int32_t* solver_iter_dev, uint8_t* status_dev,
+                    float* contact_wrench_dev, void* cuda_stream);
+
+/* Finite-difference step derivatives, mujoco.mjd_transitionFD without sensors.  State tangent x = [dq (nv) ; qvel (nv)] with the root
+ * rotation tangent in the body frame (q (x) exp(d), as mj_integratePos / mj_differentiatePos), input u = ctrl (nu); one step is one
+ * smplsim_mj_step substep, x' = (q (+) h v', v') with v' = v + h qacc.  eps_qpos (rad / m), eps_qvel and eps_ctrl (N m) are the
+ * perturbations; centered != 0 differences x + eps against x - eps, else x + eps against the nominal.  fp32 needs far larger steps
+ * than MuJoCo's fp64 default of eps = 1e-6, which is rounding noise here: SMPLSIM_FD_DEFAULTS (1e-2, 1e-1, 1.0, centered) are the
+ * measured choice (DESIGN.md 2); for a fixed active set qacc is affine in ctrl, so eps_ctrl costs no accuracy. */
+typedef struct SmplsimFdCfg {
+  float eps_qpos, eps_qvel, eps_ctrl;
+  int32_t centered, pad_;
+} SmplsimFdCfg;
+#define SMPLSIM_FD_DEFAULTS {1e-2f, 1e-1f, 1.0f, 1, 0}
+#define SMPLSIM_FD_KINK 1    /* flags: the two solves of the column ended on different active sets (a contact row or joint limit switched
+                              * inside +-eps: the column straddles a kink of the dynamics); never set with centered = 0 */
+#define SMPLSIM_FD_SOLVER 2  /* flags: a solve of the column stopped at its iteration cap, dropped joint-limit rows or saw a non-finite value */
+/* Outputs per row, row-major; qacc required, the others each NULL: not written, not all of them NULL:
+ *   qacc[n,nv]              the nominal forward pass (smplsim_forward, no warm start);
+ *   dqacc[n,nv,2nv+nu]      d qacc / d [dq, qvel, ctrl];
+ *   A[n,2nv,2nv], B[n,2nv,nu]  MuJoCo's layout, A[i,j] = d x'_i / d x_j, assembled exactly from dqacc and the integrator (not by
+ *                          differencing next states, whose fp32 rounding would swamp the h dqacc part of A - I);
+ *   flags[n,2nv+nu]         SMPLSIM_FD_* bits per column.
+ * Column j's difference is divided by the fp32 difference of the inputs actually perturbed (2 eps for a root-rotation column); each
+ * perturbed solve starts from the row's nominal qacc with empty working-set memory.  Costs the nominal pass plus (1 + centered)
+ * (2nv + nu) forward passes per row, launched in pieces of num_envs on the stream without a host sync; writes no per-env state.
+ * Single-shape handles without parameter records only: per-env shapes, parameter records and self_collision = 1 give
+ * SMPLSIM_EUNSUPPORTED.  SMPLSIM_EINVAL: a null required argument, n < 0, an eps that is not finite and > 0, or no derivative output. */
+int smplsim_transition_fd(SmplsimHandle* h, const SmplsimFdCfg* cfg, const float* qpos_dev, const float* qvel_dev, const float* ctrl_dev,
+                          int n, float* qacc_dev, float* dqacc_dev, float* A_dev, float* B_dev, uint8_t* flags_dev, void* cuda_stream);
+
 /* Mass matrix, bias forces and body Jacobians on n caller rows qpos[n,nq], qvel[n,nv] (each output NULL: skipped):
  *   qM[n,nv,nv]          mujoco.mj_fullM(qM): the dense joint-space inertia, armature on the diagonal; exactly symmetric, exact zeros
  *                        where neither dof is an ancestor of the other;

@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .abi import SmplsimAuxC, SmplsimEnvParamsC, SmplsimStateC, env_cfg_from, model_from_cfg
+from .abi import SmplsimAuxC, SmplsimEnvParamsC, SmplsimFdCfgC, SmplsimStateC, env_cfg_from, model_from_cfg
 from .model import ModelDesc
 
 
@@ -366,6 +366,69 @@ class HumanoidBatchB200:
         self._check(self._L().smplsim_inverse(self._h, _ptr(q), _ptr(v), _ptr(a), _ptr(out), _ptr(cw), n, self._stream()))
         self.gpu_launches += 1
         return (out, cw) if contact_wrench else out
+
+    def forward(self, qpos: torch.Tensor, qvel: torch.Tensor, ctrl: torch.Tensor, qacc_warmstart: Optional[torch.Tensor] = None,
+                contact_wrench: bool = False):
+        """mujoco.mj_forward on caller rows: the accelerations of ``(qpos, qvel)`` under the raw joint torques ``ctrl`` (as ``mj_step``
+        takes them, not clamped), with the floor contacts and joint limits of that state.  ``qacc_warmstart`` (None: zeros) is where the
+        constraint solve starts.  Returns a dict of ``qacc [n, nv]``, ``contact_mask [n]`` (int64 bits as ``self.contact_mask``),
+        ``solver_iter [n]``, ``status [n]`` (bits as ``self.status``) and, when asked, ``contact_wrench [n, nbody, 6]`` (as
+        ``self.contact_wrench``).  The pass is the first substep of ``mj_step(ctrl, 1)`` without the integration, from empty working-set
+        memory.  A row with a non-finite input gets its status bits and unspecified values in that row only; there is no auto-reset.
+        Float32 tensors on this batch's device; row rules of ``inverse``.  Reads no env state and changes none; ``xfrc_applied`` is not
+        taken.  Not available with ``cfg.env.self_collision``."""
+        m = self.model
+        args = (("qpos", qpos, m.nq), ("qvel", qvel, m.nv), ("ctrl", ctrl, m.nu))
+        if qacc_warmstart is not None:
+            args += (("qacc_warmstart", qacc_warmstart, m.nv),)
+        rows = self._rows(args)
+        q, v, u = rows[:3]
+        w = rows[3] if qacc_warmstart is not None else None
+        n, dv = q.shape[0], self.device
+        out = {"qacc": torch.empty(n, m.nv, dtype=torch.float32, device=dv), "contact_mask": torch.empty(n, dtype=torch.int64, device=dv),
+               "solver_iter": torch.empty(n, dtype=torch.int32, device=dv), "status": torch.empty(n, dtype=torch.uint8, device=dv)}
+        if contact_wrench:
+            out["contact_wrench"] = torch.empty(n, m.nbody, 6, dtype=torch.float32, device=dv)
+        self._check(self._L().smplsim_forward(self._h, _ptr(q), _ptr(v), _ptr(u), _ptr(w), n, _ptr(out["qacc"]), _ptr(out["contact_mask"]),
+                                              _ptr(out["solver_iter"]), _ptr(out["status"]), _ptr(out.get("contact_wrench")), self._stream()))
+        self.gpu_launches += 1
+        return out
+
+    FD_EPS = (1e-2, 1e-1, 1.0)   # eps_qpos (rad / m), eps_qvel, eps_ctrl (N m): the fp32 steps DESIGN.md 2 measured
+
+    def transition_fd(self, qpos: torch.Tensor, qvel: torch.Tensor, ctrl: torch.Tensor, eps_qpos: float = FD_EPS[0],
+                      eps_qvel: float = FD_EPS[1], eps_ctrl: float = FD_EPS[2], centered: bool = True, dqacc: bool = False):
+        """Finite-difference derivatives of one ``mj_step`` substep at caller rows, as ``mujoco.mjd_transitionFD`` without sensors.
+        State tangent ``x = [dq (nv) ; qvel (nv)]`` (root rotation tangent in the body frame, ``q * exp(d)``), input ``u = ctrl (nu)``.
+        Returns a dict of
+
+        - ``qacc [n, nv]``: the nominal forward pass;
+        - ``A [n, 2nv, 2nv]``, ``B [n, 2nv, nu]``: ``dx'/dx``, ``dx'/du`` in MuJoCo's layout, assembled from ``dqacc`` and the
+          semi-implicit Euler step;
+        - ``flags [n, 2nv + nu]`` uint8 per column: 1 the two solves ended on different active sets (the column straddles a contact or
+          joint-limit switch; never set with ``centered=False``), 2 a solve hit the iteration cap, dropped rows or saw a non-finite value;
+        - ``dqacc [n, nv, 2nv + nu]`` when asked: ``d qacc / d [dq, qvel, ctrl]``.
+
+        ``eps_*`` are the perturbations; MuJoCo's fp64 default of 1e-6 is rounding noise in fp32, and the defaults are the measured
+        choice.  ``centered=False`` differences against the nominal (half the passes).  Float32 tensors on this batch's device, any n;
+        single-shape batches without per-env parameters (raises otherwise), not with ``cfg.env.self_collision``.  Reads no env state and
+        changes none."""
+        m = self.model
+        for name, e in (("eps_qpos", eps_qpos), ("eps_qvel", eps_qvel), ("eps_ctrl", eps_ctrl)):
+            if not (np.isfinite(e) and e > 0):
+                raise ValueError(f"{name} must be finite and > 0, got {e!r}")
+        q, v, u = self._rows((("qpos", qpos, m.nq), ("qvel", qvel, m.nv), ("ctrl", ctrl, m.nu)))
+        n, nx, f32 = q.shape[0], 2 * m.nv, dict(dtype=torch.float32, device=self.device)
+        ncol = nx + m.nu
+        out = {"qacc": torch.empty(n, m.nv, **f32), "A": torch.empty(n, nx, nx, **f32), "B": torch.empty(n, nx, m.nu, **f32),
+               "flags": torch.empty(n, ncol, dtype=torch.uint8, device=self.device)}
+        if dqacc:
+            out["dqacc"] = torch.empty(n, m.nv, ncol, **f32)
+        cfg = SmplsimFdCfgC(float(eps_qpos), float(eps_qvel), float(eps_ctrl), 1 if centered else 0, 0)
+        self._check(self._L().smplsim_transition_fd(self._h, C.byref(cfg), _ptr(q), _ptr(v), _ptr(u), n, _ptr(out["qacc"]), _ptr(out.get("dqacc")),
+                                                    _ptr(out["A"]), _ptr(out["B"]), _ptr(out["flags"]), self._stream()))
+        self.gpu_launches += 1
+        return out
 
     def dynamics(self, qpos: torch.Tensor, qvel: Optional[torch.Tensor] = None, mass_matrix: bool = True, bias: bool = True,
                  jac_bodies: Optional[Sequence] = None):

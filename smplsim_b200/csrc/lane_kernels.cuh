@@ -2751,3 +2751,209 @@ __global__ void __launch_bounds__(256, 1) k_dyn5(const float* __restrict__ gimg,
     l_copy_out<C>(a.bias + eo * H.nv, sm + C::qvel, H.nv, w);
   }
 }
+
+// ------------------------------------------------------------------ forward dynamics (mujoco.mj_forward) and transition derivatives (mjd_transitionFD)
+// Forward: per caller row, the first substep's forward pass of l_substeps (raw ctrl, no clamp) without the integration, from the
+// caller's warm start and empty working-set memory.  Column pass (ncol > 0): slot s of the launch works on row s / ncol and column
+// s % ncol of x = [dq (nv) ; qvel (nv)], u = ctrl (nu); it runs the forward pass at x + eps and (centered) x - eps, both warm-started from
+// the row's nominal qacc, and writes column col of dqacc, of A or B (semi-implicit Euler assembled from dqacc) and its flags.  Uses the
+// handle's per-env scratch of the slots it runs (lane records, overflow contact entries; the column pass also gfd); writes neither the
+// working-set memory nor the sensor rows, so the stepper cannot tell that it ran.
+#define L_FD_KINK 1     // SMPLSIM_FD_KINK: the two solves of the column ended on different active sets
+#define L_FD_SOLVER 2   // SMPLSIM_FD_SOLVER: a solve of the column hit the iteration cap, dropped rows or saw a non-finite value
+struct LFwdArgs {
+  const float* qpos; const float* qvel; const float* ctrl; const float* qacc_warm;   // column pass: qacc_warm = the nominal qacc
+  float* qacc; uint64_t* contact_mask; int32_t* solver_iter; uint8_t* status; float* cwrench;
+  float* gscr; float* gfd; LMap map; int n;
+  float* dqacc; float* A; float* B; uint8_t* flags; long long s0; int ncol, centered; float eps[3];
+};
+
+#ifdef SMPLSIM_EMU
+static inline float l_div_rn(float a, float b) { return a / b; }
+#else
+__device__ __forceinline__ float l_div_rn(float a, float b) { return __fdiv_rn(a, b); }   // IEEE: a column the host can reproduce
+#endif
+
+// one forward pass of the state, ctrl (tau) and warm start (qacc) in the env's rows, from empty working-set memory: mj_checkPos / Vel,
+// S1 with collisions, the constraint solve, mj_checkAcc.  No auto-reset redo: a row with a non-finite value keeps its status bits and
+// unspecified values.
+template <class C>
+__device__ __noinline__ LFwd l_forward(const float* ms, float* sm, const LLane& w) {
+  const LHdr& H = l_hdr<C>(ms);
+  if (w.live) for (int i = w.li; i < (H.nslot + 3) / 4; i += LM_LPE) ((int*)sm)[C::pfl + i] = 0;
+  if (w.live && w.li == 0) { ((int*)sm)[C::misc + LMI_NSELF] = 0; ((int*)sm)[C::misc + LMI_NCON] = 0; ((int*)sm)[C::misc + LMI_NLIM] = 0; }
+  __syncwarp();
+  LSolveLane st; st.dirty_bits = 0u; st.rc_bits = 0u;
+  const int bad = l_check<C>(ms, sm, w, 0);
+  const LFkOut fk = l_sweep_out<C>(ms, sm, w, LF_FK | LF_VEL | LF_COLLIDE, bad != 0);
+  bool hit = false;
+  LFwd fo;
+  fo.mask = fk.mask;
+  fo.iters = l_solve<C>(ms, sm, w, fk.nrows > 0, st, &hit);
+  fo.status = bad | l_check<C>(ms, sm, w, 1) | (fk.dropped ? L_ST_ROWS_DROPPED : 0) | (hit ? L_ST_MAXITER : 0);
+  return fo;
+}
+
+__device__ __forceinline__ unsigned l_mix(unsigned x) {   // murmur3 finaliser
+  x ^= x >> 16; x *= 0x85ebca6bu; x ^= x >> 13; x *= 0xc2b2ae35u; x ^= x >> 16;
+  return x;
+}
+// active set the last solve ended on: the contact entries (slot, rows on the working set) and the joint-limit rows (dof, side, on the
+// set), summed over the env's lanes as mixed words; the same on every lane of the env
+template <class C>
+__device__ __noinline__ unsigned l_active_sig(float* sm, const LLane& w) {
+  unsigned s = 0u;
+  if (w.live) {
+    const int ncon = ((const int*)sm)[C::misc + LMI_NCON], nlim = ((const int*)sm)[C::misc + LMI_NLIM];
+    for (int c = w.li; c < ncon; c += LM_LPE) s += l_mix((unsigned)(((const int*)l_centry<C>(sm, w, c))[LCE_INFO] & 0x00ff001f));
+    for (int e = w.li; e < nlim; e += LM_LPE) {
+      const float* le = sm + C::lim + C::LIMW * e;
+      s += l_mix(0x80000000u | ((unsigned)((const int*)le)[LLE_DOF] << 2) | (le[LLE_SG] > 0.f ? 2u : 0u) | (unsigned)(((const int*)le)[LLE_FLAG] & 1));
+    }
+  }
+#pragma unroll
+  for (int o = LM_LPE / 2; o > 0; o >>= 1) s += __shfl_xor_sync(L_FULL, s, o);
+  return s;
+}
+
+// the perturbed input of column col at sign sg (0: the nominal): a qpos entry of the root translation or a hinge, a qvel or a ctrl
+// entry; for a root-rotation column the angle sg eps of q (x) exp(sg eps e_k)
+__device__ __forceinline__ float l_fd_value(const LFwdArgs& a, int nv, int nu, size_t row, int col, float sg) {
+  if (col < nv) return (col >= 3 && col < 6) ? sg * a.eps[0] : a.qpos[row * (nv + 1) + (col < 3 ? col : col + 1)] + sg * a.eps[0];
+  if (col < 2 * nv) return a.qvel[row * nv + col - nv] + sg * a.eps[1];
+  return a.ctrl[row * nu + col - 2 * nv] + sg * a.eps[2];
+}
+
+// the slot's row (qpos, qvel, ctrl -> tau, nominal qacc as the warm start) with column col's perturbation at sign sg
+template <class C>
+__device__ __noinline__ void l_fd_load(const float* ms, float* sm, const LLane& w, const LFwdArgs& a, size_t row, int col, float sg) {
+  const LHdr& H = l_hdr<C>(ms);
+  const int nv = H.nv, nu = H.nu;
+  l_copy_in<C>(sm + C::qpos, a.qpos + row * (nv + 1), nv + 1, w);
+  l_copy_in<C>(sm + C::qvel, a.qvel + row * nv, nv, w);
+  l_copy_in<C>(sm + C::tau, a.ctrl + row * nu, nu, w);
+  l_copy_in<C>(sm + C::qacc, a.qacc_warm + row * nv, nv, w);
+  __syncwarp();
+  if (w.live && w.li == 0) {
+    const float x = l_fd_value(a, nv, nu, row, col, sg);
+    if (col >= 3 && col < 6) {   // q (x) exp(x e_k), normalised
+      float* qp = sm + C::qpos + 3;
+      float sn, cs;
+      l_sincos(0.5f * x, &sn, &cs);
+      Q4 q; q.w = qp[0]; q.x = qp[1]; q.y = qp[2]; q.z = qp[3];
+      Q4 d; d.w = cs; d.x = col == 3 ? sn : 0.f; d.y = col == 4 ? sn : 0.f; d.z = col == 5 ? sn : 0.f;
+      q = qnormalize(qmul(q, d));
+      qp[0] = q.w; qp[1] = q.x; qp[2] = q.y; qp[3] = q.z;
+    } else if (col < nv) sm[C::qpos + (col < 3 ? col : col + 1)] = x;
+    else if (col < 2 * nv) sm[C::qvel + col - nv] = x;
+    else sm[C::tau + col - 2 * nv] = x;
+  }
+  __syncwarp();
+}
+
+// column col of dqacc (ap - am) / den, then of A or B by semi-implicit Euler (v' = v + h a, q' = q (+) h v'):  dv' = h dqacc + [qvel
+// column]; velocity rows dv'; translation and hinge rows [qpos column] + h dv'; root-rotation rows R(th)^T [rotation column] e +
+// J_r(th) h dv'[3:6] with th = h v'_nom[3:6], v'_nom = v + h qacc_nom
+template <class C>
+__device__ __noinline__ void l_fd_write(const float* ms, float* sm, const LLane& w, const LFwdArgs& a, size_t row, int col, float den, int flag) {
+  const LHdr& H = l_hdr<C>(ms);
+  const int nv = H.nv, nu = H.nu, ncol = a.ncol;
+  const float h = H.h;
+  const float* qnom = a.qacc_warm + row * nv;
+  if (w.live) {
+    const float* ap = a.centered ? a.gfd + (size_t)w.env * C::NV : sm + C::qacc;
+    const float* am = a.centered ? sm + C::qacc : qnom;
+    for (int i = w.li; i < nv; i += LM_LPE) {
+      const float d = l_div_rn(ap[i] - am[i], den);
+      sm[C::qacc + i] = d;
+      if (a.dqacc) a.dqacc[(row * nv + i) * ncol + col] = d;
+    }
+    if (a.flags && w.li == 0) a.flags[row * ncol + col] = (uint8_t)flag;
+  }
+  __syncwarp();
+  float* out = col < 2 * nv ? a.A : a.B;
+  if (!w.live || !out) return;
+  const int stride = col < 2 * nv ? 2 * nv : nu;
+  out += row * 2 * nv * stride + (col < 2 * nv ? col : col - 2 * nv);
+  const float* d = sm + C::qacc;
+  for (int i = w.li; i < 2 * nv; i += LM_LPE) {
+    if (i >= 3 && i < 6) continue;
+    const int j = i < nv ? i : i - nv;
+    const float dv = fmaf(h, d[j], col == nv + j ? 1.f : 0.f);
+    out[(size_t)i * stride] = i >= nv ? dv : fmaf(h, dv, col == i ? 1.f : 0.f);
+  }
+  if (w.li == 0) {
+    const float* v = a.qvel + row * nv;
+    const V3 th = h * v3(fmaf(h, qnom[3], v[3]), fmaf(h, qnom[4], v[4]), fmaf(h, qnom[5], v[5]));
+    const V3 dth = h * v3(fmaf(h, d[3], col == nv + 3 ? 1.f : 0.f), fmaf(h, d[4], col == nv + 4 ? 1.f : 0.f), fmaf(h, d[5], col == nv + 5 ? 1.f : 0.f));
+    const float t2 = dot(th, th);
+    float sinc, c1, c2;   // sin t / t, (1 - cos t) / t^2, (t - sin t) / t^3
+    if (t2 < 1e-2f) {
+      sinc = 1.f - t2 * (1.f / 6.f - t2 * (1.f / 120.f));
+      c1 = 0.5f - t2 * (1.f / 24.f - t2 * (1.f / 720.f));
+      c2 = 1.f / 6.f - t2 * (1.f / 120.f - t2 * (1.f / 5040.f));
+    } else {
+      const float t = sqrtf(t2);
+      float sn, cs;
+      l_sincos(t, &sn, &cs);
+      sinc = sn / t; c1 = (1.f - cs) / t2; c2 = (t - sn) / (t2 * t);
+    }
+    const V3 tx = cross(th, dth);
+    V3 r = dth - c1 * tx + c2 * cross(th, tx);   // J_r(th) dth
+    if (col >= 3 && col < 6) {                   // + R(th)^T e_k
+      const V3 e = v3(col == 3 ? 1.f : 0.f, col == 4 ? 1.f : 0.f, col == 5 ? 1.f : 0.f), te = cross(th, e);
+      r = r + e - sinc * te + c1 * cross(th, te);
+    }
+    out[3 * (size_t)stride] = r.x; out[4 * (size_t)stride] = r.y; out[5 * (size_t)stride] = r.z;
+  }
+}
+
+// k_fwd5<C> runs on a class of its own, LOwn<C> (C's layout and constants under another type), so that every noinline function it
+// calls is an instance of its own.  Sharing l_solve / l_check / l_contact_wrench with k_step5<C> and k_inverse5<C> changed their
+// register allocation, and with it the SASS of those kernels.
+template <class C> struct LOwn : C {};
+template <class C0>
+__global__ void __launch_bounds__(256, 1) k_fwd5(const float* __restrict__ gimg, int img_bytes, LFwdArgs a) {
+  typedef LOwn<C0> C;
+  const float* ms; LLane w;
+  float* sm = l_setup<C>(gimg, img_bytes, w, ms, a.n, a.map, a.gscr, nullptr, nullptr);
+  const LHdr& H = l_hdr<C>(ms);
+  const size_t eo = w.live ? (size_t)w.env : 0;
+  if constexpr (C::PRM) l_prm_stage<C>(ms, sm, w);
+  if (a.ncol == 0) {
+    l_copy_in<C>(sm + C::qpos, a.qpos + eo * (H.nv + 1), H.nv + 1, w);
+    l_copy_in<C>(sm + C::qvel, a.qvel + eo * H.nv, H.nv, w);
+    l_copy_in<C>(sm + C::tau, a.ctrl + eo * H.nu, H.nu, w);
+    if (a.qacc_warm) l_copy_in<C>(sm + C::qacc, a.qacc_warm + eo * H.nv, H.nv, w);
+    else if (w.live) for (int i = w.li; i < H.nv; i += LM_LPE) sm[C::qacc + i] = 0.f;
+    __syncwarp();
+    const LFwd fo = l_forward<C>(ms, sm, w);
+    if (a.cwrench) l_contact_wrench<C>(ms, sm, w, fo.iters, a.cwrench);
+    l_copy_out<C>(a.qacc + eo * H.nv, sm + C::qacc, H.nv, w);
+    if (w.live && w.li == 0) {
+      if (a.contact_mask) a.contact_mask[eo] = fo.mask;
+      if (a.solver_iter) a.solver_iter[eo] = fo.iters;
+      if (a.status) a.status[eo] = (uint8_t)fo.status;
+    }
+    return;
+  }
+  const long long s = a.s0 + (long long)eo;
+  const size_t row = (size_t)(s / a.ncol);
+  const int col = (int)(s % a.ncol);
+  unsigned sig0 = 0u;
+  int flag = 0;
+  float xp = 0.f;
+  for (int p = 0; p <= (a.centered ? 1 : 0); p++) {
+    l_fd_load<C>(ms, sm, w, a, row, col, p ? -1.f : 1.f);
+    const LFwd fo = l_forward<C>(ms, sm, w);
+    const unsigned sig = l_active_sig<C>(sm, w);
+    if (fo.status & (1 | 2 | 4 | L_ST_ROWS_DROPPED | L_ST_MAXITER)) flag |= L_FD_SOLVER;
+    if (p == 0 && a.centered) {
+      sig0 = sig;
+      l_copy_out<C>(a.gfd + eo * C::NV, sm + C::qacc, H.nv, w);
+      __syncwarp();
+    } else if (p == 1 && sig != sig0) flag |= L_FD_KINK;
+  }
+  if (w.live) xp = l_fd_value(a, H.nv, H.nu, row, col, 1.f) - l_fd_value(a, H.nv, H.nu, row, col, a.centered ? -1.f : 0.f);
+  l_fd_write<C>(ms, sm, w, a, row, col, xp, flag);
+}

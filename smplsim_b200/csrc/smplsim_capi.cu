@@ -35,6 +35,7 @@ struct SmplsimHandle {
   float* gsens = nullptr;  // body velocities of the last forward pass (obs v2 / aux)
   int* gpfl = nullptr;     // working set per contact slot, carried from call to call (solver warm start only)
   float* gbody = nullptr;  // body pose / velocity of the current forward pass (self-collision narrow phase)
+  float* gfd = nullptr;    // per-env qacc of a column's first solve (smplsim_transition_fd; handles without self-collision)
   int num_envs = 0, device = 0, nsm = 132, max_smem = 0;
   int cls = 0;             // 1 SMPL class, 2 SMPL-X class
   int selfcol = 0;         // cfg.env.self_collision: kernels with the geom-geom rows compiled in
@@ -91,6 +92,7 @@ struct LaneKernels {
   void (*kin)(const float*, int, LKinArgs);
   void (*inverse[2])(const float*, int, LInvArgs);                      // [parameter records]
   void (*dyn[2])(const float*, int, LDynArgs);                          // [parameter records]
+  void (*fwd[2])(const float*, int, LFwdArgs);                          // [parameter records]
 };
 template <class C>
 static LaneKernels lane_kernels() {
@@ -99,6 +101,7 @@ static LaneKernels lane_kernels() {
   // a self-collision class has no inverse instances (smplsim_inverse refuses such handles): NULL entries, so that none is compiled
   if constexpr (!C::SELFCOL) { k.inverse[0] = k_inverse5<C>; k.inverse[1] = k_inverse5<P>; }
   k.dyn[0] = k_dyn5<C>; k.dyn[1] = k_dyn5<P>;
+  if constexpr (!C::SELFCOL) { k.fwd[0] = k_fwd5<C>; k.fwd[1] = k_fwd5<P>; }   // as inverse: none for a self-collision class
   return k;
 }
 
@@ -127,7 +130,7 @@ static int pick_wpb(SmplsimHandle* h) {
     return ((!k || cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, cap) == cudaSuccess) && ...);
   };
   const LaneKernels K = lane_kernels<C>();
-  if (!raise(K.step[0], K.step[1], K.step[2], K.reset[0], K.reset[1], K.kin, K.inverse[0], K.inverse[1], K.dyn[0], K.dyn[1])) return -1;
+  if (!raise(K.step[0], K.step[1], K.step[2], K.reset[0], K.reset[1], K.kin, K.inverse[0], K.inverse[1], K.dyn[0], K.dyn[1], K.fwd[0], K.fwd[1])) return -1;
   return best;
 }
 
@@ -162,7 +165,7 @@ static void state_rows(const SmplsimHandle* h, void (*const kern[2])(const float
   } while (0)
 
 static void free_handle(SmplsimHandle* h) {
-  cudaFree(h->prm); cudaFree(h->dimg); cudaFree(h->gscr); cudaFree(h->gsens); cudaFree(h->gpfl); cudaFree(h->gbody); cudaFree(h->dslot_env); cudaFree(h->dblk_img); cudaFree(h->denv_model);
+  cudaFree(h->prm); cudaFree(h->dimg); cudaFree(h->gscr); cudaFree(h->gsens); cudaFree(h->gpfl); cudaFree(h->gbody); cudaFree(h->gfd); cudaFree(h->dslot_env); cudaFree(h->dblk_img); cudaFree(h->denv_model);
   delete h;
 }
 
@@ -257,6 +260,7 @@ static int create_impl(const SmplsimModelDesc* s, int nmodels, const int32_t* en
   if (e == cudaSuccess) e = cudaMalloc(&h->gpfl, pw * num_envs * 4);
   if (e == cudaSuccess) e = cudaMemset(h->gpfl, 0, pw * num_envs * 4);
   if (e == cudaSuccess && cfg->self_collision) e = cudaMalloc(&h->gbody, (size_t)10 * H.nb * num_envs * 4);
+  if (e == cudaSuccess && !cfg->self_collision) e = cudaMalloc(&h->gfd, (size_t)H.nv * num_envs * 4);
   if (e != cudaSuccess) { free_handle(h); return fail(SMPLSIM_ECUDA, std::string("smplsim_create: ") + cudaGetErrorString(e)); }
   if (std::getenv("SMPLSIM_DEBUG"))
     fprintf(stderr, "smplsim_create: class %d, %d bodies, schedule %d steps, mailboxes %d in / %d out, %d geom pairs, table %d B, %zu B per env, %d warps per CTA, %zu B shared memory per CTA, self-collision %d\n",
@@ -427,6 +431,71 @@ extern "C" int smplsim_dynamics(SmplsimHandle* h, const float* qpos_dev, const f
     if (c.jac) c.jac += r * c.njac * 6 * nv;
   };
   L_DISPATCH(h, state_rows<C_>(h, lane_kernels<C_>().dyn, a, advance, (cudaStream_t)stream));
+  CUDA_TRY(cudaGetLastError());
+  return SMPLSIM_OK;
+}
+
+// forward pass on n caller rows into qacc (and the other outputs each when non-NULL); the caller has checked the arguments
+static int forward_rows(SmplsimHandle* h, const float* qpos, const float* qvel, const float* ctrl, const float* qacc_warm, int n, float* qacc,
+                        uint64_t* contact_mask, int32_t* solver_iter, uint8_t* status, float* cwrench, cudaStream_t st) {
+  LFwdArgs a; std::memset(&a, 0, sizeof a);
+  a.qpos = qpos; a.qvel = qvel; a.ctrl = ctrl; a.qacc_warm = qacc_warm; a.qacc = qacc; a.contact_mask = contact_mask; a.solver_iter = solver_iter;
+  a.status = status; a.cwrench = cwrench; a.gscr = h->gscr; a.n = n; a.map = h->map();
+  const size_t nv = h->img.hdr()->nv, nu = h->img.hdr()->nu, nb = h->img.hdr()->nb;
+  auto advance = [nv, nu, nb](LFwdArgs& c, size_t r) {
+    c.qpos += r * (nv + 1); c.qvel += r * nv; c.ctrl += r * nu; c.qacc += r * nv;
+    if (c.qacc_warm) c.qacc_warm += r * nv;
+    if (c.contact_mask) c.contact_mask += r;
+    if (c.solver_iter) c.solver_iter += r;
+    if (c.status) c.status += r;
+    if (c.cwrench) c.cwrench += r * nb * 6;
+  };
+  L_DISPATCH(h, state_rows<C_>(h, lane_kernels<C_>().fwd, a, advance, st));
+  CUDA_TRY(cudaGetLastError());
+  return SMPLSIM_OK;
+}
+
+extern "C" int smplsim_forward(SmplsimHandle* h, const float* qpos_dev, const float* qvel_dev, const float* ctrl_dev, const float* qacc_warmstart_dev,
+                               int n, float* qacc_dev, uint64_t* contact_mask_dev, int32_t* solver_iter_dev, uint8_t* status_dev,
+                               float* contact_wrench_dev, void* stream) {
+  if (!h || n < 0) return fail(SMPLSIM_EINVAL, "smplsim_forward: null handle or n < 0");
+  if (h->selfcol)
+    return fail(SMPLSIM_EUNSUPPORTED, "smplsim_forward: the forward pass on caller rows does not build geom-geom contacts (handle created with self_collision = 1)");
+  if (n == 0) return SMPLSIM_OK;   // nothing is read: empty tensors may come as NULL
+  if (!qpos_dev || !qvel_dev || !ctrl_dev || !qacc_dev) return fail(SMPLSIM_EINVAL, "smplsim_forward: null argument");
+  if (int rc = env_rows(h, n, "smplsim_forward", true)) return rc;
+  DeviceGuard guard(h->device);
+  return forward_rows(h, qpos_dev, qvel_dev, ctrl_dev, qacc_warmstart_dev, n, qacc_dev, contact_mask_dev, solver_iter_dev, status_dev,
+                      contact_wrench_dev, (cudaStream_t)stream);
+}
+
+extern "C" int smplsim_transition_fd(SmplsimHandle* h, const SmplsimFdCfg* cfg, const float* qpos_dev, const float* qvel_dev, const float* ctrl_dev,
+                                     int n, float* qacc_dev, float* dqacc_dev, float* A_dev, float* B_dev, uint8_t* flags_dev, void* stream) {
+  if (!h || !cfg || n < 0) return fail(SMPLSIM_EINVAL, "smplsim_transition_fd: null handle / cfg or n < 0");
+  if (h->selfcol)
+    return fail(SMPLSIM_EUNSUPPORTED, "smplsim_transition_fd: the forward pass on caller rows does not build geom-geom contacts (handle created with self_collision = 1)");
+  if (h->nblocks)
+    return fail(SMPLSIM_EUNSUPPORTED, "smplsim_transition_fd: not available with per-env body shapes (the column slots of a row span CTAs of any shape)");
+  if (h->prm)
+    return fail(SMPLSIM_EUNSUPPORTED, "smplsim_transition_fd: not available while the handle has per-env parameter records (smplsim_clear_env_params)");
+  for (float e : {cfg->eps_qpos, cfg->eps_qvel, cfg->eps_ctrl})
+    if (!(std::isfinite(e) && e > 0.f)) return fail(SMPLSIM_EINVAL, "smplsim_transition_fd: eps_qpos, eps_qvel and eps_ctrl must be finite and > 0");
+  if (n == 0) return SMPLSIM_OK;   // nothing is read: empty tensors may come as NULL
+  if (!qpos_dev || !qvel_dev || !ctrl_dev || !qacc_dev) return fail(SMPLSIM_EINVAL, "smplsim_transition_fd: null argument (qpos, qvel, ctrl and qacc are required)");
+  if (!dqacc_dev && !A_dev && !B_dev && !flags_dev) return fail(SMPLSIM_EINVAL, "smplsim_transition_fd: no derivative output requested (dqacc, A, B and flags all NULL)");
+  DeviceGuard guard(h->device);
+  const cudaStream_t st = (cudaStream_t)stream;
+  if (int rc = forward_rows(h, qpos_dev, qvel_dev, ctrl_dev, nullptr, n, qacc_dev, nullptr, nullptr, nullptr, nullptr, st)) return rc;
+  const LHdr& H = *h->img.hdr();
+  LFwdArgs a; std::memset(&a, 0, sizeof a);
+  a.qpos = qpos_dev; a.qvel = qvel_dev; a.ctrl = ctrl_dev; a.qacc_warm = qacc_dev; a.gscr = h->gscr; a.gfd = h->gfd; a.map = h->map();
+  a.dqacc = dqacc_dev; a.A = A_dev; a.B = B_dev; a.flags = flags_dev; a.ncol = 2 * H.nv + H.nu; a.centered = cfg->centered ? 1 : 0;
+  a.eps[0] = cfg->eps_qpos; a.eps[1] = cfg->eps_qvel; a.eps[2] = cfg->eps_ctrl;
+  const long long slots = (long long)n * a.ncol;
+  for (long long s0 = 0; s0 < slots; s0 += h->num_envs) {   // launches of at most num_envs slots (the handle's scratch rows), in order
+    a.s0 = s0; a.n = (int)std::min<long long>(h->num_envs, slots - s0);
+    L_DISPATCH(h, lane_launch<C_>(h, lane_kernels<C_>().fwd[0], a.n, st, a));
+  }
   CUDA_TRY(cudaGetLastError());
   return SMPLSIM_OK;
 }

@@ -85,6 +85,22 @@ def mj_fullM(model, dst, qM):
         d[i * nv + j] = d[j * nv + i] = qM[k]
 
 
+def mjd_transitionFD(model, data, eps, flg_centered, A, B, C, D):
+    """``mujoco.mjd_transitionFD`` for an env's ``mj_data``: finite-difference ``A = dx'/dx`` [2nv, 2nv] and ``B = dx'/du`` [2nv, nu]
+    of one simulation substep at the data's ``qpos`` / ``qvel`` / ``ctrl``, written into ``A`` / ``B`` in place (either may be None).
+    ``eps`` is the perturbation of every qpos, qvel and ctrl entry, as in MuJoCo; ``flg_centered`` selects centered differences.  The
+    computation is fp32 on the GPU: MuJoCo's usual ``eps = 1e-6`` is rounding noise there, and ``eps = None`` takes the measured
+    defaults of ``HumanoidBatchB200.transition_fd`` (1e-2 on qpos, 1e-1 on qvel, 1 N m on ctrl).  Sensor derivatives ``C`` / ``D`` are
+    not computed: pass None for both.  ``model`` is accepted for the signature and not read."""
+    if C is not None or D is not None:
+        raise NotImplementedError("mjd_transitionFD: sensor derivatives (C, D) are not computed; pass None")
+    a, b = data._fd_fn(data.qpos, data.qvel, data.ctrl, eps, bool(flg_centered))
+    if A is not None:
+        A[...] = a.reshape(np.shape(A))
+    if B is not None:
+        B[...] = b.reshape(np.shape(B))
+
+
 class _MjData(SimpleNamespace):
     """``mj_data`` view.  ``qM`` / ``qfrc_bias`` cost a kernel call, so they are evaluated on first read."""
 
@@ -227,7 +243,7 @@ class HumanoidEnvB200(_EnvBase):
         b = self._b
         sens = np.concatenate([b.body_linvel[0].cpu().numpy().ravel(), b.body_angvel[0].cpu().numpy().ravel()])
         z3, z4 = np.zeros((1, 3)), np.array([[1.0, 0, 0, 0]])
-        return _MjData(_dyn_fn=self._fwd_dynamics, qpos=b.qpos[0].cpu().numpy().astype(np.float64), qvel=b.qvel[0].cpu().numpy().astype(np.float64),
+        return _MjData(_dyn_fn=self._fwd_dynamics, _fd_fn=self._transition_fd, qpos=b.qpos[0].cpu().numpy().astype(np.float64), qvel=b.qvel[0].cpu().numpy().astype(np.float64),
                                ctrl=b.ctrl[0].cpu().numpy().astype(np.float64), qacc=b.qacc[0].cpu().numpy().astype(np.float64),
                                xpos=np.concatenate([z3, b.xpos[0].cpu().numpy()]), xquat=np.concatenate([z4, b.xquat[0].cpu().numpy()]),
                                sensordata=sens, contact=_Contacts(int(b.contact_mask[0].item())),
@@ -255,6 +271,14 @@ class HumanoidEnvB200(_EnvBase):
         M = out["qM"][0].cpu().numpy().astype(np.float64)
         qM = np.array([M[i, j] for i, j in _pairs(self._dof_parentid)])
         return qM, out["qfrc_bias"][0].cpu().numpy().astype(np.float64)
+
+    def _transition_fd(self, qpos, qvel, ctrl, eps, centered):
+        """(A, B) of ``mjd_transitionFD`` at one state (fp32 rows of the given arrays; fp64 copies of the result)."""
+        b = self._b
+        e = b.FD_EPS if eps is None else (eps, eps, eps)
+        row = lambda x: torch.as_tensor(np.asarray(x, dtype=np.float32)[None], device=b.device)  # noqa: E731
+        out = b.transition_fd(row(qpos), row(qvel), row(ctrl), *e, centered=centered)
+        return out["A"][0].cpu().numpy().astype(np.float64), out["B"][0].cpu().numpy().astype(np.float64)
 
     def get_body_jac_by_id(self, id, jacp=None, jacr=None):
         """``mujoco.mj_jacBody`` at the current qpos for MuJoCo body id ``id`` (0 = world: zeros): the [3, nv] translational and
