@@ -189,7 +189,9 @@ typedef struct SmplsimHandle SmplsimHandle;
 
 const char* smplsim_last_error(void);
 int smplsim_version(void);   /* 300 = this header (290: before smplsim_track_eval; 280: before smplsim_motion_blend and the interpolation / future-target fields; 270: before smplsim_amp_obs / smplsim_amp_demo; 260: before smplsim_imitation; 250: before smplsim_set_env_params; 240: before smplsim_ray / smplsim_render; 230: before smplsim_dynamics; 220: before smplsim_inverse;
-                              * 210: before SmplsimAux.contact_wrench; 200: before SmplsimState.xfrc_applied; 100: before pid_* state and aux.status) */
+                              * 210: before SmplsimAux.contact_wrench; 200: before SmplsimState.xfrc_applied; 100: before pid_* state and aux.status).
+                              * smplsim_forward, smplsim_transition_fd and smplsim_rollout came later without a new number, because callers
+                              * compare it to 300 for equality: look them up by symbol (dlsym) rather than by version. */
 
 /* MjModel.from_xml_string + MjData + setup_humanoid_properties/setup_controller
  * (base_env.py:139-142, humanoid_env.py:262-323). */
@@ -284,6 +286,34 @@ typedef struct SmplsimFdCfg {
  * SMPLSIM_EUNSUPPORTED.  SMPLSIM_EINVAL: a null required argument, n < 0, an eps that is not finite and > 0, or no derivative output. */
 int smplsim_transition_fd(SmplsimHandle* h, const SmplsimFdCfg* cfg, const float* qpos_dev, const float* qvel_dev, const float* ctrl_dev,
                           int n, float* qacc_dev, float* dqacc_dev, float* A_dev, float* B_dev, uint8_t* flags_dev, void* cuda_stream);
+
+/* Rollouts from caller states, mujoco.rollout.rollout: n rows, each a start state and nstep control rows, stepped in one launch.
+ * Row i's step t is what the env path does on a freshly created handle (empty working-set memory): set_state(qpos0[i], qvel0[i])
+ * with qacc_warm = qacc_warmstart[i], then per step
+ *   SMPLSIM_ROLLOUT_ACTION: smplsim_step(control[i,t]) -- a policy action through the configured controller (uhc_pd stable PD
+ *                           including quirk Q1, pd, torque) for cfg.env.nsubsteps substeps; pass nsub = 0.  Not clamped here:
+ *                           clamp it as the caller of smplsim_step does (cfg.env.clip_actions).  simple_pid: SMPLSIM_EUNSUPPORTED
+ *                           (its integral / last error are env state);
+ *   SMPLSIM_ROLLOUT_CTRL:   smplsim_mj_step(control[i,t], nsub) -- raw joint torques (not clamped) held for nsub >= 1 substeps;
+ *                           nsub = 1 is MuJoCo's rollout, one mj_step per control row;
+ * keeping only the physics of those calls (no task target, observation, reward or termination).  The warm start and the working set
+ * carry from step to step as from call to call; a row whose state turns non-finite auto-resets to the model's qpos0 and carries on,
+ * as mj_step does.  Inputs qpos0[n,nq], qvel0[n,nv] and control[n,nstep,nu] required; qacc_warmstart[n,nv] NULL: zeros;
+ * qpos_fwd0[n,nq] / qvel_fwd0[n,nv], the state of the last forward pass that stable PD with stale inertia reads, NULL: the start state
+ * (what set_state marks).  An env's own qpos, qvel, qacc_warm, qpos_fwd and qvel_fwd continue its physics up to the solver's
+ * tolerance (its working-set memory is not taken).  Outputs row-major: qpos[n,nstep,nq], qvel[n,nstep,nv] (the state after each
+ * step) required; status[n,nstep] (the SmplsimAux.status bits of the step: 1 / 2 / 4 auto-reset, 8 rows dropped, 16 iteration cap;
+ * SMPLSIM_STATUS_SELF_CONTACT is not evaluated) NULL: not written; xpos[n,nstep,nbody,3] and xquat[n,nstep,nbody,4], the post-step
+ * poses of SmplsimAux.xpos / xquat, both or neither (asking for them changes no bit of qpos / qvel).  Takes no xfrc_applied and
+ * reads or writes no per-env state (a later smplsim_step is unaffected).  Row rules of smplsim_forward: single shape, any n >= 0
+ * (launched in pieces of at most num_envs rows on the stream); per-env shapes or parameter records: n == num_envs, row i uses env i;
+ * self_collision = 1: SMPLSIM_EUNSUPPORTED.  SMPLSIM_EINVAL: a null required argument, n < 0, nstep < 1, an unknown mode, nsub < 1 in
+ * ctrl mode or != 0 in action mode, xpos without xquat or the reverse.  n == 0 reads nothing. */
+#define SMPLSIM_ROLLOUT_ACTION 0
+#define SMPLSIM_ROLLOUT_CTRL 1
+int smplsim_rollout(SmplsimHandle* h, int mode, int nsub, const float* qpos0_dev, const float* qvel0_dev, const float* qacc_warmstart_dev,
+                    const float* qpos_fwd0_dev, const float* qvel_fwd0_dev, const float* control_dev, int n, int nstep, float* qpos_dev,
+                    float* qvel_dev, uint8_t* status_dev, float* xpos_dev, float* xquat_dev, void* cuda_stream);
 
 /* Mass matrix, bias forces and body Jacobians on n caller rows qpos[n,nq], qvel[n,nv] (each output NULL: skipped):
  *   qM[n,nv,nv]          mujoco.mj_fullM(qM): the dense joint-space inertia, armature on the diagonal; exactly symmetric, exact zeros

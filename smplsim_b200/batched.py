@@ -430,6 +430,69 @@ class HumanoidBatchB200:
         self.gpu_launches += 1
         return out
 
+    ROLLOUT_MODES = {"action": 0, "ctrl": 1}   # SMPLSIM_ROLLOUT_ACTION / SMPLSIM_ROLLOUT_CTRL
+
+    def rollout(self, qpos: torch.Tensor, qvel: torch.Tensor, control: torch.Tensor, *, mode: str = "action", nsub: Optional[int] = None,
+                qacc_warmstart: Optional[torch.Tensor] = None, qpos_fwd: Optional[torch.Tensor] = None, qvel_fwd: Optional[torch.Tensor] = None,
+                body_poses: bool = False, status: bool = True):
+        """Roll ``n`` control sequences forward from caller start states in one kernel launch, as ``mujoco.rollout.rollout``.  Row ``i``
+        starts at ``(qpos[i], qvel[i])`` and takes one step per control row ``control[i, t]`` (``control`` is ``[n, T, nu]``):
+
+        - ``mode="action"``: ``step`` -- a policy action (clamped to [-1, 1] with ``cfg.env.clip_actions``, as ``step`` does) through the
+          configured controller for ``cfg.env.nsubsteps`` substeps; ``nsub`` must be None; ``simple_pid`` is refused (its integral /
+          last error are env state);
+        - ``mode="ctrl"``: ``mj_step(control[i, t], nsub)`` -- raw joint torques, not clamped, held for ``nsub`` substeps (None: 1,
+          MuJoCo's rollout).
+
+        Each step is bit for bit what that call does on a fresh batch after ``set_state(qpos[i], qvel[i])`` with ``qacc_warm =
+        qacc_warmstart[i]``, keeping only the physics: no task target, observation, reward or termination.  ``qacc_warmstart`` (None:
+        zeros) seeds the constraint solve; ``qpos_fwd`` / ``qvel_fwd`` (None: the start state, as ``set_state`` marks) are the state of
+        the last forward pass that stable PD with stale inertia reads.  Passing an env's own ``qpos, qvel, qacc_warm, qpos_fwd,
+        qvel_fwd`` continues its physics up to the solver's tolerance (the rollout starts from empty working-set memory).
+
+        Returns a dict of ``qpos [n, T, nq]`` and ``qvel [n, T, nv]`` (the state after each step), ``status [n, T]`` uint8 (with
+        ``status``: the bits of ``self.status`` the step raises -- a row whose state turns non-finite auto-resets and carries on; the
+        self-contact bit is not evaluated) and, with ``body_poses``, ``xpos [n, T, nbody, 3]`` / ``xquat [n, T, nbody, 4]`` (the post-step
+        poses of ``self.xpos`` / ``self.xquat``; asking for them changes no bit of the trajectory).  Float32 tensors on this batch's
+        device; any n on a one-shape batch without per-env parameters, n == num_envs otherwise (row i uses env i's shape and
+        parameters).  Reads no env state and changes none; ``xfrc_applied`` is not taken.  Not available with
+        ``cfg.env.self_collision``."""
+        m = self.model
+        if mode not in self.ROLLOUT_MODES:
+            raise ValueError(f"mode must be 'action' or 'ctrl', got {mode!r}")
+        if mode == "action":
+            if nsub is not None:
+                raise ValueError("nsub is for mode='ctrl'; an action step runs cfg.env.nsubsteps substeps")
+            ns = 0
+        else:
+            ns = 1 if nsub is None else nsub
+            if isinstance(ns, bool) or not isinstance(ns, (int, np.integer)) or ns < 1:
+                raise ValueError(f"nsub must be an int >= 1, got {nsub!r}")
+        args = (("qpos", qpos, m.nq), ("qvel", qvel, m.nv))
+        opt = [(k, t, w) for k, t, w in (("qacc_warmstart", qacc_warmstart, m.nv), ("qpos_fwd", qpos_fwd, m.nq), ("qvel_fwd", qvel_fwd, m.nv))
+               if t is not None]
+        rows = dict(zip([a[0] for a in args + tuple(opt)], self._rows(args + tuple(opt))))
+        n = rows["qpos"].shape[0]
+        u = self._checked("control", control.contiguous() if isinstance(control, torch.Tensor) else control, (n, None, m.nu))
+        T = u.shape[1]
+        if T < 1:
+            raise ValueError("control must hold at least one step ([n, T, nu] with T >= 1)")
+        if mode == "action" and bool(self.cfg.env.clip_actions):
+            u = torch.clamp(u, -1.0, 1.0)
+        dv, f32 = self.device, dict(dtype=torch.float32, device=self.device)
+        out = {"qpos": torch.empty(n, T, m.nq, **f32), "qvel": torch.empty(n, T, m.nv, **f32)}
+        if status:
+            out["status"] = torch.empty(n, T, dtype=torch.uint8, device=dv)
+        if body_poses:
+            out["xpos"] = torch.empty(n, T, m.nbody, 3, **f32)
+            out["xquat"] = torch.empty(n, T, m.nbody, 4, **f32)
+        self._check(self._L().smplsim_rollout(self._h, self.ROLLOUT_MODES[mode], int(ns), _ptr(rows["qpos"]), _ptr(rows["qvel"]),
+                                              _ptr(rows.get("qacc_warmstart")), _ptr(rows.get("qpos_fwd")), _ptr(rows.get("qvel_fwd")), _ptr(u),
+                                              n, T, _ptr(out["qpos"]), _ptr(out["qvel"]), _ptr(out.get("status")), _ptr(out.get("xpos")),
+                                              _ptr(out.get("xquat")), self._stream()))
+        self.gpu_launches += 1
+        return out
+
     def dynamics(self, qpos: torch.Tensor, qvel: Optional[torch.Tensor] = None, mass_matrix: bool = True, bias: bool = True,
                  jac_bodies: Optional[Sequence] = None):
         """Joint-space mass matrix, bias forces and body Jacobians at caller rows ``(qpos, qvel)``, as MuJoCo's ``mj_fullM(qM)``,

@@ -70,6 +70,10 @@ struct LCfg {
   static constexpr int obs = mbi, xq = OBS_STAGED ? mbi + OBSW : mbi;
   static_assert(xq + 4 * NB <= lim, "xquat staging does not fit the aliased region");
 };
+// model classes the kernels are instantiated for: <bodies, dofs, geoms, contact slots, in-mailboxes, out-mailboxes, contact
+// entries in shared memory, limit rows, geom-geom rows compiled in> (smplsim_capi.cu, rollout_kernels.cu)
+#define L_SMPL(SC) LCfg<24, 75, 24, 64, 5, 2, 15, 16, SC>
+#define L_SMPLX(SC) LCfg<52, 159, 52, 128, 13, 4, 14, 16, SC>
 // misc words
 #define LMI_NCON 0
 #define LMI_NLIM 1
@@ -2957,3 +2961,26 @@ __global__ void __launch_bounds__(256, 1) k_fwd5(const float* __restrict__ gimg,
   if (w.live) xp = l_fd_value(a, H.nv, H.nu, row, col, 1.f) - l_fd_value(a, H.nv, H.nu, row, col, a.centered ? -1.f : 0.f);
   l_fd_write<C>(ms, sm, w, a, row, col, xp, flag);
 }
+
+// ------------------------------------------------------------------ rollouts from caller states (mujoco.rollout.rollout)
+// Per caller row: the start state (qpos0, qvel0, warm start), then nstep steps, each k_step5's physics on that step's control row
+// (mode 0: a policy action through the configured controller, nsub = cfg.env.nsubsteps; mode 1: raw ctrl held for nsub substeps),
+// with no task, observation or reward.  The row's state, warm start and working-set memory stay in shared memory from step to step,
+// as they pass from call to call through an env's rows; the working set starts empty.  Stable PD with stale inertia crosses a step
+// boundary as a call boundary does: the last substep integrates with l_integrate, its forward-pass state goes to the per-env scratch
+// rows scr.qpos_fwd / qvel_fwd, and the next step's l_spd_prologue rebuilds the factors from them (scr.qpos / qvel hold the state
+// at the boundary, which the prologue reloads).  Uses the handle's per-env scratch of the slots it runs (lane records, overflow
+// contact entries, scr); writes neither the working-set memory nor the sensor rows of the envs.
+struct LRollArgs {
+  const float* qpos0; const float* qvel0; const float* qacc_warm0; const float* qpos_fwd0; const float* qvel_fwd0; const float* control;
+  float* qpos; float* qvel; uint8_t* status; float* xpos; float* xquat;   // [n, nstep, ...]; status, xpos / xquat: NULL = not written
+  LState scr;   // per-env rows [num_envs, nq | nv]: qpos, qvel, qpos_fwd, qvel_fwd (stable PD, stale inertia); the other fields NULL
+  float* gscr; LMap map; int n, nstep, nsub, mode;
+};
+
+
+// k_roll5<C> is defined and instantiated in rollout_kernels.cu, a translation unit of its own, so that it is a device module of its own:
+// its callers of the noinline functions and of the sinf slow path, added to this module, changed the SASS of the existing kernels.
+// lane_roll_kernels (also there) hands the host code its instances: [0] plain, [1] with parameter records, of class 1 (SMPL) or 2
+// (SMPL-X), without self-collision.
+void lane_roll_kernels(int cls, void (*k[2])(const float*, int, LRollArgs));

@@ -23,10 +23,6 @@
 #define L_LAUNCH(kern, grid, block, smem, stream, ...) kern<<<grid, block, smem, stream>>>(__VA_ARGS__)
 #endif
 
-// model classes the kernels are instantiated for: <bodies, dofs, geoms, contact slots, in-mailboxes, out-mailboxes, contact
-// entries in shared memory, limit rows, geom-geom rows compiled in>
-#define L_SMPL(SC) LCfg<24, 75, 24, 64, 5, 2, 15, 16, SC>
-#define L_SMPLX(SC) LCfg<52, 159, 52, 128, 13, 4, 14, 16, SC>
 
 struct SmplsimHandle {
   LaneImage img;
@@ -36,6 +32,7 @@ struct SmplsimHandle {
   int* gpfl = nullptr;     // working set per contact slot, carried from call to call (solver warm start only)
   float* gbody = nullptr;  // body pose / velocity of the current forward pass (self-collision narrow phase)
   float* gfd = nullptr;    // per-env qacc of a column's first solve (smplsim_transition_fd; handles without self-collision)
+  float* groll = nullptr;  // per-env qpos, qvel, qpos_fwd, qvel_fwd at a rollout's step boundary (smplsim_rollout; as gfd)
   int num_envs = 0, device = 0, nsm = 132, max_smem = 0;
   int cls = 0;             // 1 SMPL class, 2 SMPL-X class
   int selfcol = 0;         // cfg.env.self_collision: kernels with the geom-geom rows compiled in
@@ -93,6 +90,7 @@ struct LaneKernels {
   void (*inverse[2])(const float*, int, LInvArgs);                      // [parameter records]
   void (*dyn[2])(const float*, int, LDynArgs);                          // [parameter records]
   void (*fwd[2])(const float*, int, LFwdArgs);                          // [parameter records]
+  void (*roll[2])(const float*, int, LRollArgs);                        // [parameter records]
 };
 template <class C>
 static LaneKernels lane_kernels() {
@@ -102,6 +100,7 @@ static LaneKernels lane_kernels() {
   if constexpr (!C::SELFCOL) { k.inverse[0] = k_inverse5<C>; k.inverse[1] = k_inverse5<P>; }
   k.dyn[0] = k_dyn5<C>; k.dyn[1] = k_dyn5<P>;
   if constexpr (!C::SELFCOL) { k.fwd[0] = k_fwd5<C>; k.fwd[1] = k_fwd5<P>; }   // as inverse: none for a self-collision class
+  if constexpr (!C::SELFCOL) lane_roll_kernels(C::NB == L_SMPL(0)::NB ? 1 : 2, k.roll);   // a module of its own (rollout_kernels.cu)
   return k;
 }
 
@@ -130,7 +129,8 @@ static int pick_wpb(SmplsimHandle* h) {
     return ((!k || cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, cap) == cudaSuccess) && ...);
   };
   const LaneKernels K = lane_kernels<C>();
-  if (!raise(K.step[0], K.step[1], K.step[2], K.reset[0], K.reset[1], K.kin, K.inverse[0], K.inverse[1], K.dyn[0], K.dyn[1], K.fwd[0], K.fwd[1])) return -1;
+  if (!raise(K.step[0], K.step[1], K.step[2], K.reset[0], K.reset[1], K.kin, K.inverse[0], K.inverse[1], K.dyn[0], K.dyn[1], K.fwd[0], K.fwd[1],
+             K.roll[0], K.roll[1])) return -1;
   return best;
 }
 
@@ -165,7 +165,7 @@ static void state_rows(const SmplsimHandle* h, void (*const kern[2])(const float
   } while (0)
 
 static void free_handle(SmplsimHandle* h) {
-  cudaFree(h->prm); cudaFree(h->dimg); cudaFree(h->gscr); cudaFree(h->gsens); cudaFree(h->gpfl); cudaFree(h->gbody); cudaFree(h->gfd); cudaFree(h->dslot_env); cudaFree(h->dblk_img); cudaFree(h->denv_model);
+  cudaFree(h->prm); cudaFree(h->dimg); cudaFree(h->gscr); cudaFree(h->gsens); cudaFree(h->gpfl); cudaFree(h->gbody); cudaFree(h->gfd); cudaFree(h->groll); cudaFree(h->dslot_env); cudaFree(h->dblk_img); cudaFree(h->denv_model);
   delete h;
 }
 
@@ -261,6 +261,7 @@ static int create_impl(const SmplsimModelDesc* s, int nmodels, const int32_t* en
   if (e == cudaSuccess) e = cudaMemset(h->gpfl, 0, pw * num_envs * 4);
   if (e == cudaSuccess && cfg->self_collision) e = cudaMalloc(&h->gbody, (size_t)10 * H.nb * num_envs * 4);
   if (e == cudaSuccess && !cfg->self_collision) e = cudaMalloc(&h->gfd, (size_t)H.nv * num_envs * 4);
+  if (e == cudaSuccess && !cfg->self_collision) e = cudaMalloc(&h->groll, (size_t)2 * (2 * H.nv + 1) * num_envs * 4);
   if (e != cudaSuccess) { free_handle(h); return fail(SMPLSIM_ECUDA, std::string("smplsim_create: ") + cudaGetErrorString(e)); }
   if (std::getenv("SMPLSIM_DEBUG"))
     fprintf(stderr, "smplsim_create: class %d, %d bodies, schedule %d steps, mailboxes %d in / %d out, %d geom pairs, table %d B, %zu B per env, %d warps per CTA, %zu B shared memory per CTA, self-collision %d\n",
@@ -496,6 +497,45 @@ extern "C" int smplsim_transition_fd(SmplsimHandle* h, const SmplsimFdCfg* cfg, 
     a.s0 = s0; a.n = (int)std::min<long long>(h->num_envs, slots - s0);
     L_DISPATCH(h, lane_launch<C_>(h, lane_kernels<C_>().fwd[0], a.n, st, a));
   }
+  CUDA_TRY(cudaGetLastError());
+  return SMPLSIM_OK;
+}
+
+extern "C" int smplsim_rollout(SmplsimHandle* h, int mode, int nsub, const float* qpos0_dev, const float* qvel0_dev, const float* qacc_warmstart_dev,
+                               const float* qpos_fwd0_dev, const float* qvel_fwd0_dev, const float* control_dev, int n, int nstep,
+                               float* qpos_dev, float* qvel_dev, uint8_t* status_dev, float* xpos_dev, float* xquat_dev, void* stream) {
+  if (!h || n < 0 || nstep < 1) return fail(SMPLSIM_EINVAL, "smplsim_rollout: null handle, n < 0 or nstep < 1");
+  if (mode != SMPLSIM_ROLLOUT_ACTION && mode != SMPLSIM_ROLLOUT_CTRL) return fail(SMPLSIM_EINVAL, "smplsim_rollout: unknown mode");
+  if (mode == SMPLSIM_ROLLOUT_CTRL && nsub < 1) return fail(SMPLSIM_EINVAL, "smplsim_rollout: SMPLSIM_ROLLOUT_CTRL needs nsub >= 1");
+  if (mode == SMPLSIM_ROLLOUT_ACTION && nsub != 0)
+    return fail(SMPLSIM_EINVAL, "smplsim_rollout: SMPLSIM_ROLLOUT_ACTION takes nsub = 0 (an action step runs cfg.env.nsubsteps substeps)");
+  if (!xpos_dev != !xquat_dev) return fail(SMPLSIM_EINVAL, "smplsim_rollout: give both xpos and xquat, or neither");
+  if (h->selfcol)
+    return fail(SMPLSIM_EUNSUPPORTED, "smplsim_rollout: the rollout on caller rows does not build geom-geom contacts (handle created with self_collision = 1)");
+  const LHdr& H = *h->img.hdr();
+  if (mode == SMPLSIM_ROLLOUT_ACTION && H.cfg.control_mode == SMPLSIM_CTRL_SIMPLE_PID)
+    return fail(SMPLSIM_EUNSUPPORTED, "smplsim_rollout: control_mode simple_pid keeps its integral / last error in env state, which rollout rows do not have");
+  if (n == 0) return SMPLSIM_OK;   // nothing is read: empty tensors may come as NULL
+  if (!qpos0_dev || !qvel0_dev || !control_dev || !qpos_dev || !qvel_dev)
+    return fail(SMPLSIM_EINVAL, "smplsim_rollout: null argument (qpos0, qvel0, control, qpos and qvel are required)");
+  if (int rc = env_rows(h, n, "smplsim_rollout", true)) return rc;
+  DeviceGuard guard(h->device);
+  const size_t nq = H.nv + 1, nv = H.nv, nu = H.nu, nb = H.nb, T = (size_t)nstep, N = (size_t)h->num_envs;
+  LRollArgs a; std::memset(&a, 0, sizeof a);
+  a.qpos0 = qpos0_dev; a.qvel0 = qvel0_dev; a.qacc_warm0 = qacc_warmstart_dev; a.control = control_dev;
+  a.qpos_fwd0 = qpos_fwd0_dev ? qpos_fwd0_dev : qpos0_dev; a.qvel_fwd0 = qvel_fwd0_dev ? qvel_fwd0_dev : qvel0_dev;   // as set_state marks
+  a.qpos = qpos_dev; a.qvel = qvel_dev; a.status = status_dev; a.xpos = xpos_dev; a.xquat = xquat_dev;
+  a.scr.qpos = h->groll; a.scr.qvel = a.scr.qpos + N * nq; a.scr.qpos_fwd = a.scr.qvel + N * nv; a.scr.qvel_fwd = a.scr.qpos_fwd + N * nq;
+  a.gscr = h->gscr; a.map = h->map(); a.n = n; a.nstep = nstep; a.mode = mode;
+  a.nsub = mode == SMPLSIM_ROLLOUT_ACTION ? H.cfg.nsubsteps : nsub;
+  auto advance = [nq, nv, nu, nb, T](LRollArgs& c, size_t r) {
+    c.qpos0 += r * nq; c.qvel0 += r * nv; c.qpos_fwd0 += r * nq; c.qvel_fwd0 += r * nv; c.control += r * T * nu;
+    if (c.qacc_warm0) c.qacc_warm0 += r * nv;
+    c.qpos += r * T * nq; c.qvel += r * T * nv;
+    if (c.status) c.status += r * T;
+    if (c.xpos) { c.xpos += r * T * nb * 3; c.xquat += r * T * nb * 4; }
+  };
+  L_DISPATCH(h, state_rows<C_>(h, lane_kernels<C_>().roll, a, advance, (cudaStream_t)stream));
   CUDA_TRY(cudaGetLastError());
   return SMPLSIM_OK;
 }
@@ -953,4 +993,8 @@ extern "C" int smplsim_debug_stats(int* out, int reset) {   // out: L_NSTATS cou
 #endif
   return 0;
 }
+#endif
+
+#ifdef SMPLSIM_EMU
+#include "rollout_kernels.cu"   // the device build compiles it as a translation unit of its own (_lib.build)
 #endif

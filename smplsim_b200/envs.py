@@ -101,6 +101,18 @@ def mjd_transitionFD(model, data, eps, flg_centered, A, B, C, D):
         B[...] = b.reshape(np.shape(B))
 
 
+def rollout(model, data, initial_state, control, nstep=None):
+    """``mujoco.rollout.rollout`` for an env's ``mj_data`` [MJ-upstream signature, not checked against a wheel]: ``nroll`` rollouts
+    of ``nstep`` ``mj_step`` calls each, one per control row, from caller states, in one kernel launch per row (the env's handle holds
+    one env).  ``initial_state`` is ``[nroll, 1 + nq + nv]`` (or one ``[1 + nq + nv]`` state for every row): ``[time, qpos, qvel]``,
+    MuJoCo's ``mjSTATE_FULLPHYSICS`` layout for this model, which has no activations or plugins.  ``control`` is ``[nroll, nstep,
+    nu]`` (or ``[nstep, nu]`` for every row): raw joint torques as ``data.ctrl`` holds them, not clamped.  Returns ``(state,
+    sensordata)`` as MuJoCo does: ``state [nroll, nstep, 1 + nq + nv]`` after each step (time advanced by ``model.opt.timestep``
+    per step), and ``sensordata [nroll, nstep, 0]``: sensors are not evaluated.  Each row starts from empty warm start and working-set
+    memory; fp32 on the GPU.  ``model`` is accepted for the signature; ``data``'s own state is neither read nor changed."""
+    return data._rollout_fn(initial_state, control, nstep)
+
+
 class _MjData(SimpleNamespace):
     """``mj_data`` view.  ``qM`` / ``qfrc_bias`` cost a kernel call, so they are evaluated on first read."""
 
@@ -243,7 +255,7 @@ class HumanoidEnvB200(_EnvBase):
         b = self._b
         sens = np.concatenate([b.body_linvel[0].cpu().numpy().ravel(), b.body_angvel[0].cpu().numpy().ravel()])
         z3, z4 = np.zeros((1, 3)), np.array([[1.0, 0, 0, 0]])
-        return _MjData(_dyn_fn=self._fwd_dynamics, _fd_fn=self._transition_fd, qpos=b.qpos[0].cpu().numpy().astype(np.float64), qvel=b.qvel[0].cpu().numpy().astype(np.float64),
+        return _MjData(_dyn_fn=self._fwd_dynamics, _fd_fn=self._transition_fd, _rollout_fn=self._rollout, qpos=b.qpos[0].cpu().numpy().astype(np.float64), qvel=b.qvel[0].cpu().numpy().astype(np.float64),
                                ctrl=b.ctrl[0].cpu().numpy().astype(np.float64), qacc=b.qacc[0].cpu().numpy().astype(np.float64),
                                xpos=np.concatenate([z3, b.xpos[0].cpu().numpy()]), xquat=np.concatenate([z4, b.xquat[0].cpu().numpy()]),
                                sensordata=sens, contact=_Contacts(int(b.contact_mask[0].item())),
@@ -279,6 +291,26 @@ class HumanoidEnvB200(_EnvBase):
         row = lambda x: torch.as_tensor(np.asarray(x, dtype=np.float32)[None], device=b.device)  # noqa: E731
         out = b.transition_fd(row(qpos), row(qvel), row(ctrl), *e, centered=centered)
         return out["A"][0].cpu().numpy().astype(np.float64), out["B"][0].cpu().numpy().astype(np.float64)
+
+    def _rollout(self, initial_state, control, nstep):
+        """(state, sensordata) of ``rollout``: ctrl-mode rollouts of the given rows (fp32 on the device; fp64 copies of the result)."""
+        b, m = self._b, self._b.model
+        x0 = np.asarray(initial_state, dtype=np.float64)
+        u = np.asarray(control, dtype=np.float64)
+        x0 = x0[None] if x0.ndim == 1 else x0
+        if x0.ndim != 2 or x0.shape[1] != 1 + m.nq + m.nv:
+            raise ValueError(f"initial_state must have shape [nroll, {1 + m.nq + m.nv}] ([time, qpos, qvel]), got {np.shape(initial_state)}")
+        u = np.broadcast_to(u[None], (x0.shape[0],) + u.shape) if u.ndim == 2 else u
+        if u.ndim != 3 or u.shape[0] != x0.shape[0] or u.shape[2] != m.nu:
+            raise ValueError(f"control must have shape [nroll, nstep, {m.nu}] or [nstep, {m.nu}], got {np.shape(control)}")
+        if nstep is not None and nstep != u.shape[1]:
+            raise ValueError(f"nstep = {nstep} does not match the {u.shape[1]} control rows")
+        dev = lambda x: torch.as_tensor(np.ascontiguousarray(x, dtype=np.float32), device=b.device)  # noqa: E731
+        out = b.rollout(dev(x0[:, 1:1 + m.nq]), dev(x0[:, 1 + m.nq:]), dev(u), mode="ctrl", status=False)
+        T = u.shape[1]
+        time = x0[:, :1] + self.sim_timestep * np.arange(1, T + 1)[None]
+        state = np.concatenate([time[..., None], out["qpos"].cpu().numpy().astype(np.float64), out["qvel"].cpu().numpy().astype(np.float64)], axis=2)
+        return state, np.zeros((x0.shape[0], T, 0))
 
     def get_body_jac_by_id(self, id, jacp=None, jacr=None):
         """``mujoco.mj_jacBody`` at the current qpos for MuJoCo body id ``id`` (0 = world: zeros): the [3, nv] translational and
