@@ -190,7 +190,7 @@ typedef struct SmplsimHandle SmplsimHandle;
 const char* smplsim_last_error(void);
 int smplsim_version(void);   /* 300 = this header (290: before smplsim_track_eval; 280: before smplsim_motion_blend and the interpolation / future-target fields; 270: before smplsim_amp_obs / smplsim_amp_demo; 260: before smplsim_imitation; 250: before smplsim_set_env_params; 240: before smplsim_ray / smplsim_render; 230: before smplsim_dynamics; 220: before smplsim_inverse;
                               * 210: before SmplsimAux.contact_wrench; 200: before SmplsimState.xfrc_applied; 100: before pid_* state and aux.status).
-                              * smplsim_forward, smplsim_transition_fd and smplsim_rollout came later without a new number, because callers
+                              * smplsim_forward, smplsim_transition_fd, smplsim_rollout and smplsim_inverse_fd came later without a new number, because callers
                               * compare it to 300 for equality: look them up by symbol (dlsym) rather than by version. */
 
 /* MjModel.from_xml_string + MjData + setup_humanoid_properties/setup_controller
@@ -286,6 +286,33 @@ typedef struct SmplsimFdCfg {
  * SMPLSIM_EUNSUPPORTED.  SMPLSIM_EINVAL: a null required argument, n < 0, an eps that is not finite and > 0, or no derivative output. */
 int smplsim_transition_fd(SmplsimHandle* h, const SmplsimFdCfg* cfg, const float* qpos_dev, const float* qvel_dev, const float* ctrl_dev,
                           int n, float* qacc_dev, float* dqacc_dev, float* A_dev, float* B_dev, uint8_t* flags_dev, void* cuda_stream);
+
+/* Finite-difference inverse-dynamics derivatives, mujoco.mjd_inverseFD without sensors or DmDq.  Input tangent x = [dq (nv) ; qvel (nv)
+ * ; qacc (nv)] with the root rotation tangent in the body frame (q (x) exp(d), as smplsim_transition_fd); the function differenced is
+ * smplsim_inverse's qfrc_inverse = M qacc + qfrc_bias - J^T f, f = -D min(0, J qacc - aref).  eps_qpos (rad / m), eps_qvel and eps_qacc
+ * are the perturbations; centered != 0 differences x + eps against x - eps, else x + eps against the nominal.  SMPLSIM_INVFD_DEFAULTS
+ * (1e-3, 1e-2, 1.0, centered) are the measured choice (DESIGN.md 2): ten times smaller steps on qpos and qvel than
+ * SMPLSIM_FD_DEFAULTS, because larger ones move contacts and limit rows across their switches in more columns; for a fixed row set
+ * qfrc_inverse is affine in qacc, so eps_qacc costs no accuracy. */
+typedef struct SmplsimInverseFdCfg {
+  float eps_qpos, eps_qvel, eps_qacc;
+  int32_t centered, pad_;
+} SmplsimInverseFdCfg;
+#define SMPLSIM_INVFD_DEFAULTS {1e-3f, 1e-2f, 1.0f, 1, 0}
+/* Outputs per row, row-major; qfrc_inverse required, dfrc and flags each NULL: not written, not both NULL:
+ *   qfrc_inverse[n,nv]      the nominal pass: smplsim_inverse's row path, bit for bit what smplsim_inverse gives;
+ *   dfrc[n,nv,3nv]          d qfrc_inverse / d [dq, qvel, qacc], dfrc[i,k,j] = d f_k / d x_j (smplsim_transition_fd's dqacc layout;
+ *                           mjd_inverseFD's DfDq / DfDv / DfDa are its three nv x nv blocks transposed);
+ *   flags[n,3nv]            per column SMPLSIM_FD_KINK (the two passes ended on different row sets: a contact appeared or went, or a
+ *                           row's r < 0 status flipped; never set with centered = 0) and SMPLSIM_FD_SOLVER (a pass dropped joint-limit
+ *                           rows past the kernels' cap or saw a non-finite value; the inverse has no iteration cap).
+ * Column j's difference is divided by the fp32 difference of the inputs actually perturbed (2 eps for a root-rotation column).  Costs
+ * the nominal pass plus (1 + centered) 3nv inverse passes per row, launched in pieces of num_envs on the stream without a host sync;
+ * writes no per-env state.  Row rules and errors of smplsim_transition_fd: single-shape handles without parameter records only (per-env
+ * shapes, parameter records and self_collision = 1 give SMPLSIM_EUNSUPPORTED); SMPLSIM_EINVAL: a null required argument, n < 0, an eps
+ * that is not finite and > 0, or no derivative output; n == 0 reads nothing. */
+int smplsim_inverse_fd(SmplsimHandle* h, const SmplsimInverseFdCfg* cfg, const float* qpos_dev, const float* qvel_dev, const float* qacc_dev,
+                       int n, float* qfrc_inverse_dev, float* dfrc_dev, uint8_t* flags_dev, void* cuda_stream);
 
 /* Rollouts from caller states, mujoco.rollout.rollout: n rows, each a start state and nstep control rows, stepped in one launch.
  * Row i's step t is what the env path does on a freshly created handle (empty working-set memory): set_state(qpos0[i], qvel0[i])

@@ -30,7 +30,8 @@ def build(force: bool = False, verbose: bool = False) -> str:
     if force or not os.path.exists(SO_PATH) or os.path.getmtime(SO_PATH) < newest:
         nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
         cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", SO_PATH, os.path.join(_CSRC, "smplsim_capi.cu"),
-                                                                               os.path.join(_CSRC, "rollout_kernels.cu")]
+                                                                               os.path.join(_CSRC, "rollout_kernels.cu"),
+                                                                               os.path.join(_CSRC, "inverse_fd_kernels.cu")]
         subprocess.check_call(cmd, cwd=_CSRC)
     return SO_PATH
 
@@ -54,6 +55,8 @@ _SYMBOLS = {
                                  C.c_void_p, C.c_void_p]),
     "smplsim_transition_fd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.c_void_p, C.c_void_p]),
+    "smplsim_inverse_fd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                    C.c_void_p]),
     "smplsim_rollout": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                  C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "smplsim_ray": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p,

@@ -57,6 +57,10 @@ class SmplsimFdCfgC(C.Structure):
     _fields_ = [("eps_qpos", C.c_float), ("eps_qvel", C.c_float), ("eps_ctrl", C.c_float), ("centered", C.c_int32), ("pad_", C.c_int32)]
 
 
+class SmplsimInverseFdCfgC(C.Structure):
+    _fields_ = [("eps_qpos", C.c_float), ("eps_qvel", C.c_float), ("eps_qacc", C.c_float), ("centered", C.c_int32), ("pad_", C.c_int32)]
+
+
 class SmplsimImitationCfgC(C.Structure):
     _fields_ = [("k_pos", C.c_float), ("k_rot", C.c_float), ("k_vel", C.c_float), ("k_angvel", C.c_float),
                 ("w_pos", C.c_float), ("w_rot", C.c_float), ("w_vel", C.c_float), ("w_angvel", C.c_float),

@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .abi import SmplsimAuxC, SmplsimEnvParamsC, SmplsimFdCfgC, SmplsimStateC, env_cfg_from, model_from_cfg
+from .abi import SmplsimAuxC, SmplsimEnvParamsC, SmplsimFdCfgC, SmplsimInverseFdCfgC, SmplsimStateC, env_cfg_from, model_from_cfg
 from .model import ModelDesc
 
 
@@ -427,6 +427,37 @@ class HumanoidBatchB200:
         cfg = SmplsimFdCfgC(float(eps_qpos), float(eps_qvel), float(eps_ctrl), 1 if centered else 0, 0)
         self._check(self._L().smplsim_transition_fd(self._h, C.byref(cfg), _ptr(q), _ptr(v), _ptr(u), n, _ptr(out["qacc"]), _ptr(out.get("dqacc")),
                                                     _ptr(out["A"]), _ptr(out["B"]), _ptr(out["flags"]), self._stream()))
+        self.gpu_launches += 1
+        return out
+
+    INVFD_EPS = (1e-3, 1e-2, 1.0)   # eps_qpos (rad / m), eps_qvel, eps_qacc: the fp32 steps DESIGN.md 2 measured
+
+    def inverse_fd(self, qpos: torch.Tensor, qvel: torch.Tensor, qacc: torch.Tensor, eps_qpos: float = INVFD_EPS[0],
+                   eps_qvel: float = INVFD_EPS[1], eps_qacc: float = INVFD_EPS[2], centered: bool = True):
+        """Finite-difference derivatives of ``inverse`` at caller rows, as ``mujoco.mjd_inverseFD`` without sensors or ``DmDq``.  Input
+        tangent ``x = [dq (nv) ; qvel (nv) ; qacc (nv)]`` (root rotation tangent in the body frame, ``q * exp(d)``).  Returns a dict of
+
+        - ``qfrc_inverse [n, nv]``: the nominal pass, bit for bit what ``inverse`` gives;
+        - ``dfrc [n, nv, 3nv]``: ``d qfrc_inverse / d [dq, qvel, qacc]``, ``dfrc[i, k, j] = d f_k / d x_j`` (the layout of
+          ``transition_fd``'s ``dqacc``; ``mjd_inverseFD``'s ``DfDq``, ``DfDv``, ``DfDa`` are its three blocks transposed);
+        - ``flags [n, 3nv]`` uint8 per column: 1 the two passes ended on different row sets (a contact appeared or went, or a row's
+          ``r < 0`` status flipped; never set with ``centered=False``), 2 a pass dropped joint-limit rows or saw a non-finite value.
+
+        ``eps_*`` are the perturbations; the defaults are the measured choice (fp32: MuJoCo's 1e-6 is rounding noise).  ``qfrc_inverse``
+        is affine in ``qacc`` for a fixed row set, so ``eps_qacc`` costs no accuracy.  ``centered=False`` differences against the nominal
+        (half the passes).  Float32 tensors on this batch's device, any n; single-shape batches without per-env parameters (raises
+        otherwise), not with ``cfg.env.self_collision``.  Reads no env state and changes none."""
+        m = self.model
+        for name, e in (("eps_qpos", eps_qpos), ("eps_qvel", eps_qvel), ("eps_qacc", eps_qacc)):
+            if not (np.isfinite(e) and e > 0):
+                raise ValueError(f"{name} must be finite and > 0, got {e!r}")
+        q, v, a = self._rows((("qpos", qpos, m.nq), ("qvel", qvel, m.nv), ("qacc", qacc, m.nv)))
+        n, ncol, f32 = q.shape[0], 3 * m.nv, dict(dtype=torch.float32, device=self.device)
+        out = {"qfrc_inverse": torch.empty(n, m.nv, **f32), "dfrc": torch.empty(n, m.nv, ncol, **f32),
+               "flags": torch.empty(n, ncol, dtype=torch.uint8, device=self.device)}
+        cfg = SmplsimInverseFdCfgC(float(eps_qpos), float(eps_qvel), float(eps_qacc), 1 if centered else 0, 0)
+        self._check(self._L().smplsim_inverse_fd(self._h, C.byref(cfg), _ptr(q), _ptr(v), _ptr(a), n, _ptr(out["qfrc_inverse"]),
+                                                 _ptr(out["dfrc"]), _ptr(out["flags"]), self._stream()))
         self.gpu_launches += 1
         return out
 

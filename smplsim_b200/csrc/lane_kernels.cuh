@@ -2984,3 +2984,22 @@ struct LRollArgs {
 // lane_roll_kernels (also there) hands the host code its instances: [0] plain, [1] with parameter records, of class 1 (SMPL) or 2
 // (SMPL-X), without self-collision.
 void lane_roll_kernels(int cls, void (*k[2])(const float*, int, LRollArgs));
+
+// ------------------------------------------------------------------ finite-difference inverse-dynamics derivatives (mjd_inverseFD)
+// Slot s of a launch works on row s / 3nv and column s % 3nv of x = [dq (nv) ; qvel (nv) ; qacc (nv)] (the root rotation as q (x)
+// exp(d)): k_inverse5's pass at x + eps and (centered) x - eps, column col of dfrc = d qfrc_inverse / dx divided by the fp32 difference
+// of the inputs loaded, and the column's flags (L_FD_KINK: the two passes ended on different row sets; L_FD_SOLVER: a pass dropped
+// joint-limit rows or saw a non-finite value).  Not centered, the one pass is differenced against the nominal qfrc (the row pass of
+// smplsim_inverse).  Uses the handle's per-env scratch of the slots it runs (lane records, overflow contact entries, gfd); writes
+// neither the working-set memory nor the sensor rows, so the stepper cannot tell that it ran.
+struct LInvFdArgs {
+  const float* qpos; const float* qvel; const float* qacc; const float* qfrc;   // [n, nq | nv]; qfrc: the nominal qfrc_inverse
+  float* dfrc; uint8_t* flags;   // [n, nv, 3nv], [n, 3nv]; each NULL: not written
+  float* gscr; float* gfd; LMap map; int n;
+  long long s0; int centered; float eps[3];   // eps_qpos, eps_qvel, eps_qacc
+};
+
+// k_invfd5<C> is defined and instantiated in inverse_fd_kernels.cu, a translation unit of its own as k_roll5 is, so that its callers of
+// the noinline functions leave the SASS of the existing kernels alone.  lane_invfd_kernels (also there) hands the host code its instance
+// of class 1 (SMPL) or 2 (SMPL-X), without self-collision or parameter records.
+void lane_invfd_kernels(int cls, void (**k)(const float*, int, LInvFdArgs));

@@ -31,7 +31,7 @@ struct SmplsimHandle {
   float* gsens = nullptr;  // body velocities of the last forward pass (obs v2 / aux)
   int* gpfl = nullptr;     // working set per contact slot, carried from call to call (solver warm start only)
   float* gbody = nullptr;  // body pose / velocity of the current forward pass (self-collision narrow phase)
-  float* gfd = nullptr;    // per-env qacc of a column's first solve (smplsim_transition_fd; handles without self-collision)
+  float* gfd = nullptr;    // per-env qacc / qfrc of a column's first pass (smplsim_transition_fd, smplsim_inverse_fd; handles without self-collision)
   float* groll = nullptr;  // per-env qpos, qvel, qpos_fwd, qvel_fwd at a rollout's step boundary (smplsim_rollout; as gfd)
   int num_envs = 0, device = 0, nsm = 132, max_smem = 0;
   int cls = 0;             // 1 SMPL class, 2 SMPL-X class
@@ -91,6 +91,7 @@ struct LaneKernels {
   void (*dyn[2])(const float*, int, LDynArgs);                          // [parameter records]
   void (*fwd[2])(const float*, int, LFwdArgs);                          // [parameter records]
   void (*roll[2])(const float*, int, LRollArgs);                        // [parameter records]
+  void (*invfd)(const float*, int, LInvFdArgs);                         // single shape, no parameter records
 };
 template <class C>
 static LaneKernels lane_kernels() {
@@ -101,6 +102,7 @@ static LaneKernels lane_kernels() {
   k.dyn[0] = k_dyn5<C>; k.dyn[1] = k_dyn5<P>;
   if constexpr (!C::SELFCOL) { k.fwd[0] = k_fwd5<C>; k.fwd[1] = k_fwd5<P>; }   // as inverse: none for a self-collision class
   if constexpr (!C::SELFCOL) lane_roll_kernels(C::NB == L_SMPL(0)::NB ? 1 : 2, k.roll);   // a module of its own (rollout_kernels.cu)
+  if constexpr (!C::SELFCOL) lane_invfd_kernels(C::NB == L_SMPL(0)::NB ? 1 : 2, &k.invfd);   // as roll (inverse_fd_kernels.cu)
   return k;
 }
 
@@ -130,7 +132,7 @@ static int pick_wpb(SmplsimHandle* h) {
   };
   const LaneKernels K = lane_kernels<C>();
   if (!raise(K.step[0], K.step[1], K.step[2], K.reset[0], K.reset[1], K.kin, K.inverse[0], K.inverse[1], K.dyn[0], K.dyn[1], K.fwd[0], K.fwd[1],
-             K.roll[0], K.roll[1])) return -1;
+             K.roll[0], K.roll[1], K.invfd)) return -1;
   return best;
 }
 
@@ -496,6 +498,39 @@ extern "C" int smplsim_transition_fd(SmplsimHandle* h, const SmplsimFdCfg* cfg, 
   for (long long s0 = 0; s0 < slots; s0 += h->num_envs) {   // launches of at most num_envs slots (the handle's scratch rows), in order
     a.s0 = s0; a.n = (int)std::min<long long>(h->num_envs, slots - s0);
     L_DISPATCH(h, lane_launch<C_>(h, lane_kernels<C_>().fwd[0], a.n, st, a));
+  }
+  CUDA_TRY(cudaGetLastError());
+  return SMPLSIM_OK;
+}
+
+extern "C" int smplsim_inverse_fd(SmplsimHandle* h, const SmplsimInverseFdCfg* cfg, const float* qpos_dev, const float* qvel_dev,
+                                  const float* qacc_dev, int n, float* qfrc_inverse_dev, float* dfrc_dev, uint8_t* flags_dev, void* stream) {
+  if (!h || !cfg || n < 0) return fail(SMPLSIM_EINVAL, "smplsim_inverse_fd: null handle / cfg or n < 0");
+  if (h->selfcol)
+    return fail(SMPLSIM_EUNSUPPORTED, "smplsim_inverse_fd: the inverse does not build geom-geom contacts (handle created with self_collision = 1)");
+  if (h->nblocks)
+    return fail(SMPLSIM_EUNSUPPORTED, "smplsim_inverse_fd: not available with per-env body shapes (the column slots of a row span CTAs of any shape)");
+  if (h->prm)
+    return fail(SMPLSIM_EUNSUPPORTED, "smplsim_inverse_fd: not available while the handle has per-env parameter records (smplsim_clear_env_params)");
+  for (float e : {cfg->eps_qpos, cfg->eps_qvel, cfg->eps_qacc})
+    if (!(std::isfinite(e) && e > 0.f)) return fail(SMPLSIM_EINVAL, "smplsim_inverse_fd: eps_qpos, eps_qvel and eps_qacc must be finite and > 0");
+  if (n == 0) return SMPLSIM_OK;   // nothing is read: empty tensors may come as NULL
+  if (!qpos_dev || !qvel_dev || !qacc_dev || !qfrc_inverse_dev)
+    return fail(SMPLSIM_EINVAL, "smplsim_inverse_fd: null argument (qpos, qvel, qacc and qfrc_inverse are required)");
+  if (!dfrc_dev && !flags_dev) return fail(SMPLSIM_EINVAL, "smplsim_inverse_fd: no derivative output requested (dfrc and flags both NULL)");
+  // the nominal pass is smplsim_inverse's row path, so qfrc_inverse is bit for bit what smplsim_inverse gives
+  if (int rc = smplsim_inverse(h, qpos_dev, qvel_dev, qacc_dev, qfrc_inverse_dev, nullptr, n, stream)) return rc;
+  DeviceGuard guard(h->device);
+  const cudaStream_t st = (cudaStream_t)stream;
+  const LHdr& H = *h->img.hdr();
+  LInvFdArgs a; std::memset(&a, 0, sizeof a);
+  a.qpos = qpos_dev; a.qvel = qvel_dev; a.qacc = qacc_dev; a.qfrc = qfrc_inverse_dev; a.dfrc = dfrc_dev; a.flags = flags_dev;
+  a.gscr = h->gscr; a.gfd = h->gfd; a.map = h->map(); a.centered = cfg->centered ? 1 : 0;
+  a.eps[0] = cfg->eps_qpos; a.eps[1] = cfg->eps_qvel; a.eps[2] = cfg->eps_qacc;
+  const long long slots = (long long)n * 3 * H.nv;
+  for (long long s0 = 0; s0 < slots; s0 += h->num_envs) {   // launches of at most num_envs slots (the handle's scratch rows), in order
+    a.s0 = s0; a.n = (int)std::min<long long>(h->num_envs, slots - s0);
+    L_DISPATCH(h, lane_launch<C_>(h, lane_kernels<C_>().invfd, a.n, st, a));
   }
   CUDA_TRY(cudaGetLastError());
   return SMPLSIM_OK;
@@ -997,4 +1032,5 @@ extern "C" int smplsim_debug_stats(int* out, int reset) {   // out: L_NSTATS cou
 
 #ifdef SMPLSIM_EMU
 #include "rollout_kernels.cu"   // the device build compiles it as a translation unit of its own (_lib.build)
+#include "inverse_fd_kernels.cu"   // as rollout_kernels.cu
 #endif

@@ -101,6 +101,25 @@ def mjd_transitionFD(model, data, eps, flg_centered, A, B, C, D):
         B[...] = b.reshape(np.shape(B))
 
 
+def mjd_inverseFD(model, data, eps, flg_actuation, DfDq, DfDv, DfDa, DsDq, DsDv, DsDa, DmDq):
+    """``mujoco.mjd_inverseFD`` for an env's ``mj_data``: finite-difference derivatives of the inverse dynamics ``qfrc_inverse`` at the
+    data's ``qpos`` / ``qvel`` / ``qacc``, written into ``DfDq`` / ``DfDv`` / ``DfDa`` [nv, nv] in place (each may be None) in MuJoCo's
+    transposed layout: ``DfDq[j, i] = d qfrc_inverse_i / d q_j`` (root rotation tangent in the body frame).  ``eps`` is the
+    perturbation of every qpos, qvel and qacc entry, as in MuJoCo; the differences are centered.  The computation is fp32 on the GPU:
+    MuJoCo's usual ``eps = 1e-6`` is rounding noise there, and ``eps = None`` takes the measured defaults of
+    ``HumanoidBatchB200.inverse_fd`` (1e-3 on qpos, 1e-2 on qvel, 1 on qacc).  ``flg_actuation`` (subtract ``qfrc_actuator``) is
+    accepted and changes nothing: this model's motor forces depend on ``ctrl`` only, so their derivatives by qpos, qvel and qacc are
+    zero.  Sensor derivatives ``DsDq`` / ``DsDv`` / ``DsDa`` and ``DmDq`` are not computed: pass None.  ``model`` is accepted for the
+    signature and not read."""
+    if DsDq is not None or DsDv is not None or DsDa is not None or DmDq is not None:
+        raise NotImplementedError("mjd_inverseFD: sensor derivatives (DsDq, DsDv, DsDa) and DmDq are not computed; pass None")
+    dfrc = data._invfd_fn(data.qpos, data.qvel, data.qacc, eps)
+    nv = dfrc.shape[0]
+    for k, out in enumerate((DfDq, DfDv, DfDa)):
+        if out is not None:
+            out[...] = dfrc[:, k * nv:(k + 1) * nv].T.reshape(np.shape(out))
+
+
 def rollout(model, data, initial_state, control, nstep=None):
     """``mujoco.rollout.rollout`` for an env's ``mj_data`` [MJ-upstream signature, not checked against a wheel]: ``nroll`` rollouts
     of ``nstep`` ``mj_step`` calls each, one per control row, from caller states, in one kernel launch per row (the env's handle holds
@@ -255,7 +274,7 @@ class HumanoidEnvB200(_EnvBase):
         b = self._b
         sens = np.concatenate([b.body_linvel[0].cpu().numpy().ravel(), b.body_angvel[0].cpu().numpy().ravel()])
         z3, z4 = np.zeros((1, 3)), np.array([[1.0, 0, 0, 0]])
-        return _MjData(_dyn_fn=self._fwd_dynamics, _fd_fn=self._transition_fd, _rollout_fn=self._rollout, qpos=b.qpos[0].cpu().numpy().astype(np.float64), qvel=b.qvel[0].cpu().numpy().astype(np.float64),
+        return _MjData(_dyn_fn=self._fwd_dynamics, _fd_fn=self._transition_fd, _rollout_fn=self._rollout, _invfd_fn=self._inverse_fd, qpos=b.qpos[0].cpu().numpy().astype(np.float64), qvel=b.qvel[0].cpu().numpy().astype(np.float64),
                                ctrl=b.ctrl[0].cpu().numpy().astype(np.float64), qacc=b.qacc[0].cpu().numpy().astype(np.float64),
                                xpos=np.concatenate([z3, b.xpos[0].cpu().numpy()]), xquat=np.concatenate([z4, b.xquat[0].cpu().numpy()]),
                                sensordata=sens, contact=_Contacts(int(b.contact_mask[0].item())),
@@ -291,6 +310,13 @@ class HumanoidEnvB200(_EnvBase):
         row = lambda x: torch.as_tensor(np.asarray(x, dtype=np.float32)[None], device=b.device)  # noqa: E731
         out = b.transition_fd(row(qpos), row(qvel), row(ctrl), *e, centered=centered)
         return out["A"][0].cpu().numpy().astype(np.float64), out["B"][0].cpu().numpy().astype(np.float64)
+
+    def _inverse_fd(self, qpos, qvel, qacc, eps):
+        """dfrc [nv, 3nv] of ``mjd_inverseFD`` at one state (fp32 rows of the given arrays; an fp64 copy of the result)."""
+        b = self._b
+        e = b.INVFD_EPS if eps is None else (eps, eps, eps)
+        row = lambda x: torch.as_tensor(np.asarray(x, dtype=np.float32)[None], device=b.device)  # noqa: E731
+        return b.inverse_fd(row(qpos), row(qvel), row(qacc), *e)["dfrc"][0].cpu().numpy().astype(np.float64)
 
     def _rollout(self, initial_state, control, nstep):
         """(state, sensordata) of ``rollout``: ctrl-mode rollouts of the given rows (fp32 on the device; fp64 copies of the result)."""
