@@ -21,6 +21,14 @@ def _ptr(t: Optional[torch.Tensor]):
     return None if t is None else C.c_void_p(t.data_ptr())
 
 
+def _fd_eps(**eps: float):
+    """The finite-difference steps of ``transition_fd`` / ``inverse_fd`` as floats, in the order given; raises unless each is finite and > 0."""
+    for name, e in eps.items():
+        if not (np.isfinite(e) and e > 0):
+            raise ValueError(f"{name} must be finite and > 0, got {e!r}")
+    return [float(e) for e in eps.values()]
+
+
 class HumanoidBatchB200:
     """N independent SMPL humanoid envs stepped in lockstep on one GPU.
 
@@ -414,9 +422,7 @@ class HumanoidBatchB200:
         single-shape batches without per-env parameters (raises otherwise), not with ``cfg.env.self_collision``.  Reads no env state and
         changes none."""
         m = self.model
-        for name, e in (("eps_qpos", eps_qpos), ("eps_qvel", eps_qvel), ("eps_ctrl", eps_ctrl)):
-            if not (np.isfinite(e) and e > 0):
-                raise ValueError(f"{name} must be finite and > 0, got {e!r}")
+        eps = _fd_eps(eps_qpos=eps_qpos, eps_qvel=eps_qvel, eps_ctrl=eps_ctrl)
         q, v, u = self._rows((("qpos", qpos, m.nq), ("qvel", qvel, m.nv), ("ctrl", ctrl, m.nu)))
         n, nx, f32 = q.shape[0], 2 * m.nv, dict(dtype=torch.float32, device=self.device)
         ncol = nx + m.nu
@@ -424,7 +430,7 @@ class HumanoidBatchB200:
                "flags": torch.empty(n, ncol, dtype=torch.uint8, device=self.device)}
         if dqacc:
             out["dqacc"] = torch.empty(n, m.nv, ncol, **f32)
-        cfg = SmplsimFdCfgC(float(eps_qpos), float(eps_qvel), float(eps_ctrl), 1 if centered else 0, 0)
+        cfg = SmplsimFdCfgC(*eps, 1 if centered else 0, 0)
         self._check(self._L().smplsim_transition_fd(self._h, C.byref(cfg), _ptr(q), _ptr(v), _ptr(u), n, _ptr(out["qacc"]), _ptr(out.get("dqacc")),
                                                     _ptr(out["A"]), _ptr(out["B"]), _ptr(out["flags"]), self._stream()))
         self.gpu_launches += 1
@@ -448,14 +454,12 @@ class HumanoidBatchB200:
         (half the passes).  Float32 tensors on this batch's device, any n; single-shape batches without per-env parameters (raises
         otherwise), not with ``cfg.env.self_collision``.  Reads no env state and changes none."""
         m = self.model
-        for name, e in (("eps_qpos", eps_qpos), ("eps_qvel", eps_qvel), ("eps_qacc", eps_qacc)):
-            if not (np.isfinite(e) and e > 0):
-                raise ValueError(f"{name} must be finite and > 0, got {e!r}")
+        eps = _fd_eps(eps_qpos=eps_qpos, eps_qvel=eps_qvel, eps_qacc=eps_qacc)
         q, v, a = self._rows((("qpos", qpos, m.nq), ("qvel", qvel, m.nv), ("qacc", qacc, m.nv)))
         n, ncol, f32 = q.shape[0], 3 * m.nv, dict(dtype=torch.float32, device=self.device)
         out = {"qfrc_inverse": torch.empty(n, m.nv, **f32), "dfrc": torch.empty(n, m.nv, ncol, **f32),
                "flags": torch.empty(n, ncol, dtype=torch.uint8, device=self.device)}
-        cfg = SmplsimInverseFdCfgC(float(eps_qpos), float(eps_qvel), float(eps_qacc), 1 if centered else 0, 0)
+        cfg = SmplsimInverseFdCfgC(*eps, 1 if centered else 0, 0)
         self._check(self._L().smplsim_inverse_fd(self._h, C.byref(cfg), _ptr(q), _ptr(v), _ptr(a), n, _ptr(out["qfrc_inverse"]),
                                                  _ptr(out["dfrc"]), _ptr(out["flags"]), self._stream()))
         self.gpu_launches += 1

@@ -16,14 +16,6 @@
 #undef l_impedance
 #undef k_zero_wrench
 
-// the perturbed input of column col at sign sg (0: the nominal): a qpos entry of the root translation or a hinge, a qvel or a qacc
-// entry; for a root-rotation column the angle sg eps of q (x) exp(sg eps e_k)
-__device__ __forceinline__ float l_ifd_value(const LInvFdArgs& a, int nv, size_t row, int col, float sg) {
-  if (col < nv) return (col >= 3 && col < 6) ? sg * a.eps[0] : a.qpos[row * (nv + 1) + (col < 3 ? col : col + 1)] + sg * a.eps[0];
-  if (col < 2 * nv) return a.qvel[row * nv + col - nv] + sg * a.eps[1];
-  return a.qacc[row * nv + col - 2 * nv] + sg * a.eps[2];
-}
-
 // any entry of the env's n words at p non-finite or beyond mjMAXVAL (mj_checkPos / Vel / Acc's test), on every lane of the env
 template <class C>
 __device__ __forceinline__ bool l_ifd_bad(const float* p, int n, const LLane& w) {
@@ -32,42 +24,21 @@ __device__ __forceinline__ bool l_ifd_bad(const float* p, int n, const LLane& w)
   return l_gany(b, w);
 }
 
-// one inverse pass of the slot's row with column col's perturbation at sign sg: the row (qpos, qvel, qacc) into shared memory, the
-// perturbation (the root rotation as l_fd_load applies it), then k_inverse5's pass -- S1 with collisions, the body accelerations and
-// row residuals, the working set := (rs < 0) of every row, the inward force sweep -- leaving qfrc_inverse in the qvel row.  Returns
-// L_FD_SOLVER when the pass dropped joint-limit rows or saw a non-finite value in its inputs or its result.
+// one inverse pass (l_inv_pass) of the slot's rows with column col's perturbation at sign sg, leaving qfrc_inverse in the qvel row.
+// Returns L_FD_SOLVER when the pass dropped joint-limit rows or saw a non-finite value in its inputs or its result.
 template <class C>
-__device__ __noinline__ int l_ifd_pass(const float* ms, float* sm, const LLane& w, const LInvFdArgs& a, size_t row, int col, float sg) {
-  const LHdr& H = l_hdr<C>(ms);
-  const int nv = H.nv;
-  if (w.live && w.li == 0) { ((int*)sm)[C::misc + LMI_NSELF] = 0; ((int*)sm)[C::misc + LMI_NCON] = 0; ((int*)sm)[C::misc + LMI_NLIM] = 0; }
-  if (w.live) for (int i = w.li; i < (H.nslot + 3) / 4; i += LM_LPE) ((int*)sm)[C::pfl + i] = 0;
-  l_copy_in<C>(sm + C::qpos, a.qpos + row * (nv + 1), nv + 1, w);
-  l_copy_in<C>(sm + C::qvel, a.qvel + row * nv, nv, w);
-  l_copy_in<C>(sm + C::qacc, a.qacc + row * nv, nv, w);
-  __syncwarp();
-  if (w.live && w.li == 0) {
-    const float x = l_ifd_value(a, nv, row, col, sg);
-    if (col >= 3 && col < 6) {   // q (x) exp(x e_k), normalised
-      float* qp = sm + C::qpos + 3;
-      float sn, cs;
-      l_sincos(0.5f * x, &sn, &cs);
-      Q4 q; q.w = qp[0]; q.x = qp[1]; q.y = qp[2]; q.z = qp[3];
-      Q4 d; d.w = cs; d.x = col == 3 ? sn : 0.f; d.y = col == 4 ? sn : 0.f; d.z = col == 5 ? sn : 0.f;
-      q = qnormalize(qmul(q, d));
-      qp[0] = q.w; qp[1] = q.x; qp[2] = q.y; qp[3] = q.z;
-    } else if (col < nv) sm[C::qpos + (col < 3 ? col : col + 1)] = x;
-    else if (col < 2 * nv) sm[C::qvel + col - nv] = x;
-    else sm[C::qacc + col - 2 * nv] = x;
-  }
-  __syncwarp();
-  bool bad = l_ifd_bad<C>(sm + C::qpos, nv + 1, w) | l_ifd_bad<C>(sm + C::qvel, nv, w) | l_ifd_bad<C>(sm + C::qacc, nv, w);
-  const LFkOut fk = l_sweep_out<C>(ms, sm, w, LF_FK | LF_VEL | LF_COLLIDE, false);
-  l_inv_acc<C>(ms, sm, w);
+__device__ __noinline__ int l_ifd_pass(const float* ms, float* sm, const LLane& w, const LFdCols& f, const float* qpos, const float* qvel,
+                                       const float* qacc, int col, float sg) {
+  const int nv = l_hdr<C>(ms).nv;
+  bool bad = false;
   float o4[5];
-  l_rows<C>(sm, w, w.live, 0, 0.f, o4);   // working set := (rs < 0) of every row, as k_inverse5
-  __syncwarp();
-  l_inv_force<C>(ms, sm, w);
+  const LFkOut fk = l_inv_pass<C>(ms, sm, w, o4, [&] {
+    l_copy_in<C>(sm + C::qpos, qpos, nv + 1, w);
+    l_copy_in<C>(sm + C::qvel, qvel, nv, w);
+    l_copy_in<C>(sm + C::qacc, qacc, nv, w);
+    l_fd_perturb<C>(sm, w, f, nv, qpos, qvel, qacc, C::qacc, col, sg);
+    bad = l_ifd_bad<C>(sm + C::qpos, nv + 1, w) | l_ifd_bad<C>(sm + C::qvel, nv, w) | l_ifd_bad<C>(sm + C::qacc, nv, w);
+  });
   bad = bad | l_ifd_bad<C>(sm + C::qvel, nv, w);
   return (bad || fk.dropped) ? L_FD_SOLVER : 0;
 }
@@ -80,32 +51,32 @@ template <class C>
 __global__ void __launch_bounds__(256, 1) k_invfd5(const float* __restrict__ gimg, int img_bytes, LInvFdArgs a) {
   const float* ms; LLane w;
   float* sm = l_setup<C>(gimg, img_bytes, w, ms, a.n, a.map, a.gscr, nullptr, nullptr);
-  const LHdr& H = l_hdr<C>(ms);
-  const int nv = H.nv, ncol = 3 * nv;
+  const int nv = l_hdr<C>(ms).nv, ncol = a.fd.ncol;
   const size_t eo = w.live ? (size_t)w.env : 0;
-  const long long s = a.s0 + (long long)eo;
+  const long long s = a.fd.s0 + (long long)eo;
   const size_t row = (size_t)(s / ncol);
   const int col = (int)(s % ncol);
+  const float *qpos = a.qpos + row * (nv + 1), *qvel = a.qvel + row * nv, *qacc = a.qacc + row * nv;
   unsigned sig0 = 0u;
   int flag = 0;
-  for (int p = 0; p <= (a.centered ? 1 : 0); p++) {
-    flag |= l_ifd_pass<C>(ms, sm, w, a, row, col, p ? -1.f : 1.f);
+  for (int p = 0; p <= (a.fd.centered ? 1 : 0); p++) {
+    flag |= l_ifd_pass<C>(ms, sm, w, a.fd, qpos, qvel, qacc, col, p ? -1.f : 1.f);
     const unsigned sig = l_active_sig<C>(sm, w);
-    if (p == 0 && a.centered) {
+    if (p == 0 && a.fd.centered) {
       sig0 = sig;
-      l_copy_out<C>(a.gfd + eo * nv, sm + C::qvel, nv, w);
+      l_copy_out<C>(a.fd.gfd + eo * C::NV, sm + C::qvel, nv, w);
       __syncwarp();
     } else if (p == 1 && sig != sig0) flag |= L_FD_KINK;
   }
   if (!w.live) return;
-  const float den = l_ifd_value(a, nv, row, col, 1.f) - l_ifd_value(a, nv, row, col, a.centered ? -1.f : 0.f);
-  const float* fp = a.centered ? a.gfd + eo * nv : sm + C::qvel;
-  const float* fm = a.centered ? sm + C::qvel : a.qfrc + row * nv;
+  const float den = l_fd_den(a.fd, qpos, qvel, qacc, nv, col);
+  const float* fp = a.fd.centered ? a.fd.gfd + eo * C::NV : sm + C::qvel;
+  const float* fm = a.fd.centered ? sm + C::qvel : a.qfrc + row * nv;
   for (int i = w.li; i < nv; i += LM_LPE) {
     const float d = l_div_rn(fp[i] - fm[i], den);
     if (a.dfrc) a.dfrc[(row * nv + i) * ncol + col] = d;
   }
-  if (a.flags && w.li == 0) a.flags[row * ncol + col] = (uint8_t)flag;
+  if (a.fd.flags && w.li == 0) a.fd.flags[row * ncol + col] = (uint8_t)flag;
 }
 
 void lane_invfd_kernels(int cls, void (**k)(const float*, int, LInvFdArgs)) {

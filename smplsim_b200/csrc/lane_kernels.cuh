@@ -2579,6 +2579,25 @@ __device__ __noinline__ void l_inv_force(const float* ms, float* sm, const LLane
 // Uses the handle's per-env scratch (lane records, overflow contact entries) of the rows it runs; writes neither the working-set memory
 // (gpfl) nor the sensor rows (gsens), so the stepper cannot tell that it ran.
 struct LInvArgs { const float* qpos; const float* qvel; const float* qacc; float* qfrc; float* cwrench; float* gscr; LMap map; int n; };
+
+// the pass of k_inverse5 and k_invfd5: clear the row counts and working-set memory, load() qpos, qvel, qacc into shared memory, S1 with
+// collisions, l_inv_acc, the working set := (rs < 0) of every row, l_inv_force; qfrc_inverse ends in the qvel row.  o4 (l_rows' output)
+// is the caller's: as a local here it would take k_inverse5's first stack slot and change its SASS.
+template <class C, class Load>
+__device__ __forceinline__ LFkOut l_inv_pass(const float* ms, float* sm, const LLane& w, float* o4, Load load) {
+  const LHdr& H = l_hdr<C>(ms);
+  if (w.live && w.li == 0) { ((int*)sm)[C::misc + LMI_NSELF] = 0; ((int*)sm)[C::misc + LMI_NCON] = 0; ((int*)sm)[C::misc + LMI_NLIM] = 0; }
+  if (w.live) for (int i = w.li; i < (H.nslot + 3) / 4; i += LM_LPE) ((int*)sm)[C::pfl + i] = 0;
+  load();
+  __syncwarp();
+  const LFkOut fk = l_sweep_out<C>(ms, sm, w, LF_FK | LF_VEL | LF_COLLIDE, false);
+  l_inv_acc<C>(ms, sm, w);
+  l_rows<C>(sm, w, w.live, 0, 0.f, o4);
+  __syncwarp();
+  l_inv_force<C>(ms, sm, w);
+  return fk;
+}
+
 template <class C>
 __global__ void __launch_bounds__(256, 1) k_inverse5(const float* __restrict__ gimg, int img_bytes, LInvArgs a) {
   const float* ms; LLane w;
@@ -2586,18 +2605,12 @@ __global__ void __launch_bounds__(256, 1) k_inverse5(const float* __restrict__ g
   const LHdr& H = l_hdr<C>(ms);
   const size_t eo = w.live ? (size_t)w.env : 0;
   if constexpr (C::PRM) l_prm_stage<C>(ms, sm, w);
-  if (w.live && w.li == 0) { ((int*)sm)[C::misc + LMI_NSELF] = 0; ((int*)sm)[C::misc + LMI_NCON] = 0; ((int*)sm)[C::misc + LMI_NLIM] = 0; }
-  if (w.live) for (int i = w.li; i < (H.nslot + 3) / 4; i += LM_LPE) ((int*)sm)[C::pfl + i] = 0;
-  l_copy_in<C>(sm + C::qpos, a.qpos + eo * (H.nv + 1), H.nv + 1, w);
-  l_copy_in<C>(sm + C::qvel, a.qvel + eo * H.nv, H.nv, w);
-  l_copy_in<C>(sm + C::qacc, a.qacc + eo * H.nv, H.nv, w);
-  __syncwarp();
-  l_sweep_out<C>(ms, sm, w, LF_FK | LF_VEL | LF_COLLIDE, false);
-  l_inv_acc<C>(ms, sm, w);
   float o4[5];
-  l_rows<C>(sm, w, w.live, 0, 0.f, o4);   // working set := (rs < 0) of every row (its phi / r bookkeeping is not read here)
-  __syncwarp();
-  l_inv_force<C>(ms, sm, w);
+  l_inv_pass<C>(ms, sm, w, o4, [&] {
+    l_copy_in<C>(sm + C::qpos, a.qpos + eo * (H.nv + 1), H.nv + 1, w);
+    l_copy_in<C>(sm + C::qvel, a.qvel + eo * H.nv, H.nv, w);
+    l_copy_in<C>(sm + C::qacc, a.qacc + eo * H.nv, H.nv, w);
+  });
   if (a.cwrench) l_contact_wrench<C>(ms, sm, w, 0, a.cwrench);
   l_copy_out<C>(a.qfrc + eo * H.nv, sm + C::qvel, H.nv, w);
 }
@@ -2765,11 +2778,13 @@ __global__ void __launch_bounds__(256, 1) k_dyn5(const float* __restrict__ gimg,
 // working-set memory nor the sensor rows, so the stepper cannot tell that it ran.
 #define L_FD_KINK 1     // SMPLSIM_FD_KINK: the two solves of the column ended on different active sets
 #define L_FD_SOLVER 2   // SMPLSIM_FD_SOLVER: a solve of the column hit the iteration cap, dropped rows or saw a non-finite value
+// the column fields of LFwdArgs and LInvFdArgs: slot s is row s / ncol, column s % ncol; gfd [num_envs, NV]; flags [n, ncol] (NULL: none)
+struct LFdCols { float* gfd; uint8_t* flags; long long s0; int ncol, centered; float eps[3]; };
 struct LFwdArgs {
   const float* qpos; const float* qvel; const float* ctrl; const float* qacc_warm;   // column pass: qacc_warm = the nominal qacc
   float* qacc; uint64_t* contact_mask; int32_t* solver_iter; uint8_t* status; float* cwrench;
-  float* gscr; float* gfd; LMap map; int n;
-  float* dqacc; float* A; float* B; uint8_t* flags; long long s0; int ncol, centered; float eps[3];
+  float* gscr; LMap map; int n;
+  float* dqacc; float* A; float* B; LFdCols fd;
 };
 
 #ifdef SMPLSIM_EMU
@@ -2820,26 +2835,26 @@ __device__ __noinline__ unsigned l_active_sig(float* sm, const LLane& w) {
   return s;
 }
 
-// the perturbed input of column col at sign sg (0: the nominal): a qpos entry of the root translation or a hinge, a qvel or a ctrl
-// entry; for a root-rotation column the angle sg eps of q (x) exp(sg eps e_k)
-__device__ __forceinline__ float l_fd_value(const LFwdArgs& a, int nv, int nu, size_t row, int col, float sg) {
-  if (col < nv) return (col >= 3 && col < 6) ? sg * a.eps[0] : a.qpos[row * (nv + 1) + (col < 3 ? col : col + 1)] + sg * a.eps[0];
-  if (col < 2 * nv) return a.qvel[row * nv + col - nv] + sg * a.eps[1];
-  return a.ctrl[row * nu + col - 2 * nv] + sg * a.eps[2];
+// FD columns over x = [dq (nv) ; qvel (nv) ; z], z = ctrl (transition) or qacc (inverse).  Column col at sign sg (0: nominal) of the rows
+// qpos, qvel, z: a root translation, hinge, qvel or z entry; for a root-rotation column the angle sg eps of q (x) exp(sg eps e_k)
+__device__ __forceinline__ float l_fd_value(const LFdCols& f, const float* qpos, const float* qvel, const float* z, int nv, int col, float sg) {
+  if (col < nv) return (col >= 3 && col < 6) ? sg * f.eps[0] : qpos[col < 3 ? col : col + 1] + sg * f.eps[0];
+  if (col < 2 * nv) return qvel[col - nv] + sg * f.eps[1];
+  return z[col - 2 * nv] + sg * f.eps[2];
 }
 
-// the slot's row (qpos, qvel, ctrl -> tau, nominal qacc as the warm start) with column col's perturbation at sign sg
+// the column's denominator: the fp32 difference of the inputs the passes loaded (centered: x+ - x-; else x+ - x)
+__device__ __forceinline__ float l_fd_den(const LFdCols& f, const float* qpos, const float* qvel, const float* z, int nv, int col) {
+  return l_fd_value(f, qpos, qvel, z, nv, col, 1.f) - l_fd_value(f, qpos, qvel, z, nv, col, f.centered ? -1.f : 0.f);
+}
+
+// column col's perturbation at sign sg of the slot's rows, loaded into shared memory (z at sm + zo), between two __syncwarp
 template <class C>
-__device__ __noinline__ void l_fd_load(const float* ms, float* sm, const LLane& w, const LFwdArgs& a, size_t row, int col, float sg) {
-  const LHdr& H = l_hdr<C>(ms);
-  const int nv = H.nv, nu = H.nu;
-  l_copy_in<C>(sm + C::qpos, a.qpos + row * (nv + 1), nv + 1, w);
-  l_copy_in<C>(sm + C::qvel, a.qvel + row * nv, nv, w);
-  l_copy_in<C>(sm + C::tau, a.ctrl + row * nu, nu, w);
-  l_copy_in<C>(sm + C::qacc, a.qacc_warm + row * nv, nv, w);
+__device__ __forceinline__ void l_fd_perturb(float* sm, const LLane& w, const LFdCols& f, int nv, const float* qpos, const float* qvel,
+                                             const float* z, int zo, int col, float sg) {
   __syncwarp();
   if (w.live && w.li == 0) {
-    const float x = l_fd_value(a, nv, nu, row, col, sg);
+    const float x = l_fd_value(f, qpos, qvel, z, nv, col, sg);
     if (col >= 3 && col < 6) {   // q (x) exp(x e_k), normalised
       float* qp = sm + C::qpos + 3;
       float sn, cs;
@@ -2850,9 +2865,21 @@ __device__ __noinline__ void l_fd_load(const float* ms, float* sm, const LLane& 
       qp[0] = q.w; qp[1] = q.x; qp[2] = q.y; qp[3] = q.z;
     } else if (col < nv) sm[C::qpos + (col < 3 ? col : col + 1)] = x;
     else if (col < 2 * nv) sm[C::qvel + col - nv] = x;
-    else sm[C::tau + col - 2 * nv] = x;
+    else sm[zo + col - 2 * nv] = x;
   }
   __syncwarp();
+}
+
+// the slot's row for the forward pass (qpos, qvel, ctrl -> tau, nominal qacc as the warm start) with column col's perturbation
+template <class C>
+__device__ __noinline__ void l_fd_load(const float* ms, float* sm, const LLane& w, const LFwdArgs& a, size_t row, int col, float sg) {
+  const LHdr& H = l_hdr<C>(ms);
+  const int nv = H.nv, nu = H.nu;
+  l_copy_in<C>(sm + C::qpos, a.qpos + row * (nv + 1), nv + 1, w);
+  l_copy_in<C>(sm + C::qvel, a.qvel + row * nv, nv, w);
+  l_copy_in<C>(sm + C::tau, a.ctrl + row * nu, nu, w);
+  l_copy_in<C>(sm + C::qacc, a.qacc_warm + row * nv, nv, w);
+  l_fd_perturb<C>(sm, w, a.fd, nv, a.qpos + row * (nv + 1), a.qvel + row * nv, a.ctrl + row * nu, C::tau, col, sg);
 }
 
 // column col of dqacc (ap - am) / den, then of A or B by semi-implicit Euler (v' = v + h a, q' = q (+) h v'):  dv' = h dqacc + [qvel
@@ -2861,18 +2888,18 @@ __device__ __noinline__ void l_fd_load(const float* ms, float* sm, const LLane& 
 template <class C>
 __device__ __noinline__ void l_fd_write(const float* ms, float* sm, const LLane& w, const LFwdArgs& a, size_t row, int col, float den, int flag) {
   const LHdr& H = l_hdr<C>(ms);
-  const int nv = H.nv, nu = H.nu, ncol = a.ncol;
+  const int nv = H.nv, nu = H.nu, ncol = a.fd.ncol;
   const float h = H.h;
   const float* qnom = a.qacc_warm + row * nv;
   if (w.live) {
-    const float* ap = a.centered ? a.gfd + (size_t)w.env * C::NV : sm + C::qacc;
-    const float* am = a.centered ? sm + C::qacc : qnom;
+    const float* ap = a.fd.centered ? a.fd.gfd + (size_t)w.env * C::NV : sm + C::qacc;
+    const float* am = a.fd.centered ? sm + C::qacc : qnom;
     for (int i = w.li; i < nv; i += LM_LPE) {
       const float d = l_div_rn(ap[i] - am[i], den);
       sm[C::qacc + i] = d;
       if (a.dqacc) a.dqacc[(row * nv + i) * ncol + col] = d;
     }
-    if (a.flags && w.li == 0) a.flags[row * ncol + col] = (uint8_t)flag;
+    if (a.fd.flags && w.li == 0) a.fd.flags[row * ncol + col] = (uint8_t)flag;
   }
   __syncwarp();
   float* out = col < 2 * nv ? a.A : a.B;
@@ -2924,7 +2951,7 @@ __global__ void __launch_bounds__(256, 1) k_fwd5(const float* __restrict__ gimg,
   const LHdr& H = l_hdr<C>(ms);
   const size_t eo = w.live ? (size_t)w.env : 0;
   if constexpr (C::PRM) l_prm_stage<C>(ms, sm, w);
-  if (a.ncol == 0) {
+  if (a.fd.ncol == 0) {
     l_copy_in<C>(sm + C::qpos, a.qpos + eo * (H.nv + 1), H.nv + 1, w);
     l_copy_in<C>(sm + C::qvel, a.qvel + eo * H.nv, H.nv, w);
     l_copy_in<C>(sm + C::tau, a.ctrl + eo * H.nu, H.nu, w);
@@ -2941,24 +2968,25 @@ __global__ void __launch_bounds__(256, 1) k_fwd5(const float* __restrict__ gimg,
     }
     return;
   }
-  const long long s = a.s0 + (long long)eo;
-  const size_t row = (size_t)(s / a.ncol);
-  const int col = (int)(s % a.ncol);
+  const long long s = a.fd.s0 + (long long)eo;
+  const size_t row = (size_t)(s / a.fd.ncol);
+  const int col = (int)(s % a.fd.ncol);
+  // k_invfd5's column loop with the forward pass, written out: a shared driver slowed the forward rows (DESIGN.md 3, k_fwd5)
   unsigned sig0 = 0u;
   int flag = 0;
   float xp = 0.f;
-  for (int p = 0; p <= (a.centered ? 1 : 0); p++) {
+  for (int p = 0; p <= (a.fd.centered ? 1 : 0); p++) {
     l_fd_load<C>(ms, sm, w, a, row, col, p ? -1.f : 1.f);
     const LFwd fo = l_forward<C>(ms, sm, w);
     const unsigned sig = l_active_sig<C>(sm, w);
     if (fo.status & (1 | 2 | 4 | L_ST_ROWS_DROPPED | L_ST_MAXITER)) flag |= L_FD_SOLVER;
-    if (p == 0 && a.centered) {
+    if (p == 0 && a.fd.centered) {
       sig0 = sig;
-      l_copy_out<C>(a.gfd + eo * C::NV, sm + C::qacc, H.nv, w);
+      l_copy_out<C>(a.fd.gfd + eo * C::NV, sm + C::qacc, H.nv, w);
       __syncwarp();
     } else if (p == 1 && sig != sig0) flag |= L_FD_KINK;
   }
-  if (w.live) xp = l_fd_value(a, H.nv, H.nu, row, col, 1.f) - l_fd_value(a, H.nv, H.nu, row, col, a.centered ? -1.f : 0.f);
+  if (w.live) xp = l_fd_den(a.fd, a.qpos + row * (H.nv + 1), a.qvel + row * H.nv, a.ctrl + row * H.nu, H.nv, col);
   l_fd_write<C>(ms, sm, w, a, row, col, xp, flag);
 }
 
@@ -2986,17 +3014,15 @@ struct LRollArgs {
 void lane_roll_kernels(int cls, void (*k[2])(const float*, int, LRollArgs));
 
 // ------------------------------------------------------------------ finite-difference inverse-dynamics derivatives (mjd_inverseFD)
-// Slot s of a launch works on row s / 3nv and column s % 3nv of x = [dq (nv) ; qvel (nv) ; qacc (nv)] (the root rotation as q (x)
-// exp(d)): k_inverse5's pass at x + eps and (centered) x - eps, column col of dfrc = d qfrc_inverse / dx divided by the fp32 difference
-// of the inputs loaded, and the column's flags (L_FD_KINK: the two passes ended on different row sets; L_FD_SOLVER: a pass dropped
-// joint-limit rows or saw a non-finite value).  Not centered, the one pass is differenced against the nominal qfrc (the row pass of
-// smplsim_inverse).  Uses the handle's per-env scratch of the slots it runs (lane records, overflow contact entries, gfd); writes
-// neither the working-set memory nor the sensor rows, so the stepper cannot tell that it ran.
+// The column pass of k_fwd5 over x = [dq ; qvel ; qacc], ncol = 3nv, with k_inverse5's pass: column col of dfrc = d qfrc_inverse / dx
+// and its flags (L_FD_SOLVER: a pass dropped joint-limit rows or saw a non-finite value).  Not centered, differenced against the nominal
+// qfrc (smplsim_inverse's row pass).  Uses the handle's per-env scratch of the slots it runs (lane records, overflow contact entries,
+// gfd); writes neither the working-set memory nor the sensor rows, so the stepper cannot tell that it ran.
 struct LInvFdArgs {
   const float* qpos; const float* qvel; const float* qacc; const float* qfrc;   // [n, nq | nv]; qfrc: the nominal qfrc_inverse
-  float* dfrc; uint8_t* flags;   // [n, nv, 3nv], [n, 3nv]; each NULL: not written
-  float* gscr; float* gfd; LMap map; int n;
-  long long s0; int centered; float eps[3];   // eps_qpos, eps_qvel, eps_qacc
+  float* dfrc;   // [n, nv, 3nv]; NULL: not written
+  float* gscr; LMap map; int n;
+  LFdCols fd;   // eps: eps_qpos, eps_qvel, eps_qacc
 };
 
 // k_invfd5<C> is defined and instantiated in inverse_fd_kernels.cu, a translation unit of its own as k_roll5 is, so that its callers of

@@ -472,17 +472,37 @@ extern "C" int smplsim_forward(SmplsimHandle* h, const float* qpos_dev, const fl
                       contact_wrench_dev, (cudaStream_t)stream);
 }
 
+// the refusals smplsim_transition_fd and smplsim_inverse_fd share, in order; selfcol: why fn refuses self-collision handles
+static int fd_refusals(const SmplsimHandle* h, const std::string& fn, const char* selfcol, const char* eps_names, const float eps[3]) {
+  if (h->selfcol) return fail(SMPLSIM_EUNSUPPORTED, fn + ": " + selfcol + " (handle created with self_collision = 1)");
+  if (h->nblocks) return fail(SMPLSIM_EUNSUPPORTED, fn + ": not available with per-env body shapes (the column slots of a row span CTAs of any shape)");
+  if (h->prm) return fail(SMPLSIM_EUNSUPPORTED, fn + ": not available while the handle has per-env parameter records (smplsim_clear_env_params)");
+  for (int k = 0; k < 3; k++)
+    if (!(std::isfinite(eps[k]) && eps[k] > 0.f)) return fail(SMPLSIM_EINVAL, fn + ": " + eps_names + " must be finite and > 0");
+  return SMPLSIM_OK;
+}
+
+// the column launches of smplsim_transition_fd and smplsim_inverse_fd: n rows of a.fd.ncol slots, in launches of at most num_envs
+// slots (the handle's per-env scratch rows), in order on st; kern picks the kernel from lane_kernels
+template <class A, class K>
+static int fd_columns(SmplsimHandle* h, A a, int n, K kern, cudaStream_t st) {
+  a.gscr = h->gscr; a.map = h->map(); a.fd.gfd = h->gfd;
+  const long long slots = (long long)n * a.fd.ncol;
+  for (long long s0 = 0; s0 < slots; s0 += h->num_envs) {
+    a.fd.s0 = s0; a.n = (int)std::min<long long>(h->num_envs, slots - s0);
+    L_DISPATCH(h, lane_launch<C_>(h, kern(lane_kernels<C_>()), a.n, st, a));
+  }
+  CUDA_TRY(cudaGetLastError());
+  return SMPLSIM_OK;
+}
+
 extern "C" int smplsim_transition_fd(SmplsimHandle* h, const SmplsimFdCfg* cfg, const float* qpos_dev, const float* qvel_dev, const float* ctrl_dev,
                                      int n, float* qacc_dev, float* dqacc_dev, float* A_dev, float* B_dev, uint8_t* flags_dev, void* stream) {
   if (!h || !cfg || n < 0) return fail(SMPLSIM_EINVAL, "smplsim_transition_fd: null handle / cfg or n < 0");
-  if (h->selfcol)
-    return fail(SMPLSIM_EUNSUPPORTED, "smplsim_transition_fd: the forward pass on caller rows does not build geom-geom contacts (handle created with self_collision = 1)");
-  if (h->nblocks)
-    return fail(SMPLSIM_EUNSUPPORTED, "smplsim_transition_fd: not available with per-env body shapes (the column slots of a row span CTAs of any shape)");
-  if (h->prm)
-    return fail(SMPLSIM_EUNSUPPORTED, "smplsim_transition_fd: not available while the handle has per-env parameter records (smplsim_clear_env_params)");
-  for (float e : {cfg->eps_qpos, cfg->eps_qvel, cfg->eps_ctrl})
-    if (!(std::isfinite(e) && e > 0.f)) return fail(SMPLSIM_EINVAL, "smplsim_transition_fd: eps_qpos, eps_qvel and eps_ctrl must be finite and > 0");
+  LFwdArgs a; std::memset(&a, 0, sizeof a);
+  a.fd.eps[0] = cfg->eps_qpos; a.fd.eps[1] = cfg->eps_qvel; a.fd.eps[2] = cfg->eps_ctrl;
+  if (int rc = fd_refusals(h, "smplsim_transition_fd", "the forward pass on caller rows does not build geom-geom contacts",
+                           "eps_qpos, eps_qvel and eps_ctrl", a.fd.eps)) return rc;
   if (n == 0) return SMPLSIM_OK;   // nothing is read: empty tensors may come as NULL
   if (!qpos_dev || !qvel_dev || !ctrl_dev || !qacc_dev) return fail(SMPLSIM_EINVAL, "smplsim_transition_fd: null argument (qpos, qvel, ctrl and qacc are required)");
   if (!dqacc_dev && !A_dev && !B_dev && !flags_dev) return fail(SMPLSIM_EINVAL, "smplsim_transition_fd: no derivative output requested (dqacc, A, B and flags all NULL)");
@@ -490,30 +510,17 @@ extern "C" int smplsim_transition_fd(SmplsimHandle* h, const SmplsimFdCfg* cfg, 
   const cudaStream_t st = (cudaStream_t)stream;
   if (int rc = forward_rows(h, qpos_dev, qvel_dev, ctrl_dev, nullptr, n, qacc_dev, nullptr, nullptr, nullptr, nullptr, st)) return rc;
   const LHdr& H = *h->img.hdr();
-  LFwdArgs a; std::memset(&a, 0, sizeof a);
-  a.qpos = qpos_dev; a.qvel = qvel_dev; a.ctrl = ctrl_dev; a.qacc_warm = qacc_dev; a.gscr = h->gscr; a.gfd = h->gfd; a.map = h->map();
-  a.dqacc = dqacc_dev; a.A = A_dev; a.B = B_dev; a.flags = flags_dev; a.ncol = 2 * H.nv + H.nu; a.centered = cfg->centered ? 1 : 0;
-  a.eps[0] = cfg->eps_qpos; a.eps[1] = cfg->eps_qvel; a.eps[2] = cfg->eps_ctrl;
-  const long long slots = (long long)n * a.ncol;
-  for (long long s0 = 0; s0 < slots; s0 += h->num_envs) {   // launches of at most num_envs slots (the handle's scratch rows), in order
-    a.s0 = s0; a.n = (int)std::min<long long>(h->num_envs, slots - s0);
-    L_DISPATCH(h, lane_launch<C_>(h, lane_kernels<C_>().fwd[0], a.n, st, a));
-  }
-  CUDA_TRY(cudaGetLastError());
-  return SMPLSIM_OK;
+  a.qpos = qpos_dev; a.qvel = qvel_dev; a.ctrl = ctrl_dev; a.qacc_warm = qacc_dev; a.dqacc = dqacc_dev; a.A = A_dev; a.B = B_dev;
+  a.fd.flags = flags_dev; a.fd.ncol = 2 * H.nv + H.nu; a.fd.centered = cfg->centered ? 1 : 0;
+  return fd_columns(h, a, n, [](const LaneKernels& k) { return k.fwd[0]; }, st);
 }
 
 extern "C" int smplsim_inverse_fd(SmplsimHandle* h, const SmplsimInverseFdCfg* cfg, const float* qpos_dev, const float* qvel_dev,
                                   const float* qacc_dev, int n, float* qfrc_inverse_dev, float* dfrc_dev, uint8_t* flags_dev, void* stream) {
   if (!h || !cfg || n < 0) return fail(SMPLSIM_EINVAL, "smplsim_inverse_fd: null handle / cfg or n < 0");
-  if (h->selfcol)
-    return fail(SMPLSIM_EUNSUPPORTED, "smplsim_inverse_fd: the inverse does not build geom-geom contacts (handle created with self_collision = 1)");
-  if (h->nblocks)
-    return fail(SMPLSIM_EUNSUPPORTED, "smplsim_inverse_fd: not available with per-env body shapes (the column slots of a row span CTAs of any shape)");
-  if (h->prm)
-    return fail(SMPLSIM_EUNSUPPORTED, "smplsim_inverse_fd: not available while the handle has per-env parameter records (smplsim_clear_env_params)");
-  for (float e : {cfg->eps_qpos, cfg->eps_qvel, cfg->eps_qacc})
-    if (!(std::isfinite(e) && e > 0.f)) return fail(SMPLSIM_EINVAL, "smplsim_inverse_fd: eps_qpos, eps_qvel and eps_qacc must be finite and > 0");
+  LInvFdArgs a; std::memset(&a, 0, sizeof a);
+  a.fd.eps[0] = cfg->eps_qpos; a.fd.eps[1] = cfg->eps_qvel; a.fd.eps[2] = cfg->eps_qacc;
+  if (int rc = fd_refusals(h, "smplsim_inverse_fd", "the inverse does not build geom-geom contacts", "eps_qpos, eps_qvel and eps_qacc", a.fd.eps)) return rc;
   if (n == 0) return SMPLSIM_OK;   // nothing is read: empty tensors may come as NULL
   if (!qpos_dev || !qvel_dev || !qacc_dev || !qfrc_inverse_dev)
     return fail(SMPLSIM_EINVAL, "smplsim_inverse_fd: null argument (qpos, qvel, qacc and qfrc_inverse are required)");
@@ -521,19 +528,9 @@ extern "C" int smplsim_inverse_fd(SmplsimHandle* h, const SmplsimInverseFdCfg* c
   // the nominal pass is smplsim_inverse's row path, so qfrc_inverse is bit for bit what smplsim_inverse gives
   if (int rc = smplsim_inverse(h, qpos_dev, qvel_dev, qacc_dev, qfrc_inverse_dev, nullptr, n, stream)) return rc;
   DeviceGuard guard(h->device);
-  const cudaStream_t st = (cudaStream_t)stream;
-  const LHdr& H = *h->img.hdr();
-  LInvFdArgs a; std::memset(&a, 0, sizeof a);
-  a.qpos = qpos_dev; a.qvel = qvel_dev; a.qacc = qacc_dev; a.qfrc = qfrc_inverse_dev; a.dfrc = dfrc_dev; a.flags = flags_dev;
-  a.gscr = h->gscr; a.gfd = h->gfd; a.map = h->map(); a.centered = cfg->centered ? 1 : 0;
-  a.eps[0] = cfg->eps_qpos; a.eps[1] = cfg->eps_qvel; a.eps[2] = cfg->eps_qacc;
-  const long long slots = (long long)n * 3 * H.nv;
-  for (long long s0 = 0; s0 < slots; s0 += h->num_envs) {   // launches of at most num_envs slots (the handle's scratch rows), in order
-    a.s0 = s0; a.n = (int)std::min<long long>(h->num_envs, slots - s0);
-    L_DISPATCH(h, lane_launch<C_>(h, lane_kernels<C_>().invfd, a.n, st, a));
-  }
-  CUDA_TRY(cudaGetLastError());
-  return SMPLSIM_OK;
+  a.qpos = qpos_dev; a.qvel = qvel_dev; a.qacc = qacc_dev; a.qfrc = qfrc_inverse_dev; a.dfrc = dfrc_dev;
+  a.fd.flags = flags_dev; a.fd.ncol = 3 * h->img.hdr()->nv; a.fd.centered = cfg->centered ? 1 : 0;
+  return fd_columns(h, a, n, [](const LaneKernels& k) { return k.invfd; }, (cudaStream_t)stream);
 }
 
 extern "C" int smplsim_rollout(SmplsimHandle* h, int mode, int nsub, const float* qpos0_dev, const float* qvel0_dev, const float* qacc_warmstart_dev,

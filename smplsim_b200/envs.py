@@ -303,20 +303,20 @@ class HumanoidEnvB200(_EnvBase):
         qM = np.array([M[i, j] for i, j in _pairs(self._dof_parentid)])
         return qM, out["qfrc_bias"][0].cpu().numpy().astype(np.float64)
 
+    def _fd_row(self, fd, x, eps, **kw):
+        """The batch's ``fd`` (``transition_fd`` / ``inverse_fd``) at one state ``x`` (fp32 rows), eps (None: the defaults); fp64 outputs."""
+        dv = self._b.device
+        out = fd(*(torch.as_tensor(np.asarray(v, dtype=np.float32)[None], device=dv) for v in x), *(() if eps is None else (eps,) * 3), **kw)
+        return {k: v[0].cpu().numpy().astype(np.float64) for k, v in out.items()}
+
     def _transition_fd(self, qpos, qvel, ctrl, eps, centered):
-        """(A, B) of ``mjd_transitionFD`` at one state (fp32 rows of the given arrays; fp64 copies of the result)."""
-        b = self._b
-        e = b.FD_EPS if eps is None else (eps, eps, eps)
-        row = lambda x: torch.as_tensor(np.asarray(x, dtype=np.float32)[None], device=b.device)  # noqa: E731
-        out = b.transition_fd(row(qpos), row(qvel), row(ctrl), *e, centered=centered)
-        return out["A"][0].cpu().numpy().astype(np.float64), out["B"][0].cpu().numpy().astype(np.float64)
+        """(A, B) of ``mjd_transitionFD`` at one state."""
+        out = self._fd_row(self._b.transition_fd, (qpos, qvel, ctrl), eps, centered=centered)
+        return out["A"], out["B"]
 
     def _inverse_fd(self, qpos, qvel, qacc, eps):
-        """dfrc [nv, 3nv] of ``mjd_inverseFD`` at one state (fp32 rows of the given arrays; an fp64 copy of the result)."""
-        b = self._b
-        e = b.INVFD_EPS if eps is None else (eps, eps, eps)
-        row = lambda x: torch.as_tensor(np.asarray(x, dtype=np.float32)[None], device=b.device)  # noqa: E731
-        return b.inverse_fd(row(qpos), row(qvel), row(qacc), *e)["dfrc"][0].cpu().numpy().astype(np.float64)
+        """dfrc [nv, 3nv] of ``mjd_inverseFD`` at one state."""
+        return self._fd_row(self._b.inverse_fd, (qpos, qvel, qacc), eps)["dfrc"]
 
     def _rollout(self, initial_state, control, nstep):
         """(state, sensordata) of ``rollout``: ctrl-mode rollouts of the given rows (fp32 on the device; fp64 copies of the result)."""
