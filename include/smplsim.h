@@ -190,7 +190,7 @@ typedef struct SmplsimHandle SmplsimHandle;
 const char* smplsim_last_error(void);
 int smplsim_version(void);   /* 300 = this header (290: before smplsim_track_eval; 280: before smplsim_motion_blend and the interpolation / future-target fields; 270: before smplsim_amp_obs / smplsim_amp_demo; 260: before smplsim_imitation; 250: before smplsim_set_env_params; 240: before smplsim_ray / smplsim_render; 230: before smplsim_dynamics; 220: before smplsim_inverse;
                               * 210: before SmplsimAux.contact_wrench; 200: before SmplsimState.xfrc_applied; 100: before pid_* state and aux.status).
-                              * smplsim_forward, smplsim_transition_fd, smplsim_rollout and smplsim_inverse_fd came later without a new number, because callers
+                              * smplsim_forward, smplsim_transition_fd, smplsim_rollout, smplsim_inverse_fd and smplsim_centroidal came later without a new number, because callers
                               * compare it to 300 for equality: look them up by symbol (dlsym) rather than by version. */
 
 /* MjModel.from_xml_string + MjData + setup_humanoid_properties/setup_controller
@@ -358,6 +358,31 @@ int smplsim_rollout(SmplsimHandle* h, int mode, int nsub, const float* qpos0_dev
  * [MJ-upstream] mj_fullM / mj_rne / mj_jacBody (engine_support.c, engine_core_smooth.c); not checked against a MuJoCo wheel. */
 int smplsim_dynamics(SmplsimHandle* h, const float* qpos_dev, const float* qvel_dev, int n, float* qM_dev, float* qfrc_bias_dev,
                      const int32_t* jac_body, int njac, float* jac_dev, void* cuda_stream);
+
+/* Centre of mass and centroidal momentum on n caller rows qpos[n,nq], qvel[n,nv] (each output NULL: skipped).  World frame, robot body
+ * order: row b is body b's subtree, row 0 the root's, i.e. the whole robot (MuJoCo body 1):
+ *   subtree_com[n,nbody,3]     mj_data.subtree_com[1:]: centre of mass of each body's subtree;
+ *   subtree_linvel[n,nbody,3]  mj_subtreeVel: the velocity of that centre of mass;
+ *   subtree_angmom[n,nbody,3]  mj_subtreeVel: the subtree's angular momentum about its own centre of mass;
+ *   cmm[n,6,nv]                centroidal momentum matrix: rows 0-2 linear momentum, rows 3-5 angular momentum about the whole-body centre of
+ *                              mass, per unit qvel, so cmm qvel = [m subtree_linvel[0] ; subtree_angmom[0]]; bodies only (armature is not
+ *                              body momentum);
+ *   cmm_bias[n,6]              the momentum rate at qacc = 0 without gravity (Adot qvel, rows as cmm): for any qacc the momentum rate is
+ *                              cmm qacc + cmm_bias, and the net external wrench on the robot is that minus [m g ; 0];
+ *   jac_com[n,njac,3,nv]       mj_jacSubtreeCom of each listed body: the velocity of its subtree's centre of mass per unit qvel.
+ * jac_body: host array of njac robot body indices (0 = root, repeats allowed, njac <= nbody).  Root columns follow the qvel convention of
+ * smplsim_dynamics: [0:3] world-frame translation, [3:6] rotation about the root body's axes.  No output depends on gravity, so per-env
+ * gravity changes nothing; per-env body mass scales (parameter records) move the centre of mass and are taken.  Nothing here depends on
+ * contacts, so every handle kind is supported; no per-env state is read or written (a later smplsim_step is unaffected).  Row rules of
+ * smplsim_dynamics: single shape without parameter records, any n >= 0 (launched in pieces of at most num_envs rows on the stream); per-env
+ * shapes or parameter records: n == num_envs, row i uses env i.  SMPLSIM_EINVAL: a bad body index, njac > nbody, njac > 0 with
+ * jac_com_dev NULL, subtree_linvel / subtree_angmom / cmm_bias without qvel, a null qpos, or every output NULL with n > 0; n == 0
+ * reads nothing.
+ * [MJ-upstream] mj_comPos / mj_subtreeVel (engine_core_smooth.c), mj_jacSubtreeCom (engine_support.c); not checked against a MuJoCo
+ * wheel. */
+int smplsim_centroidal(SmplsimHandle* h, const float* qpos_dev, const float* qvel_dev, int n, float* subtree_com_dev,
+                       float* subtree_linvel_dev, float* subtree_angmom_dev, float* cmm_dev, float* cmm_bias_dev, const int32_t* jac_body,
+                       int njac, float* jac_com_dev, void* cuda_stream);
 
 /* Ray casting and camera images of the robot geoms and the floor, on caller body poses xpos[n,nbody,3] / xquat[n,nbody,4] (the
  * layout of SmplsimAux.xpos / xquat: the post-step poses a batch holds, smplsim_kinematics of any qpos, or motion-table rows).

@@ -574,6 +574,63 @@ class HumanoidBatchB200:
             self.gpu_launches += 1
         return out
 
+    def centroidal(self, qpos: torch.Tensor, qvel: Optional[torch.Tensor] = None, *, com: bool = True, velocity: bool = True, cmm: bool = True,
+                   jac_com_bodies: Optional[Sequence] = None):
+        """Centre of mass and centroidal momentum at caller rows ``(qpos, qvel)``, as MuJoCo's ``subtree_com``, ``mj_subtreeVel`` and
+        ``mj_jacSubtreeCom``, plus the centroidal momentum matrix.  Row ``b`` of the per-body outputs is body ``b``'s subtree; row 0 (the
+        root's) is the whole robot.  Returns a dict with the outputs asked for:
+
+        - ``subtree_com`` ``[n, nbody, 3]`` (``com``): the world-frame centre of mass of each subtree;
+        - ``subtree_linvel`` / ``subtree_angmom`` ``[n, nbody, 3]`` (``velocity``, needs ``qvel``): its velocity, and the subtree's angular
+          momentum about it;
+        - ``cmm`` ``[n, 6, nv]`` (``cmm``): the centroidal momentum matrix, linear momentum (rows 0-2) over angular momentum about the
+          whole-body centre of mass (rows 3-5) per unit qvel, so ``cmm @ qvel = [m subtree_linvel[:, 0] ; subtree_angmom[:, 0]]``;
+        - ``cmm_bias`` ``[n, 6]`` (``cmm`` and ``velocity``): the momentum rate at qacc = 0 without gravity, so that the rate at any qacc is
+          ``cmm @ qacc + cmm_bias`` (Newton-Euler: ``[m g + sum of external forces ; their torques about the centre of mass]``);
+        - ``jac_com`` ``[n, k, 3, nv]`` (``jac_com_bodies``: k robot body indices, 0 = root, or body names): the velocity of each listed
+          body's subtree centre of mass per unit qvel.
+
+        Root dofs follow the qvel convention: ``[0:3]`` world-frame translation, ``[3:6]`` rotation about the root body's axes.  No
+        output depends on gravity; per-env mass scales (``set_env_params``) are taken.  Float32 tensors on this batch's device, ``[n, nq]``
+        / ``[n, nv]``; any n on a one-shape batch without per-env parameters, n == num_envs otherwise (row i uses env i's shape and
+        parameters).  Reads no env state and changes none; every handle kind (self-collision too) is supported."""
+        m = self.model
+        if velocity and qvel is None:
+            raise ValueError("velocity=True needs qvel")
+        args = (("qpos", qpos, m.nq),) + ((("qvel", qvel, m.nv),) if qvel is not None else ())
+        rows = self._rows(args)
+        q, v = rows[0], (rows[1] if qvel is not None else None)
+        bodies = []
+        for b in (jac_com_bodies if jac_com_bodies is not None else []):
+            if isinstance(b, str):
+                if b not in m.body_names:
+                    raise ValueError(f"unknown body name {b!r}")
+                b = list(m.body_names).index(b)
+            if isinstance(b, bool) or not isinstance(b, (int, np.integer)) or not 0 <= int(b) < m.nbody:
+                raise ValueError(f"jac_com_bodies entries must be body names or indices in [0, {m.nbody}), got {b!r}")
+            bodies.append(int(b))
+        n, f32 = q.shape[0], dict(dtype=torch.float32, device=self.device)
+        out = {}
+        if com:
+            out["subtree_com"] = torch.empty(n, m.nbody, 3, **f32)
+        if velocity:
+            out["subtree_linvel"] = torch.empty(n, m.nbody, 3, **f32)
+            out["subtree_angmom"] = torch.empty(n, m.nbody, 3, **f32)
+        if cmm:
+            out["cmm"] = torch.empty(n, 6, m.nv, **f32)
+            if velocity:
+                out["cmm_bias"] = torch.empty(n, 6, **f32)
+        if jac_com_bodies is not None:
+            out["jac_com"] = torch.empty(n, len(bodies), 3, m.nv, **f32)
+        if com or velocity or cmm or bodies:
+            jb = np.ascontiguousarray(np.asarray(bodies, dtype=np.int32))
+            self._check(self._L().smplsim_centroidal(self._h, _ptr(q), _ptr(v), n, _ptr(out.get("subtree_com")), _ptr(out.get("subtree_linvel")),
+                                                     _ptr(out.get("subtree_angmom")), _ptr(out.get("cmm")), _ptr(out.get("cmm_bias")),
+                                                     C.c_void_p(jb.ctypes.data) if bodies else None, len(bodies),
+                                                     _ptr(out["jac_com"]) if bodies else None, self._stream()))
+            self.gpu_launches += 1
+        return out
+
     # ------------------------------------------------------------------ ray casting and cameras (mj_ray, mujoco.Renderer)
     def _checked(self, name, t, shape):
         """A caller tensor checked as xfrc_applied is: shape (None entries free), float32, this batch's device, contiguous."""

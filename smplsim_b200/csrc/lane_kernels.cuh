@@ -3029,3 +3029,21 @@ struct LInvFdArgs {
 // the noinline functions leave the SASS of the existing kernels alone.  lane_invfd_kernels (also there) hands the host code its instance
 // of class 1 (SMPL) or 2 (SMPL-X), without self-collision or parameter records.
 void lane_invfd_kernels(int cls, void (**k)(const float*, int, LInvFdArgs));
+
+// ------------------------------------------------------------------ centre of mass and centroidal momentum (mj_comPos's subtree_com, mj_subtreeVel, mj_jacSubtreeCom)
+// On caller rows (qpos, qvel; qvel NULL: zero, only without the velocity outputs), each output NULL: skipped, world frame, robot body
+// order (body 0's subtree = the whole robot): com / linvel / angmom [n, nb, 3] (subtree centre of mass, its velocity, the subtree's
+// angular momentum about it), cmm [n, 6, nv] (linear momentum over angular momentum about the whole-body centre of mass, per unit
+// qvel, armature left out), cbias [n, 6] (the momentum rate at qacc = 0 without gravity), jac [n, njac, 3, nv] (centre-of-mass
+// Jacobians of the subtrees of bodies jb).  Uses the handle's per-env scratch of the rows it runs (lane records, the overflow contact
+// entries); writes neither the working-set memory nor the sensor rows, so the stepper cannot tell that it ran.
+struct LCentArgs {
+  const float* qpos; const float* qvel;
+  float* com; float* linvel; float* angmom; float* cmm; float* cbias; float* jac;
+  float* gscr; LMap map; int n, njac; unsigned char jb[LM_MAXB];
+};
+
+// k_cent5<C> is defined and instantiated in centroidal_kernels.cu, a translation unit of its own as k_roll5 is.  lane_cent_kernels (also
+// there) hands the host code its instances, [0] plain, [1] with parameter records, of class 1 (SMPL) or 2 (SMPL-X), with or without
+// self-collision (nothing here depends on contacts).
+void lane_cent_kernels(int cls, int selfcol, void (*k[2])(const float*, int, LCentArgs));

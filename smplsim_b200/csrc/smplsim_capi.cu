@@ -92,6 +92,7 @@ struct LaneKernels {
   void (*fwd[2])(const float*, int, LFwdArgs);                          // [parameter records]
   void (*roll[2])(const float*, int, LRollArgs);                        // [parameter records]
   void (*invfd)(const float*, int, LInvFdArgs);                         // single shape, no parameter records
+  void (*cent[2])(const float*, int, LCentArgs);                        // [parameter records]
 };
 template <class C>
 static LaneKernels lane_kernels() {
@@ -103,6 +104,7 @@ static LaneKernels lane_kernels() {
   if constexpr (!C::SELFCOL) { k.fwd[0] = k_fwd5<C>; k.fwd[1] = k_fwd5<P>; }   // as inverse: none for a self-collision class
   if constexpr (!C::SELFCOL) lane_roll_kernels(C::NB == L_SMPL(0)::NB ? 1 : 2, k.roll);   // a module of its own (rollout_kernels.cu)
   if constexpr (!C::SELFCOL) lane_invfd_kernels(C::NB == L_SMPL(0)::NB ? 1 : 2, &k.invfd);   // as roll (inverse_fd_kernels.cu)
+  lane_cent_kernels(C::NB == L_SMPL(0)::NB ? 1 : 2, C::SELFCOL, k.cent);   // as roll (centroidal_kernels.cu); every class, as dyn
   return k;
 }
 
@@ -132,7 +134,7 @@ static int pick_wpb(SmplsimHandle* h) {
   };
   const LaneKernels K = lane_kernels<C>();
   if (!raise(K.step[0], K.step[1], K.step[2], K.reset[0], K.reset[1], K.kin, K.inverse[0], K.inverse[1], K.dyn[0], K.dyn[1], K.fwd[0], K.fwd[1],
-             K.roll[0], K.roll[1], K.invfd)) return -1;
+             K.roll[0], K.roll[1], K.invfd, K.cent[0], K.cent[1])) return -1;
   return best;
 }
 
@@ -434,6 +436,45 @@ extern "C" int smplsim_dynamics(SmplsimHandle* h, const float* qpos_dev, const f
     if (c.jac) c.jac += r * c.njac * 6 * nv;
   };
   L_DISPATCH(h, state_rows<C_>(h, lane_kernels<C_>().dyn, a, advance, (cudaStream_t)stream));
+  CUDA_TRY(cudaGetLastError());
+  return SMPLSIM_OK;
+}
+
+extern "C" int smplsim_centroidal(SmplsimHandle* h, const float* qpos_dev, const float* qvel_dev, int n, float* subtree_com_dev,
+                                  float* subtree_linvel_dev, float* subtree_angmom_dev, float* cmm_dev, float* cmm_bias_dev, const int32_t* jac_body,
+                                  int njac, float* jac_com_dev, void* stream) {
+  if (!h || n < 0 || njac < 0) return fail(SMPLSIM_EINVAL, "smplsim_centroidal: null handle, n < 0 or njac < 0");
+  const LHdr& H = *h->img.hdr();
+  if (njac > H.nb) return fail(SMPLSIM_EINVAL, "smplsim_centroidal: njac > nbody");
+  if (njac > 0 && !jac_body) return fail(SMPLSIM_EINVAL, "smplsim_centroidal: njac > 0 needs jac_body");
+  for (int j = 0; j < njac; j++)
+    if (jac_body[j] < 0 || jac_body[j] >= H.nb) return fail(SMPLSIM_EINVAL, "smplsim_centroidal: jac_body entry out of range [0, nbody)");
+  if ((subtree_linvel_dev || subtree_angmom_dev || cmm_bias_dev) && !qvel_dev)
+    return fail(SMPLSIM_EINVAL, "smplsim_centroidal: subtree_linvel, subtree_angmom and cmm_bias need qvel");
+  if (n == 0) return SMPLSIM_OK;   // nothing is read: empty tensors may come as NULL
+  if (njac > 0 && !jac_com_dev) return fail(SMPLSIM_EINVAL, "smplsim_centroidal: njac > 0 needs jac_com_dev");
+  if (!subtree_com_dev && !subtree_linvel_dev && !subtree_angmom_dev && !cmm_dev && !cmm_bias_dev && !njac)
+    return fail(SMPLSIM_EINVAL, "smplsim_centroidal: no output requested");
+  if (!qpos_dev) return fail(SMPLSIM_EINVAL, "smplsim_centroidal: null qpos");
+  if (int rc = env_rows(h, n, "smplsim_centroidal", true)) return rc;
+  DeviceGuard guard(h->device);
+  LCentArgs a; std::memset(&a, 0, sizeof a);
+  a.qpos = qpos_dev; a.qvel = qvel_dev; a.com = subtree_com_dev; a.linvel = subtree_linvel_dev; a.angmom = subtree_angmom_dev;
+  a.cmm = cmm_dev; a.cbias = cmm_bias_dev; a.jac = njac ? jac_com_dev : nullptr; a.gscr = h->gscr; a.n = n; a.njac = njac;
+  for (int j = 0; j < njac; j++) a.jb[j] = (unsigned char)jac_body[j];
+  a.map = h->map();
+  const size_t nv = H.nv, nb = H.nb;
+  auto advance = [nv, nb](LCentArgs& c, size_t r) {
+    c.qpos += r * (nv + 1);
+    if (c.qvel) c.qvel += r * nv;
+    if (c.com) c.com += r * nb * 3;
+    if (c.linvel) c.linvel += r * nb * 3;
+    if (c.angmom) c.angmom += r * nb * 3;
+    if (c.cmm) c.cmm += r * 6 * nv;
+    if (c.cbias) c.cbias += r * 6;
+    if (c.jac) c.jac += r * c.njac * 3 * nv;
+  };
+  L_DISPATCH(h, state_rows<C_>(h, lane_kernels<C_>().cent, a, advance, (cudaStream_t)stream));
   CUDA_TRY(cudaGetLastError());
   return SMPLSIM_OK;
 }
@@ -1030,4 +1071,5 @@ extern "C" int smplsim_debug_stats(int* out, int reset) {   // out: L_NSTATS cou
 #ifdef SMPLSIM_EMU
 #include "rollout_kernels.cu"   // the device build compiles it as a translation unit of its own (_lib.build)
 #include "inverse_fd_kernels.cu"   // as rollout_kernels.cu
+#include "centroidal_kernels.cu"   // as rollout_kernels.cu
 #endif

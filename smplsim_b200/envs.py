@@ -132,8 +132,38 @@ def rollout(model, data, initial_state, control, nstep=None):
     return data._rollout_fn(initial_state, control, nstep)
 
 
+def mj_subtreeVel(model, data):
+    """``mujoco.mj_subtreeVel`` for an env's ``mj_data``: fills ``data.subtree_linvel`` and ``data.subtree_angmom`` [nbody + 1, 3]
+    (MuJoCo body order; row 0, the world's subtree, is the whole robot's), the velocity of each subtree's centre of mass and the
+    subtree's angular momentum about it, at the state of the last forward pass as ``subtree_com``.  fp32 on the GPU
+    (``HumanoidBatchB200.centroidal``).  ``model`` is accepted for the signature and not read."""
+    c = data._cent()
+    data.subtree_linvel = c["subtree_linvel"].copy()
+    data.subtree_angmom = c["subtree_angmom"].copy()
+
+
+def mj_jacSubtreeCom(model, data, jacp, body):
+    """``mujoco.mj_jacSubtreeCom`` for an env's ``mj_data``: the [3, nv] Jacobian of the centre of mass of MuJoCo body ``body``'s
+    subtree (0 = world: the whole robot) at the state of the last forward pass, written into ``jacp`` in place (any shape of 3 nv
+    entries).  fp32 on the GPU.  ``model`` is accepted for the signature and not read."""
+    nb = data._cent()["subtree_com"].shape[0]
+    if isinstance(body, bool) or not isinstance(body, (int, np.integer)) or not 0 <= int(body) < nb:
+        raise ValueError(f"body must be a MuJoCo body id in [0, {nb}), got {body!r}")
+    jac = data._jac_com_fn(max(int(body) - 1, 0))
+    jacp.reshape(jac.size)[:] = jac.ravel()
+
+
 class _MjData(SimpleNamespace):
-    """``mj_data`` view.  ``qM`` / ``qfrc_bias`` cost a kernel call, so they are evaluated on first read."""
+    """``mj_data`` view.  ``qM`` / ``qfrc_bias`` and ``subtree_com`` cost a kernel call, so they are evaluated on first read."""
+
+    @property
+    def subtree_com(self):
+        return self._cent()["subtree_com"]
+
+    def _cent(self):
+        if "_cent_val" not in self.__dict__:
+            self._cent_val = self._cent_fn()
+        return self._cent_val
 
     @property
     def qM(self):
@@ -269,12 +299,14 @@ class HumanoidEnvB200(_EnvBase):
     # ------------------------------------------------------------------ mj_data-style views (examples poke env.mj_data)
     @property
     def mj_data(self):
-        """``qM`` (compressed, ``mj_model.dof_Madr`` layout) and ``qfrc_bias`` are those of the last forward pass, at
-        ``(qpos_fwd, qvel_fwd)``, as on an MjData after ``mj_step``."""
+        """``qM`` (compressed, ``mj_model.dof_Madr`` layout), ``qfrc_bias`` and ``subtree_com`` ([nbody + 1, 3], the world row the
+        whole robot's) are those of the last forward pass, at ``(qpos_fwd, qvel_fwd)``, as on an MjData after ``mj_step``
+        (``mj_kinematics`` does not refresh ``subtree_com``)."""
         b = self._b
         sens = np.concatenate([b.body_linvel[0].cpu().numpy().ravel(), b.body_angvel[0].cpu().numpy().ravel()])
         z3, z4 = np.zeros((1, 3)), np.array([[1.0, 0, 0, 0]])
-        return _MjData(_dyn_fn=self._fwd_dynamics, _fd_fn=self._transition_fd, _rollout_fn=self._rollout, _invfd_fn=self._inverse_fd, qpos=b.qpos[0].cpu().numpy().astype(np.float64), qvel=b.qvel[0].cpu().numpy().astype(np.float64),
+        return _MjData(_dyn_fn=self._fwd_dynamics, _fd_fn=self._transition_fd, _rollout_fn=self._rollout, _invfd_fn=self._inverse_fd,
+                               _cent_fn=self._centroidal, _jac_com_fn=self._jac_com, qpos=b.qpos[0].cpu().numpy().astype(np.float64), qvel=b.qvel[0].cpu().numpy().astype(np.float64),
                                ctrl=b.ctrl[0].cpu().numpy().astype(np.float64), qacc=b.qacc[0].cpu().numpy().astype(np.float64),
                                xpos=np.concatenate([z3, b.xpos[0].cpu().numpy()]), xquat=np.concatenate([z4, b.xquat[0].cpu().numpy()]),
                                sensordata=sens, contact=_Contacts(int(b.contact_mask[0].item())),
@@ -302,6 +334,18 @@ class HumanoidEnvB200(_EnvBase):
         M = out["qM"][0].cpu().numpy().astype(np.float64)
         qM = np.array([M[i, j] for i, j in _pairs(self._dof_parentid)])
         return qM, out["qfrc_bias"][0].cpu().numpy().astype(np.float64)
+
+    def _centroidal(self):
+        """subtree_com, subtree_linvel, subtree_angmom [nbody + 1, 3] at the state of the last forward pass, world row first (fp64)."""
+        b = self._b
+        out = b.centroidal(b.qpos_fwd, b.qvel_fwd, cmm=False)
+        return {k: np.concatenate([v[0, :1], v[0]]).astype(np.float64) for k, v in ((k, v.cpu().numpy()) for k, v in out.items())}
+
+    def _jac_com(self, body):
+        """jac_com [3, nv] of robot body ``body``'s subtree at the state of the last forward pass (fp64)."""
+        b = self._b
+        out = b.centroidal(b.qpos_fwd, None, com=False, velocity=False, cmm=False, jac_com_bodies=[body])
+        return out["jac_com"][0, 0].cpu().numpy().astype(np.float64)
 
     def _fd_row(self, fd, x, eps, **kw):
         """The batch's ``fd`` (``transition_fd`` / ``inverse_fd``) at one state ``x`` (fp32 rows), eps (None: the defaults); fp64 outputs."""

@@ -255,6 +255,12 @@ class MotionLibB200:
         qacc = (qvel[hi] - qvel[lo]) / self._motion_dt[clip][:, None]
         return self.env.inverse(qpos, qvel, qacc, contact_wrench=contact_wrench)
 
+    def centroidal(self, **kw):
+        """``env.centroidal`` over every frame of the library: subtree centres of mass, their velocities, angular momenta, the
+        centroidal momentum matrix and its bias, and COM Jacobians of the frames' ``qpos`` / ``qvel``, indexed like the tables.  Keywords
+        go to ``centroidal`` (``com``, ``velocity``, ``cmm``, ``jac_com_bodies``)."""
+        return self.env.centroidal(self.tables["qpos"], self.tables["qvel"], **kw)
+
     def render_clip(self, motion_id: int, camera="side", width: int = 320, height: int = 240, **kw):
         """``env.render`` of every frame of clip ``motion_id`` from the library's ``xpos`` / ``xquat`` tables: ``rgb [F, H, W, 3]``
         uint8 (F = the clip's frame count).  Further keywords go to ``render`` (``geom_rgb``).  Needs a one-shape batch."""
