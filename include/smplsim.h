@@ -190,7 +190,7 @@ typedef struct SmplsimHandle SmplsimHandle;
 const char* smplsim_last_error(void);
 int smplsim_version(void);   /* 300 = this header (290: before smplsim_track_eval; 280: before smplsim_motion_blend and the interpolation / future-target fields; 270: before smplsim_amp_obs / smplsim_amp_demo; 260: before smplsim_imitation; 250: before smplsim_set_env_params; 240: before smplsim_ray / smplsim_render; 230: before smplsim_dynamics; 220: before smplsim_inverse;
                               * 210: before SmplsimAux.contact_wrench; 200: before SmplsimState.xfrc_applied; 100: before pid_* state and aux.status).
-                              * smplsim_forward, smplsim_transition_fd, smplsim_rollout, smplsim_inverse_fd and smplsim_centroidal came later without a new number, because callers
+                              * smplsim_forward, smplsim_transition_fd, smplsim_rollout, smplsim_inverse_fd, smplsim_centroidal and smplsim_rne_post came later without a new number, because callers
                               * compare it to 300 for equality: look them up by symbol (dlsym) rather than by version. */
 
 /* MjModel.from_xml_string + MjData + setup_humanoid_properties/setup_controller
@@ -383,6 +383,34 @@ int smplsim_dynamics(SmplsimHandle* h, const float* qpos_dev, const float* qvel_
 int smplsim_centroidal(SmplsimHandle* h, const float* qpos_dev, const float* qvel_dev, int n, float* subtree_com_dev,
                        float* subtree_linvel_dev, float* subtree_angmom_dev, float* cmm_dev, float* cmm_bias_dev, const int32_t* jac_body,
                        int njac, float* jac_com_dev, void* cuda_stream);
+
+/* Body accelerations, joint reaction wrenches and IMU readings (mj_rnePostConstraint's cacc / cfrc_int and the acceleration-stage
+ * sensors) on n caller rows qpos[n,nq], qvel[n,nv], qacc[n,nv] (all required), with xfrc_applied[n,nbody,6] (NULL: none; the layout
+ * and convention of SmplsimState.xfrc_applied).  Each output NULL: skipped; world frame, robot body order:
+ *   body_acc[n,nbody,6]      rows 0-2 the linear acceleration of the body origin, d^2 xpos / dt^2 (gravity not included), rows 3-5 the
+ *                            angular acceleration: J_b qacc + Jdot_b qvel, rows as smplsim_dynamics' jac;
+ *   joint_wrench[n,nbody,6]  the wrench body b's parent (the world, for the root) applies to b's subtree through b's joint (MuJoCo's
+ *                            cfrc_int): world-frame force, then torque about the body origin xpos.  It is the subtree's net inertial
+ *                            wrench (gravity and the velocity products included) minus the floor-contact forces and xfrc_applied acting
+ *                            on the subtree; joint-limit forces act between parent and child and appear only here.  For a hinge k of
+ *                            body b, S_k^T F_b = qfrc_inverse_k - armature_k qacc_k + the limit force on dof k (no xfrc_applied);
+ *   accelerometer / gyro / force / torque [n,nsite,3]  per IMU site s, on robot body site_body[s] at site_pos[s] (body frame) with
+ *                            orientation site_quat[s] (wxyz unit quaternion, body frame): R_s^T (a_site - g) (the proper acceleration:
+ *                            +|g| upward at rest, zero in free fall; g the env's gravity), R_s^T w_b, and joint_wrench of the site's body
+ *                            moved to the site point in the site frame (MuJoCo's accelerometer, gyro, force and torque sensors).
+ * site_body / site_pos / site_quat are host arrays of nsite <= 64 entries.  The floor-contact and joint-limit forces are those of
+ * smplsim_inverse at (qpos, qvel, qacc): f = -D min(0, J qacc - aref) over the rows mj_forward at (qpos, qvel) builds.  Row rules of
+ * smplsim_inverse: single shape without parameter records, any n >= 0 (launched in pieces of at most num_envs rows on the stream);
+ * per-env shapes or parameter records: n == num_envs, row i uses env i (its gravity and mass scales); self_collision = 1:
+ * SMPLSIM_EUNSUPPORTED.  SMPLSIM_EINVAL: a null required input, n < 0, nsite < 0 or > 64, a bad site body index, a site quaternion
+ * whose norm is off by more than 1e-3, nsite > 0 with every site output NULL, a site output with nsite == 0, or every output NULL with
+ * n > 0; n == 0 reads nothing.  No per-env state is read or written (a later smplsim_step is unaffected); a row with non-finite inputs
+ * gets unspecified values in that row only.
+ * [MJ-upstream] mj_rnePostConstraint (engine_core_smooth.c), mj_computeSensorAcc (engine_sensor.c); not checked against a MuJoCo wheel. */
+int smplsim_rne_post(SmplsimHandle* h, const float* qpos_dev, const float* qvel_dev, const float* qacc_dev, const float* xfrc_applied_dev,
+                     int n, float* body_acc_dev, float* joint_wrench_dev, const int32_t* site_body, const float* site_pos,
+                     const float* site_quat, int nsite, float* accelerometer_dev, float* gyro_dev, float* force_dev, float* torque_dev,
+                     void* cuda_stream);
 
 /* Ray casting and camera images of the robot geoms and the floor, on caller body poses xpos[n,nbody,3] / xquat[n,nbody,4] (the
  * layout of SmplsimAux.xpos / xquat: the post-step poses a batch holds, smplsim_kinematics of any qpos, or motion-table rows).

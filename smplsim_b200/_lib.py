@@ -32,7 +32,8 @@ def build(force: bool = False, verbose: bool = False) -> str:
         cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", SO_PATH, os.path.join(_CSRC, "smplsim_capi.cu"),
                                                                                os.path.join(_CSRC, "rollout_kernels.cu"),
                                                                                os.path.join(_CSRC, "inverse_fd_kernels.cu"),
-                                                                               os.path.join(_CSRC, "centroidal_kernels.cu")]
+                                                                               os.path.join(_CSRC, "centroidal_kernels.cu"),
+                                                                               os.path.join(_CSRC, "rne_post_kernels.cu")]
         subprocess.check_call(cmd, cwd=_CSRC)
     return SO_PATH
 
@@ -54,6 +55,8 @@ _SYMBOLS = {
     "smplsim_dynamics": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "smplsim_centroidal": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                     C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "smplsim_rne_post": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                  C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "smplsim_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_void_p, C.c_void_p]),
     "smplsim_transition_fd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,

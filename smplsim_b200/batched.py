@@ -631,6 +631,80 @@ class HumanoidBatchB200:
             self.gpu_launches += 1
         return out
 
+    RNE_POST_MAX_SITES = 64
+
+    def _imu_sites(self, imu_sites):
+        """(site_body int32 [k], site_pos float32 [k, 3], site_quat float32 [k, 4]) of ``rne_post``'s ``imu_sites``."""
+        m = self.model
+        if isinstance(imu_sites, str):
+            if imu_sites != "bodies":
+                raise ValueError(f"imu_sites must be 'bodies' or a sequence of (body, pos, quat), got {imu_sites!r}")
+            imu_sites = [(b, (0.0, 0.0, 0.0), (1.0, 0.0, 0.0, 0.0)) for b in range(m.nbody)]
+        sites = list(imu_sites)
+        if len(sites) > self.RNE_POST_MAX_SITES:
+            raise ValueError(f"at most {self.RNE_POST_MAX_SITES} imu_sites, got {len(sites)}")
+        sb, sp, sq = [], [], []
+        for s in sites:
+            if not isinstance(s, (tuple, list)) or len(s) != 3:
+                raise ValueError(f"imu_sites entries must be (body name or index, pos[3], quat[4]), got {s!r}")
+            b, p, q = s
+            if isinstance(b, str):
+                if b not in m.body_names:
+                    raise ValueError(f"unknown body name {b!r}")
+                b = list(m.body_names).index(b)
+            if isinstance(b, bool) or not isinstance(b, (int, np.integer)) or not 0 <= int(b) < m.nbody:
+                raise ValueError(f"imu_sites bodies must be body names or indices in [0, {m.nbody}), got {b!r}")
+            p, q = np.asarray(p, dtype=np.float64), np.asarray(q, dtype=np.float64)
+            if p.shape != (3,) or not np.all(np.isfinite(p)):
+                raise ValueError(f"imu_sites pos must be 3 finite numbers, got {s[1]!r}")
+            if q.shape != (4,) or not abs(float(np.linalg.norm(q)) - 1.0) <= 1e-3:
+                raise ValueError(f"imu_sites quat must be a unit quaternion (w, x, y, z), got {s[2]!r}")
+            sb.append(int(b)); sp.append(p); sq.append(q)
+        return (np.ascontiguousarray(np.asarray(sb, dtype=np.int32)), np.ascontiguousarray(np.asarray(sp, dtype=np.float32).reshape(-1, 3)),
+                np.ascontiguousarray(np.asarray(sq, dtype=np.float32).reshape(-1, 4)))
+
+    def rne_post(self, qpos: torch.Tensor, qvel: torch.Tensor, qacc: torch.Tensor, *, acc: bool = True, joint_wrench: bool = True,
+                 imu_sites=None, xfrc_applied: Optional[torch.Tensor] = None):
+        """Body accelerations, joint reaction wrenches and IMU readings at caller rows ``(qpos, qvel, qacc)``, as MuJoCo's
+        ``mj_rnePostConstraint`` (``cacc``, ``cfrc_int``) and its acceleration-stage sensors.  Returns a dict with the outputs asked for
+        (world frame, robot body order):
+
+        - ``body_acc`` ``[n, nbody, 6]`` (``acc``): the linear acceleration of each body origin (``xpos``; gravity not included), then
+          its angular acceleration;
+        - ``joint_wrench`` ``[n, nbody, 6]`` (``joint_wrench``): the force, then the torque about the body origin, that body b's parent
+          (the world, for the root) applies to b's subtree through b's joint -- the joint's reaction load, joint-limit forces included;
+        - ``accelerometer`` / ``gyro`` / ``force`` / ``torque`` ``[n, k, 3]`` (``imu_sites``): per site, in the site frame, the proper
+          acceleration ``R^T (a - g)`` (``+|g|`` upward at rest, zero in free fall), the angular velocity, and the joint wrench of the
+          site's body moved to the site (MuJoCo's sensors of those names).  ``imu_sites`` is a sequence of at most 64
+          ``(body name or index, pos[3], quat[4])``, position and unit quaternion (w, x, y, z) in the body frame, or ``"bodies"``: one
+          site at every body frame.
+
+        The floor-contact and joint-limit forces are ``inverse``'s at the same rows; ``xfrc_applied`` (``[n, nbody, 6]``, the
+        convention of ``self.xfrc_applied``; None: none) acts on the bodies as well.  Float32 tensors on this batch's device; any n on a
+        one-shape batch without per-env parameters, n == num_envs otherwise (row i uses env i's shape, gravity and mass scales).  Reads no
+        env state and changes none.  Not available with ``cfg.env.self_collision``."""
+        m = self.model
+        q, v, a = self._rows((("qpos", qpos, m.nq), ("qvel", qvel, m.nv), ("qacc", qacc, m.nv)))
+        n, f32 = q.shape[0], dict(dtype=torch.float32, device=self.device)
+        xf = None if xfrc_applied is None else self._checked("xfrc_applied", xfrc_applied, (n, m.nbody, 6))
+        sb, sp, sq = self._imu_sites(imu_sites) if imu_sites is not None else (None, None, None)
+        ns = 0 if sb is None else len(sb)
+        out = {}
+        if acc:
+            out["body_acc"] = torch.empty(n, m.nbody, 6, **f32)
+        if joint_wrench:
+            out["joint_wrench"] = torch.empty(n, m.nbody, 6, **f32)
+        if ns:
+            for k in ("accelerometer", "gyro", "force", "torque"):
+                out[k] = torch.empty(n, ns, 3, **f32)
+        if out:
+            hp = (lambda x: C.c_void_p(x.ctypes.data) if ns else None)
+            self._check(self._L().smplsim_rne_post(self._h, _ptr(q), _ptr(v), _ptr(a), _ptr(xf), n, _ptr(out.get("body_acc")),
+                                                   _ptr(out.get("joint_wrench")), hp(sb), hp(sp), hp(sq), ns, _ptr(out.get("accelerometer")),
+                                                   _ptr(out.get("gyro")), _ptr(out.get("force")), _ptr(out.get("torque")), self._stream()))
+            self.gpu_launches += 1
+        return out
+
     # ------------------------------------------------------------------ ray casting and cameras (mj_ray, mujoco.Renderer)
     def _checked(self, name, t, shape):
         """A caller tensor checked as xfrc_applied is: shape (None entries free), float32, this batch's device, contiguous."""

@@ -3047,3 +3047,31 @@ struct LCentArgs {
 // there) hands the host code its instances, [0] plain, [1] with parameter records, of class 1 (SMPL) or 2 (SMPL-X), with or without
 // self-collision (nothing here depends on contacts).
 void lane_cent_kernels(int cls, int selfcol, void (*k[2])(const float*, int, LCentArgs));
+
+// ------------------------------------------------------------------ body accelerations, joint wrenches, IMU sites (mj_rnePostConstraint, acceleration-stage sensors)
+// On caller rows (qpos, qvel, qacc; xfrc [n, nb, 6] NULL: none, SmplsimState.xfrc_applied's layout and convention), each output NULL:
+// skipped, world frame, robot body order:
+//   acc [n, nb, 6]     the classical acceleration of the body origin (d^2 xpos / dt^2, gravity not included), then the angular
+//                      acceleration: J_b qacc + Jdot_b qvel in the row order of smplsim_dynamics' jac;
+//   jw [n, nb, 6]      F_b, the wrench body b's parent (the world, for the root) applies to b's subtree through b's joint (MuJoCo's
+//                      cfrc_int): force, then torque about the body origin.  It is the subtree's net inertial wrench (gravity and the
+//                      velocity products included) minus the floor-contact row forces of inverse dynamics and xfrc on the subtree;
+//                      joint-limit forces act between parent and child and so appear only inside it;
+//   accel / gyro / force / torque [n, nsite, 3]  nsite IMU sites, site s on body sb[s] at spos[s] (body frame) with orientation
+//                      squat[s] (wxyz, body frame; normalised here): R_s^T (a_site - g), R_s^T w_b, and F_b moved to the site point in
+//                      the site frame (MuJoCo's accelerometer, gyro, force and torque sensors); g is the env's gravity.
+// The row forces are those of smplsim_inverse at (qpos, qvel, qacc).  Uses the handle's per-env scratch of the rows it runs (lane records,
+// overflow contact entries, and gf [num_envs, 6 nb], the rollout's step-boundary scratch); writes neither the working-set memory nor the
+// sensor rows, so the stepper cannot tell that it ran.
+#define LRNEP_MAXS 64
+struct LRnepArgs {
+  const float* qpos; const float* qvel; const float* qacc; const float* xfrc;
+  float* acc; float* jw; float* accel; float* gyro; float* force; float* torque;
+  float* gscr; float* gf; LMap map; int n, nsite;
+  unsigned char sb[LRNEP_MAXS]; float spos[3 * LRNEP_MAXS]; float squat[4 * LRNEP_MAXS];
+};
+
+// k_rnep5<C> is defined and instantiated in rne_post_kernels.cu, a translation unit of its own as k_cent5 is.  lane_rnep_kernels (also
+// there) hands the host code its instances, [0] plain, [1] with parameter records, of class 1 (SMPL) or 2 (SMPL-X), without
+// self-collision (the inverse's pass builds no geom-geom rows).
+void lane_rnep_kernels(int cls, void (*k[2])(const float*, int, LRnepArgs));

@@ -93,6 +93,7 @@ struct LaneKernels {
   void (*roll[2])(const float*, int, LRollArgs);                        // [parameter records]
   void (*invfd)(const float*, int, LInvFdArgs);                         // single shape, no parameter records
   void (*cent[2])(const float*, int, LCentArgs);                        // [parameter records]
+  void (*rnep[2])(const float*, int, LRnepArgs);                        // [parameter records]
 };
 template <class C>
 static LaneKernels lane_kernels() {
@@ -105,6 +106,7 @@ static LaneKernels lane_kernels() {
   if constexpr (!C::SELFCOL) lane_roll_kernels(C::NB == L_SMPL(0)::NB ? 1 : 2, k.roll);   // a module of its own (rollout_kernels.cu)
   if constexpr (!C::SELFCOL) lane_invfd_kernels(C::NB == L_SMPL(0)::NB ? 1 : 2, &k.invfd);   // as roll (inverse_fd_kernels.cu)
   lane_cent_kernels(C::NB == L_SMPL(0)::NB ? 1 : 2, C::SELFCOL, k.cent);   // as roll (centroidal_kernels.cu); every class, as dyn
+  if constexpr (!C::SELFCOL) lane_rnep_kernels(C::NB == L_SMPL(0)::NB ? 1 : 2, k.rnep);   // as roll (rne_post_kernels.cu); as inverse
   return k;
 }
 
@@ -134,7 +136,7 @@ static int pick_wpb(SmplsimHandle* h) {
   };
   const LaneKernels K = lane_kernels<C>();
   if (!raise(K.step[0], K.step[1], K.step[2], K.reset[0], K.reset[1], K.kin, K.inverse[0], K.inverse[1], K.dyn[0], K.dyn[1], K.fwd[0], K.fwd[1],
-             K.roll[0], K.roll[1], K.invfd, K.cent[0], K.cent[1])) return -1;
+             K.roll[0], K.roll[1], K.invfd, K.cent[0], K.cent[1], K.rnep[0], K.rnep[1])) return -1;
   return best;
 }
 
@@ -475,6 +477,54 @@ extern "C" int smplsim_centroidal(SmplsimHandle* h, const float* qpos_dev, const
     if (c.jac) c.jac += r * c.njac * 3 * nv;
   };
   L_DISPATCH(h, state_rows<C_>(h, lane_kernels<C_>().cent, a, advance, (cudaStream_t)stream));
+  CUDA_TRY(cudaGetLastError());
+  return SMPLSIM_OK;
+}
+
+extern "C" int smplsim_rne_post(SmplsimHandle* h, const float* qpos_dev, const float* qvel_dev, const float* qacc_dev, const float* xfrc_applied_dev,
+                                int n, float* body_acc_dev, float* joint_wrench_dev, const int32_t* site_body, const float* site_pos,
+                                const float* site_quat, int nsite, float* accelerometer_dev, float* gyro_dev, float* force_dev, float* torque_dev,
+                                void* stream) {
+  if (!h || n < 0 || nsite < 0) return fail(SMPLSIM_EINVAL, "smplsim_rne_post: null handle, n < 0 or nsite < 0");
+  if (h->selfcol)
+    return fail(SMPLSIM_EUNSUPPORTED, "smplsim_rne_post: the inverse's pass does not build geom-geom contacts (handle created with self_collision = 1)");
+  const LHdr& H = *h->img.hdr();
+  if (nsite > LRNEP_MAXS) return fail(SMPLSIM_EINVAL, "smplsim_rne_post: nsite > 64");
+  if (nsite > 0 && (!site_body || !site_pos || !site_quat))
+    return fail(SMPLSIM_EINVAL, "smplsim_rne_post: nsite > 0 needs site_body, site_pos and site_quat");
+  for (int s = 0; s < nsite; s++) {
+    if (site_body[s] < 0 || site_body[s] >= H.nb) return fail(SMPLSIM_EINVAL, "smplsim_rne_post: site_body entry out of range [0, nbody)");
+    const float* q = site_quat + 4 * s;
+    const double nq = std::sqrt((double)q[0] * q[0] + (double)q[1] * q[1] + (double)q[2] * q[2] + (double)q[3] * q[3]);
+    if (!(std::fabs(nq - 1.0) <= 1e-3)) return fail(SMPLSIM_EINVAL, "smplsim_rne_post: site_quat entry is not a unit quaternion (|norm - 1| > 1e-3)");
+  }
+  if (n == 0) return SMPLSIM_OK;   // nothing is read: empty tensors may come as NULL
+  const bool site_out = accelerometer_dev || gyro_dev || force_dev || torque_dev;
+  if (nsite > 0 && !site_out) return fail(SMPLSIM_EINVAL, "smplsim_rne_post: nsite > 0 needs a site output");
+  if (nsite == 0 && site_out) return fail(SMPLSIM_EINVAL, "smplsim_rne_post: a site output needs nsite > 0");
+  if (!body_acc_dev && !joint_wrench_dev && !site_out) return fail(SMPLSIM_EINVAL, "smplsim_rne_post: no output requested");
+  if (!qpos_dev || !qvel_dev || !qacc_dev) return fail(SMPLSIM_EINVAL, "smplsim_rne_post: null qpos, qvel or qacc");
+  if (int rc = env_rows(h, n, "smplsim_rne_post", true)) return rc;
+  DeviceGuard guard(h->device);
+  LRnepArgs a; std::memset(&a, 0, sizeof a);
+  a.qpos = qpos_dev; a.qvel = qvel_dev; a.qacc = qacc_dev; a.xfrc = xfrc_applied_dev; a.acc = body_acc_dev; a.jw = joint_wrench_dev;
+  a.accel = accelerometer_dev; a.gyro = gyro_dev; a.force = force_dev; a.torque = torque_dev;
+  a.gscr = h->gscr; a.gf = h->groll; a.map = h->map(); a.n = n; a.nsite = nsite;
+  for (int s = 0; s < nsite; s++) {
+    a.sb[s] = (unsigned char)site_body[s];
+    for (int j = 0; j < 3; j++) a.spos[3 * s + j] = site_pos[3 * s + j];
+    for (int j = 0; j < 4; j++) a.squat[4 * s + j] = site_quat[4 * s + j];
+  }
+  const size_t nv = H.nv, nb = H.nb, ns = nsite;
+  auto advance = [nv, nb, ns](LRnepArgs& c, size_t r) {
+    c.qpos += r * (nv + 1); c.qvel += r * nv; c.qacc += r * nv;
+    if (c.xfrc) c.xfrc += r * nb * 6;
+    if (c.acc) c.acc += r * nb * 6;
+    if (c.jw) c.jw += r * nb * 6;
+    for (float** p : {&c.accel, &c.gyro, &c.force, &c.torque})
+      if (*p) *p += r * ns * 3;
+  };
+  L_DISPATCH(h, state_rows<C_>(h, lane_kernels<C_>().rnep, a, advance, (cudaStream_t)stream));
   CUDA_TRY(cudaGetLastError());
   return SMPLSIM_OK;
 }
@@ -1072,4 +1122,5 @@ extern "C" int smplsim_debug_stats(int* out, int reset) {   // out: L_NSTATS cou
 #include "rollout_kernels.cu"   // the device build compiles it as a translation unit of its own (_lib.build)
 #include "inverse_fd_kernels.cu"   // as rollout_kernels.cu
 #include "centroidal_kernels.cu"   // as rollout_kernels.cu
+#include "rne_post_kernels.cu"   // as rollout_kernels.cu
 #endif

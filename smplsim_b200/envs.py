@@ -153,6 +153,18 @@ def mj_jacSubtreeCom(model, data, jacp, body):
     jacp.reshape(jac.size)[:] = jac.ravel()
 
 
+def mj_rnePostConstraint(model, data):
+    """``mujoco.mj_rnePostConstraint`` for an env's ``mj_data``: fills ``data.cacc``, ``data.cfrc_int`` and ``data.cfrc_ext``
+    [nbody + 1, 6] in MuJoCo's layout (MuJoCo body order, world row first; rotation first; com-based, i.e. about the root subtree's
+    centre of mass ``subtree_com[0]``): each body's spatial acceleration with the ``-g`` offset MuJoCo carries (the world row is
+    ``[0 ; -g]``), the wrench its parent applies through its joint, and the external wrench on it (contact forces plus
+    ``xfrc_applied``).  Evaluated at the last forward pass (``qpos_fwd``, ``qvel_fwd``, ``data.qacc``) with the env's
+    ``xfrc_applied``; fp32 on the GPU (``HumanoidBatchB200.rne_post``), converted on the host.  ``model`` is accepted for the signature
+    and not read."""
+    r = data._rnep_fn()
+    data.cacc, data.cfrc_int, data.cfrc_ext = r["cacc"], r["cfrc_int"], r["cfrc_ext"]
+
+
 class _MjData(SimpleNamespace):
     """``mj_data`` view.  ``qM`` / ``qfrc_bias`` and ``subtree_com`` cost a kernel call, so they are evaluated on first read."""
 
@@ -306,7 +318,7 @@ class HumanoidEnvB200(_EnvBase):
         sens = np.concatenate([b.body_linvel[0].cpu().numpy().ravel(), b.body_angvel[0].cpu().numpy().ravel()])
         z3, z4 = np.zeros((1, 3)), np.array([[1.0, 0, 0, 0]])
         return _MjData(_dyn_fn=self._fwd_dynamics, _fd_fn=self._transition_fd, _rollout_fn=self._rollout, _invfd_fn=self._inverse_fd,
-                               _cent_fn=self._centroidal, _jac_com_fn=self._jac_com, qpos=b.qpos[0].cpu().numpy().astype(np.float64), qvel=b.qvel[0].cpu().numpy().astype(np.float64),
+                               _cent_fn=self._centroidal, _jac_com_fn=self._jac_com, _rnep_fn=self._rne_post, qpos=b.qpos[0].cpu().numpy().astype(np.float64), qvel=b.qvel[0].cpu().numpy().astype(np.float64),
                                ctrl=b.ctrl[0].cpu().numpy().astype(np.float64), qacc=b.qacc[0].cpu().numpy().astype(np.float64),
                                xpos=np.concatenate([z3, b.xpos[0].cpu().numpy()]), xquat=np.concatenate([z4, b.xquat[0].cpu().numpy()]),
                                sensordata=sens, contact=_Contacts(int(b.contact_mask[0].item())),
@@ -346,6 +358,36 @@ class HumanoidEnvB200(_EnvBase):
         b = self._b
         out = b.centroidal(b.qpos_fwd, None, com=False, velocity=False, cmm=False, jac_com_bodies=[body])
         return out["jac_com"][0, 0].cpu().numpy().astype(np.float64)
+
+    def _rne_post(self):
+        """cacc, cfrc_int, cfrc_ext [nbody + 1, 6] (MuJoCo's com-based layout, world row first) at the last forward pass (fp64)."""
+        b = self._b
+        m = b.model
+        q, v, a = b.qpos_fwd, b.qvel_fwd, b.qacc
+        xf = torch.as_tensor(self._xfrc_applied[1:], dtype=torch.float32, device=b.device)[None].contiguous()
+        out = b.rne_post(q, v, a, xfrc_applied=xf)
+        jac = b.dynamics(q, None, mass_matrix=False, bias=False, jac_bodies=list(range(m.nbody)))
+        J = torch.cat([jac["jacp"], jac["jacr"]], 2)[0].cpu().numpy().astype(np.float64)
+        vel = J @ v[0].cpu().numpy().astype(np.float64)                 # [nb, 6]: origin velocity, angular velocity
+        c = b.centroidal(q, None, velocity=False, cmm=False)["subtree_com"][0, 0].cpu().numpy().astype(np.float64)
+        xpos, xquat = (x[0].cpu().numpy().astype(np.float64) for x in b.kinematics(q))
+        cw = b.inverse(q, v, a, contact_wrench=True)[1][0].cpu().numpy().astype(np.float64)
+        g = b.env_params["gravity"][0].cpu().numpy().astype(np.float64)
+        acc, jw = (out[k][0].cpu().numpy().astype(np.float64) for k in ("body_acc", "joint_wrench"))
+        w, x, y, z = xquat.T / np.linalg.norm(xquat, axis=1)
+        R = np.stack([np.stack([1 - 2 * (y * y + z * z), 2 * (x * y - w * z), 2 * (x * z + w * y)], -1),
+                      np.stack([2 * (x * y + w * z), 1 - 2 * (x * x + z * z), 2 * (y * z - w * x)], -1),
+                      np.stack([2 * (x * z - w * y), 2 * (y * z + w * x), 1 - 2 * (x * x + y * y)], -1)], 1)
+        xipos = xpos + np.einsum("bij,bj->bi", R, np.asarray(m.body_ipos, dtype=np.float64))
+        wb, wd = vel[:, 3:], acc[:, 3:]
+        # spatial acceleration about the fixed point c: classical acceleration of the body origin + wd x (c - x) - w x v_origin
+        lin = acc[:, :3] + np.cross(wd, c - xpos) - np.cross(wb, vel[:, :3]) - g
+        f_ext = cw[:, :3] + xf[0, :, :3].cpu().numpy().astype(np.float64)
+        t_ext = cw[:, 3:] + xf[0, :, 3:].cpu().numpy().astype(np.float64) + np.cross(xipos - c, f_ext)
+        world = np.zeros((1, 6))
+        return {"cacc": np.concatenate([np.concatenate([[0.0, 0.0, 0.0], -g])[None], np.concatenate([wd, lin], 1)]),
+                "cfrc_int": np.concatenate([world, np.concatenate([jw[:, 3:] + np.cross(xpos - c, jw[:, :3]), jw[:, :3]], 1)]),
+                "cfrc_ext": np.concatenate([world, np.concatenate([t_ext, f_ext], 1)])}
 
     def _fd_row(self, fd, x, eps, **kw):
         """The batch's ``fd`` (``transition_fd`` / ``inverse_fd``) at one state ``x`` (fp32 rows), eps (None: the defaults); fp64 outputs."""

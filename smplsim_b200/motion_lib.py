@@ -246,14 +246,24 @@ class MotionLibB200:
         nbody, 6]``), indexed like the tables.  ``qfrc_inverse[:, 0:6]`` is the root residual force of each frame.  ``qacc`` is the
         forward difference of ``qvel`` over the clip's ``motion_dt``; a clip's last frame repeats its previous difference (a one-frame clip
         gets zero), so nothing is differenced across clips."""
-        qpos, qvel = self.tables["qpos"], self.tables["qvel"]
+        return self.env.inverse(self.tables["qpos"], self.tables["qvel"], self._frame_qacc(), contact_wrench=contact_wrench)
+
+    def _frame_qacc(self):
+        """qacc of every frame: the forward difference of ``qvel`` over the clip's ``motion_dt``; a clip's last frame repeats its
+        previous difference (a one-frame clip gets zero), so nothing is differenced across clips."""
+        qvel = self.tables["qvel"]
         idx = torch.arange(qvel.shape[0], device=qvel.device)
         clip = torch.searchsorted(self.length_starts.long(), idx, right=True) - 1
         start, last = self.length_starts.long()[clip], (self.length_starts.long() + self._motion_num_frames.long() - 1)[clip]
         hi = torch.where(idx < last, idx + 1, idx)
         lo = torch.maximum(hi - 1, start)
-        qacc = (qvel[hi] - qvel[lo]) / self._motion_dt[clip][:, None]
-        return self.env.inverse(qpos, qvel, qacc, contact_wrench=contact_wrench)
+        return (qvel[hi] - qvel[lo]) / self._motion_dt[clip][:, None]
+
+    def rne_post(self, **kw):
+        """``env.rne_post`` over every frame of the library, at the frames' ``qpos`` / ``qvel`` and the ``qacc`` that
+        ``inverse_dynamics`` uses: body accelerations, joint reaction wrenches and IMU readings, indexed like the tables.  Keywords go to
+        ``rne_post`` (``acc``, ``joint_wrench``, ``imu_sites``, ``xfrc_applied``)."""
+        return self.env.rne_post(self.tables["qpos"], self.tables["qvel"], self._frame_qacc(), **kw)
 
     def centroidal(self, **kw):
         """``env.centroidal`` over every frame of the library: subtree centres of mass, their velocities, angular momenta, the
