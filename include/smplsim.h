@@ -190,7 +190,7 @@ typedef struct SmplsimHandle SmplsimHandle;
 const char* smplsim_last_error(void);
 int smplsim_version(void);   /* 300 = this header (290: before smplsim_track_eval; 280: before smplsim_motion_blend and the interpolation / future-target fields; 270: before smplsim_amp_obs / smplsim_amp_demo; 260: before smplsim_imitation; 250: before smplsim_set_env_params; 240: before smplsim_ray / smplsim_render; 230: before smplsim_dynamics; 220: before smplsim_inverse;
                               * 210: before SmplsimAux.contact_wrench; 200: before SmplsimState.xfrc_applied; 100: before pid_* state and aux.status).
-                              * smplsim_forward, smplsim_transition_fd, smplsim_rollout, smplsim_inverse_fd, smplsim_centroidal and smplsim_rne_post came later without a new number, because callers
+                              * smplsim_forward, smplsim_transition_fd, smplsim_rollout, smplsim_inverse_fd, smplsim_centroidal, smplsim_rne_post and smplsim_rollout_feedback came later without a new number, because callers
                               * compare it to 300 for equality: look them up by symbol (dlsym) rather than by version. */
 
 /* MjModel.from_xml_string + MjData + setup_humanoid_properties/setup_controller
@@ -341,6 +341,29 @@ int smplsim_inverse_fd(SmplsimHandle* h, const SmplsimInverseFdCfg* cfg, const f
 int smplsim_rollout(SmplsimHandle* h, int mode, int nsub, const float* qpos0_dev, const float* qvel0_dev, const float* qacc_warmstart_dev,
                     const float* qpos_fwd0_dev, const float* qvel_fwd0_dev, const float* control_dev, int n, int nstep, float* qpos_dev,
                     float* qvel_dev, uint8_t* status_dev, float* xpos_dev, float* xquat_dev, void* cuda_stream);
+
+/* Closed-loop rollouts: smplsim_rollout with time-varying linear state feedback applied inside the launch (an iLQR / DDP forward pass,
+ * time-varying LQR tracking, a linear feedback policy).  Row i's control at step t (0 <= t < nstep) is
+ *   u_t = ubar_t + K_t dx_t,   dx_t = x_t (-) xbar_t = [dq ; qvel_t - qvel_ref_t]   (length 2 nv)
+ * with ubar_t = control[i,t], K_t = gain[r,t] ([nu, 2nv] row-major), xbar_t = (qpos_ref[r,t], qvel_ref[r,t]), r = 0 when ref_rows == 1
+ * (one schedule shared by every row) and r = i when ref_rows == n.  x_t is the state before step t: the start state for t = 0, else
+ * exactly the output row t - 1 (after the root-quaternion normalisation and after an auto-reset).  dq is the tangent of transition_fd's
+ * A and B (mju_subQuat for the root rotation, in the reference's body frame):
+ *   dq[0:3] = q[0:3] - qbar[0:3];  dq[6:] = q[7:] - qbar[7:];
+ *   dq[3:6] = log(r), r = normalise(qbar[3:7])^-1 (x) normalise(q[3:7]) flipped to r_w >= 0 (the shortest arc),
+ *             log(r) = 2 atan2(|r_xyz|, r_w) r_xyz / |r_xyz|, and 0 when |r_xyz| = 0.
+ * A state equal to its reference bit for bit gives dx = 0 exactly (the terms that cancel in r_xyz are rounded products), so a row with
+ * x_t == xbar_t applies ubar_t exactly.  SMPLSIM_ROLLOUT_ACTION with clip_actions != 0 clamps u_t to [-1, 1] (cfg.env.clip_actions, as
+ * the caller of smplsim_step does); a NaN passes unclamped and takes the row through the auto-reset and status path.  Ctrl mode does not
+ * clamp.  Step t then runs exactly as smplsim_rollout's step t on control row u_t.  Inputs gain[ref_rows,nstep,nu,2nv],
+ * qpos_ref[ref_rows,nstep,nq], qvel_ref[ref_rows,nstep,nv] required; control_applied[n,nstep,nu], the u_t each step used, NULL: not
+ * written (replaying those rows through smplsim_rollout gives every output bit for bit).  Every other argument, the row rules and the
+ * unsupported cases are smplsim_rollout's.  SMPLSIM_EINVAL as smplsim_rollout, and for a null gain or reference or ref_rows not 1 or n. */
+int smplsim_rollout_feedback(SmplsimHandle* h, int mode, int nsub, const float* qpos0_dev, const float* qvel0_dev,
+                             const float* qacc_warmstart_dev, const float* qpos_fwd0_dev, const float* qvel_fwd0_dev, const float* control_dev,
+                             int n, int nstep, float* qpos_dev, float* qvel_dev, uint8_t* status_dev, float* xpos_dev, float* xquat_dev,
+                             const float* gain_dev, const float* qpos_ref_dev, const float* qvel_ref_dev, int ref_rows, int clip_actions,
+                             float* control_applied_dev, void* cuda_stream);
 
 /* Mass matrix, bias forces and body Jacobians on n caller rows qpos[n,nq], qvel[n,nv] (each output NULL: skipped):
  *   qM[n,nv,nv]          mujoco.mj_fullM(qM): the dense joint-space inertia, armature on the diagonal; exactly symmetric, exact zeros

@@ -31,6 +31,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
         cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", SO_PATH, os.path.join(_CSRC, "smplsim_capi.cu"),
                                                                                os.path.join(_CSRC, "rollout_kernels.cu"),
+                                                                               os.path.join(_CSRC, "rollout_feedback_kernels.cu"),
                                                                                os.path.join(_CSRC, "inverse_fd_kernels.cu"),
                                                                                os.path.join(_CSRC, "centroidal_kernels.cu"),
                                                                                os.path.join(_CSRC, "rne_post_kernels.cu")]
@@ -65,6 +66,9 @@ _SYMBOLS = {
                                     C.c_void_p]),
     "smplsim_rollout": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                  C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "smplsim_rollout_feedback": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "smplsim_ray": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
                              C.c_void_p, C.c_void_p]),
     "smplsim_render": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p,

@@ -469,7 +469,8 @@ class HumanoidBatchB200:
 
     def rollout(self, qpos: torch.Tensor, qvel: torch.Tensor, control: torch.Tensor, *, mode: str = "action", nsub: Optional[int] = None,
                 qacc_warmstart: Optional[torch.Tensor] = None, qpos_fwd: Optional[torch.Tensor] = None, qvel_fwd: Optional[torch.Tensor] = None,
-                body_poses: bool = False, status: bool = True):
+                body_poses: bool = False, status: bool = True, gains: Optional[torch.Tensor] = None, qpos_ref: Optional[torch.Tensor] = None,
+                qvel_ref: Optional[torch.Tensor] = None):
         """Roll ``n`` control sequences forward from caller start states in one kernel launch, as ``mujoco.rollout.rollout``.  Row ``i``
         starts at ``(qpos[i], qvel[i])`` and takes one step per control row ``control[i, t]`` (``control`` is ``[n, T, nu]``):
 
@@ -491,8 +492,20 @@ class HumanoidBatchB200:
         poses of ``self.xpos`` / ``self.xquat``; asking for them changes no bit of the trajectory).  Float32 tensors on this batch's
         device; any n on a one-shape batch without per-env parameters, n == num_envs otherwise (row i uses env i's shape and
         parameters).  Reads no env state and changes none; ``xfrc_applied`` is not taken.  Not available with
-        ``cfg.env.self_collision``."""
+        ``cfg.env.self_collision``.
+
+        Closed loop (``gains`` given; ``qpos_ref`` and ``qvel_ref`` then required): ``control`` is the feedforward ``ubar`` and step ``t``
+        applies ``u_t = ubar_t + K_t dx_t`` with ``K_t = gains[r, t]`` (``[nu, 2 nv]``), ``dx_t = differentiate_pos(qpos_ref[r, t], q_t)``
+        stacked on ``qvel_t - qvel_ref[r, t]``, where ``(q_t, qvel_t)`` is the state before step ``t`` (the start state, then the output row
+        ``t - 1``) and ``r`` is 0 when the leading dimension of ``gains`` / ``qpos_ref`` / ``qvel_ref`` is 1 (one schedule for every row)
+        or the row when it is ``n``.  ``dx`` is the tangent of ``transition_fd``'s ``A`` and ``B`` (root rotation in the reference's body
+        frame, on the shortest arc) and is exactly 0 for a state equal to its reference.  In ``mode="action"`` ``u_t`` is clamped to
+        [-1, 1] with ``cfg.env.clip_actions`` (a NaN passes, as ``torch.clamp`` lets it, and resets the row); ctrl mode does not clamp.
+        All of it runs in the one launch (an iLQR forward pass with its line-search steps as rows, TVLQR tracking from many starts).
+        The result adds ``control [n, T, nu]``, the ``u_t`` each step applied: ``rollout`` on those rows replays the run bit for bit."""
         m = self.model
+        if gains is None and (qpos_ref is not None or qvel_ref is not None):
+            raise ValueError("qpos_ref / qvel_ref are the reference of the feedback law: give gains with them")
         if mode not in self.ROLLOUT_MODES:
             raise ValueError(f"mode must be 'action' or 'ctrl', got {mode!r}")
         if mode == "action":
@@ -512,7 +525,17 @@ class HumanoidBatchB200:
         T = u.shape[1]
         if T < 1:
             raise ValueError("control must hold at least one step ([n, T, nu] with T >= 1)")
-        if mode == "action" and bool(self.cfg.env.clip_actions):
+        if gains is not None:
+            if qpos_ref is None or qvel_ref is None:
+                raise ValueError("gains need qpos_ref and qvel_ref (the reference state of the feedback law)")
+            nx = 2 * m.nv
+            K = self._checked("gains", gains.contiguous() if isinstance(gains, torch.Tensor) else gains, (None, T, m.nu, nx))
+            r = K.shape[0]
+            if r not in (1, n):
+                raise ValueError(f"gains, qpos_ref and qvel_ref must have leading dimension 1 (shared) or n = {n}, got {r}")
+            qr = self._checked("qpos_ref", qpos_ref.contiguous() if isinstance(qpos_ref, torch.Tensor) else qpos_ref, (r, T, m.nq))
+            vr = self._checked("qvel_ref", qvel_ref.contiguous() if isinstance(qvel_ref, torch.Tensor) else qvel_ref, (r, T, m.nv))
+        elif mode == "action" and bool(self.cfg.env.clip_actions):
             u = torch.clamp(u, -1.0, 1.0)
         dv, f32 = self.device, dict(dtype=torch.float32, device=self.device)
         out = {"qpos": torch.empty(n, T, m.nq, **f32), "qvel": torch.empty(n, T, m.nv, **f32)}
@@ -521,12 +544,59 @@ class HumanoidBatchB200:
         if body_poses:
             out["xpos"] = torch.empty(n, T, m.nbody, 3, **f32)
             out["xquat"] = torch.empty(n, T, m.nbody, 4, **f32)
-        self._check(self._L().smplsim_rollout(self._h, self.ROLLOUT_MODES[mode], int(ns), _ptr(rows["qpos"]), _ptr(rows["qvel"]),
-                                              _ptr(rows.get("qacc_warmstart")), _ptr(rows.get("qpos_fwd")), _ptr(rows.get("qvel_fwd")), _ptr(u),
-                                              n, T, _ptr(out["qpos"]), _ptr(out["qvel"]), _ptr(out.get("status")), _ptr(out.get("xpos")),
-                                              _ptr(out.get("xquat")), self._stream()))
+        if gains is None:
+            self._check(self._L().smplsim_rollout(self._h, self.ROLLOUT_MODES[mode], int(ns), _ptr(rows["qpos"]), _ptr(rows["qvel"]),
+                                                  _ptr(rows.get("qacc_warmstart")), _ptr(rows.get("qpos_fwd")), _ptr(rows.get("qvel_fwd")), _ptr(u),
+                                                  n, T, _ptr(out["qpos"]), _ptr(out["qvel"]), _ptr(out.get("status")), _ptr(out.get("xpos")),
+                                                  _ptr(out.get("xquat")), self._stream()))
+        else:
+            out["control"] = torch.empty(n, T, m.nu, **f32)
+            self._check(self._L().smplsim_rollout_feedback(
+                self._h, self.ROLLOUT_MODES[mode], int(ns), _ptr(rows["qpos"]), _ptr(rows["qvel"]), _ptr(rows.get("qacc_warmstart")),
+                _ptr(rows.get("qpos_fwd")), _ptr(rows.get("qvel_fwd")), _ptr(u), n, T, _ptr(out["qpos"]), _ptr(out["qvel"]),
+                _ptr(out.get("status")), _ptr(out.get("xpos")), _ptr(out.get("xquat")), _ptr(K), _ptr(qr), _ptr(vr), r,
+                int(bool(self.cfg.env.clip_actions)), _ptr(out["control"]), self._stream()))
         self.gpu_launches += 1
         return out
+
+    def differentiate_pos(self, qpos_ref: torch.Tensor, qpos: torch.Tensor) -> torch.Tensor:
+        """``mj_differentiatePos(qpos_ref -> qpos)`` without the division by dt, batched over leading dimensions: ``[..., nq]`` pairs to
+        ``[..., nv]``.  The position part of the tangent of ``transition_fd``'s ``A`` / ``B`` and of ``rollout``'s feedback law: root
+        translation difference in the world frame, root rotation ``log(normalise(ref)^-1 * normalise(q))`` on the shortest arc (in the
+        reference's body frame), hinge differences.  Any float dtype (fp64 for a Riccati pass); on the inputs' device."""
+        qr, q = torch.broadcast_tensors(qpos_ref, qpos)
+        if q.shape[-1] != self.model.nq:
+            raise ValueError(f"qpos_ref / qpos must end in nq = {self.model.nq}, got {tuple(q.shape)}")
+        b = qr[..., 3:7] / torch.linalg.vector_norm(qr[..., 3:7], dim=-1, keepdim=True)
+        c = q[..., 3:7] / torch.linalg.vector_norm(q[..., 3:7], dim=-1, keepdim=True)
+        bw, bv, cw, cv = b[..., :1], b[..., 1:], c[..., :1], c[..., 1:]
+        rw = bw * cw + (bv * cv).sum(-1, keepdim=True)                      # conj(b) * c
+        rv = bw * cv - cw * bv - torch.linalg.cross(bv, cv)
+        sgn = torch.where(rw < 0, -1.0, 1.0).to(rw.dtype)
+        rw, rv = rw * sgn, rv * sgn
+        s = torch.linalg.vector_norm(rv, dim=-1, keepdim=True)
+        f = torch.where(s > 0, 2 * torch.atan2(s, rw) / torch.where(s > 0, s, torch.ones_like(s)), torch.zeros_like(s))
+        return torch.cat([q[..., 0:3] - qr[..., 0:3], f * rv, q[..., 7:] - qr[..., 7:]], dim=-1)
+
+    def integrate_pos(self, qpos: torch.Tensor, dq: torch.Tensor) -> torch.Tensor:
+        """``mj_integratePos(qpos, dq, 1)``, the inverse of ``differentiate_pos``: ``[..., nq]`` and ``[..., nv]`` to ``[..., nq]``, the
+        root rotation as ``q * exp(dq[3:6])`` (body frame), normalised.  Any float dtype; on the inputs' device."""
+        if qpos.shape[-1] != self.model.nq or dq.shape[-1] != self.model.nv:
+            raise ValueError(f"qpos must end in nq = {self.model.nq} and dq in nv = {self.model.nv}, got {tuple(qpos.shape)}, {tuple(dq.shape)}")
+        lead = torch.broadcast_shapes(qpos.shape[:-1], dq.shape[:-1])
+        qpos, dq = qpos.expand(lead + (self.model.nq,)), dq.expand(lead + (self.model.nv,))
+        w = dq[..., 3:6]
+        th = torch.linalg.vector_norm(w, dim=-1, keepdim=True)
+        half = 0.5 * th
+        k = torch.where(th > 0, torch.sin(half) / torch.where(th > 0, th, torch.ones_like(th)), torch.full_like(th, 0.5))
+        ew, ev = torch.cos(half), k * w                                     # exp(w) = (cos |w|/2, sin |w|/2 w / |w|)
+        a = qpos[..., 3:7]
+        aw, av = a[..., :1], a[..., 1:]
+        rw = aw * ew - (av * ev).sum(-1, keepdim=True)
+        rv = aw * ev + ew * av + torch.linalg.cross(av, ev)
+        r = torch.cat([rw, rv], dim=-1)
+        r = r / torch.linalg.vector_norm(r, dim=-1, keepdim=True)
+        return torch.cat([qpos[..., 0:3] + dq[..., 0:3], r, qpos[..., 7:] + dq[..., 6:]], dim=-1)
 
     def dynamics(self, qpos: torch.Tensor, qvel: Optional[torch.Tensor] = None, mass_matrix: bool = True, bias: bool = True,
                  jac_bodies: Optional[Sequence] = None):

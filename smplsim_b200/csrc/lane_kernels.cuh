@@ -3013,6 +3013,22 @@ struct LRollArgs {
 // (SMPL-X), without self-collision.
 void lane_roll_kernels(int cls, void (*k[2])(const float*, int, LRollArgs));
 
+// Closed-loop rollouts (smplsim_rollout_feedback): k_roll5's steps with the control row of step t computed in the launch,
+// u = control[row, t] + gain[rr, t] (x_t (-) ref[rr, t]) (rr = 0 with shared_ref, else the row; law in smplsim.h), clamped to [-1, 1]
+// when clip (action mode), then handed to l_roll_step as its control row.  u goes to control_applied[row, t], or to the per-env scratch
+// row uscr when that is NULL; dx (2nv floats) is staged in the per-env scratch row dx.  A struct of its own around r, so that k_roll5's
+// parameter layout stays as it is.
+struct LRollFbArgs {
+  LRollArgs r;   // r.control: the feedforward rows [n, nstep, nu]
+  const float* gain; const float* qpos_ref; const float* qvel_ref;   // [ref_rows, nstep, nu, 2nv | nq | nv]
+  float* control_applied;                                            // [n, nstep, nu]; NULL: not written
+  float* dx; float* uscr;                                            // per-env scratch rows [num_envs, 2nv | nu]
+  int shared_ref, clip;
+};
+// k_rollfb5<C> is defined and instantiated in rollout_feedback_kernels.cu, a device module of its own as k_roll5's is;
+// lane_rollfb_kernels (also there) hands the host code its instances as lane_roll_kernels does.
+void lane_rollfb_kernels(int cls, void (*k[2])(const float*, int, LRollFbArgs));
+
 // ------------------------------------------------------------------ finite-difference inverse-dynamics derivatives (mjd_inverseFD)
 // The column pass of k_fwd5 over x = [dq ; qvel ; qacc], ncol = 3nv, with k_inverse5's pass: column col of dfrc = d qfrc_inverse / dx
 // and its flags (L_FD_SOLVER: a pass dropped joint-limit rows or saw a non-finite value).  Not centered, differenced against the nominal

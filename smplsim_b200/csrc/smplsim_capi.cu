@@ -33,6 +33,7 @@ struct SmplsimHandle {
   float* gbody = nullptr;  // body pose / velocity of the current forward pass (self-collision narrow phase)
   float* gfd = nullptr;    // per-env qacc / qfrc of a column's first pass (smplsim_transition_fd, smplsim_inverse_fd; handles without self-collision)
   float* groll = nullptr;  // per-env qpos, qvel, qpos_fwd, qvel_fwd at a rollout's step boundary (smplsim_rollout; as gfd)
+  float* gfb = nullptr;    // per-env dx [2nv] and u [nu] of a closed-loop rollout step (smplsim_rollout_feedback; as gfd)
   int num_envs = 0, device = 0, nsm = 132, max_smem = 0;
   int cls = 0;             // 1 SMPL class, 2 SMPL-X class
   int selfcol = 0;         // cfg.env.self_collision: kernels with the geom-geom rows compiled in
@@ -91,6 +92,7 @@ struct LaneKernels {
   void (*dyn[2])(const float*, int, LDynArgs);                          // [parameter records]
   void (*fwd[2])(const float*, int, LFwdArgs);                          // [parameter records]
   void (*roll[2])(const float*, int, LRollArgs);                        // [parameter records]
+  void (*rollfb[2])(const float*, int, LRollFbArgs);                    // [parameter records]
   void (*invfd)(const float*, int, LInvFdArgs);                         // single shape, no parameter records
   void (*cent[2])(const float*, int, LCentArgs);                        // [parameter records]
   void (*rnep[2])(const float*, int, LRnepArgs);                        // [parameter records]
@@ -104,6 +106,7 @@ static LaneKernels lane_kernels() {
   k.dyn[0] = k_dyn5<C>; k.dyn[1] = k_dyn5<P>;
   if constexpr (!C::SELFCOL) { k.fwd[0] = k_fwd5<C>; k.fwd[1] = k_fwd5<P>; }   // as inverse: none for a self-collision class
   if constexpr (!C::SELFCOL) lane_roll_kernels(C::NB == L_SMPL(0)::NB ? 1 : 2, k.roll);   // a module of its own (rollout_kernels.cu)
+  if constexpr (!C::SELFCOL) lane_rollfb_kernels(C::NB == L_SMPL(0)::NB ? 1 : 2, k.rollfb);   // as roll (rollout_feedback_kernels.cu)
   if constexpr (!C::SELFCOL) lane_invfd_kernels(C::NB == L_SMPL(0)::NB ? 1 : 2, &k.invfd);   // as roll (inverse_fd_kernels.cu)
   lane_cent_kernels(C::NB == L_SMPL(0)::NB ? 1 : 2, C::SELFCOL, k.cent);   // as roll (centroidal_kernels.cu); every class, as dyn
   if constexpr (!C::SELFCOL) lane_rnep_kernels(C::NB == L_SMPL(0)::NB ? 1 : 2, k.rnep);   // as roll (rne_post_kernels.cu); as inverse
@@ -136,7 +139,7 @@ static int pick_wpb(SmplsimHandle* h) {
   };
   const LaneKernels K = lane_kernels<C>();
   if (!raise(K.step[0], K.step[1], K.step[2], K.reset[0], K.reset[1], K.kin, K.inverse[0], K.inverse[1], K.dyn[0], K.dyn[1], K.fwd[0], K.fwd[1],
-             K.roll[0], K.roll[1], K.invfd, K.cent[0], K.cent[1], K.rnep[0], K.rnep[1])) return -1;
+             K.roll[0], K.roll[1], K.rollfb[0], K.rollfb[1], K.invfd, K.cent[0], K.cent[1], K.rnep[0], K.rnep[1])) return -1;
   return best;
 }
 
@@ -149,14 +152,17 @@ static void lane_launch(const SmplsimHandle* h, K kern, int rows, cudaStream_t s
 // inverse / dynamics on n caller rows of state.  One shape without parameter records: launches of at most num_envs rows (the
 // handle's scratch rows), in order on the caller's stream, `advance` moving every row pointer of a chunk to its first row.  Otherwise
 // (env_rows holds n == num_envs) one launch, of the instance that reads the records while the handle has them (row i = env i).
+template <class A> static int& row_count(A& a) { return a.n; }
+static int& row_count(LRollFbArgs& a) { return a.r.n; }   // the rows of the closed-loop rollout are its rollout's
 template <class C, class A, class F>
 static void state_rows(const SmplsimHandle* h, void (*const kern[2])(const float*, int, A), const A& a, F advance, cudaStream_t st) {
-  if (h->prm || h->nblocks) return lane_launch<C>(h, kern[h->prm ? 1 : 0], a.n, st, a);
-  for (int r0 = 0; r0 < a.n; r0 += h->num_envs) {
+  const int n = row_count(const_cast<A&>(a));
+  if (h->prm || h->nblocks) return lane_launch<C>(h, kern[h->prm ? 1 : 0], n, st, a);
+  for (int r0 = 0; r0 < n; r0 += h->num_envs) {
     A c = a;
-    c.n = std::min(h->num_envs, a.n - r0);
+    row_count(c) = std::min(h->num_envs, n - r0);
     advance(c, (size_t)r0);
-    lane_launch<C>(h, kern[0], c.n, st, c);
+    lane_launch<C>(h, kern[0], row_count(c), st, c);
   }
 }
 // dispatch over (model class, self-collision)
@@ -171,7 +177,7 @@ static void state_rows(const SmplsimHandle* h, void (*const kern[2])(const float
   } while (0)
 
 static void free_handle(SmplsimHandle* h) {
-  cudaFree(h->prm); cudaFree(h->dimg); cudaFree(h->gscr); cudaFree(h->gsens); cudaFree(h->gpfl); cudaFree(h->gbody); cudaFree(h->gfd); cudaFree(h->groll); cudaFree(h->dslot_env); cudaFree(h->dblk_img); cudaFree(h->denv_model);
+  cudaFree(h->prm); cudaFree(h->dimg); cudaFree(h->gscr); cudaFree(h->gsens); cudaFree(h->gpfl); cudaFree(h->gbody); cudaFree(h->gfd); cudaFree(h->groll); cudaFree(h->gfb); cudaFree(h->dslot_env); cudaFree(h->dblk_img); cudaFree(h->denv_model);
   delete h;
 }
 
@@ -268,6 +274,7 @@ static int create_impl(const SmplsimModelDesc* s, int nmodels, const int32_t* en
   if (e == cudaSuccess && cfg->self_collision) e = cudaMalloc(&h->gbody, (size_t)10 * H.nb * num_envs * 4);
   if (e == cudaSuccess && !cfg->self_collision) e = cudaMalloc(&h->gfd, (size_t)H.nv * num_envs * 4);
   if (e == cudaSuccess && !cfg->self_collision) e = cudaMalloc(&h->groll, (size_t)2 * (2 * H.nv + 1) * num_envs * 4);
+  if (e == cudaSuccess && !cfg->self_collision) e = cudaMalloc(&h->gfb, (size_t)(2 * H.nv + H.nu) * num_envs * 4);
   if (e != cudaSuccess) { free_handle(h); return fail(SMPLSIM_ECUDA, std::string("smplsim_create: ") + cudaGetErrorString(e)); }
   if (std::getenv("SMPLSIM_DEBUG"))
     fprintf(stderr, "smplsim_create: class %d, %d bodies, schedule %d steps, mailboxes %d in / %d out, %d geom pairs, table %d B, %zu B per env, %d warps per CTA, %zu B shared memory per CTA, self-collision %d\n",
@@ -624,41 +631,89 @@ extern "C" int smplsim_inverse_fd(SmplsimHandle* h, const SmplsimInverseFdCfg* c
   return fd_columns(h, a, n, [](const LaneKernels& k) { return k.invfd; }, (cudaStream_t)stream);
 }
 
-extern "C" int smplsim_rollout(SmplsimHandle* h, int mode, int nsub, const float* qpos0_dev, const float* qvel0_dev, const float* qacc_warmstart_dev,
-                               const float* qpos_fwd0_dev, const float* qvel_fwd0_dev, const float* control_dev, int n, int nstep,
-                               float* qpos_dev, float* qvel_dev, uint8_t* status_dev, float* xpos_dev, float* xquat_dev, void* stream) {
-  if (!h || n < 0 || nstep < 1) return fail(SMPLSIM_EINVAL, "smplsim_rollout: null handle, n < 0 or nstep < 1");
-  if (mode != SMPLSIM_ROLLOUT_ACTION && mode != SMPLSIM_ROLLOUT_CTRL) return fail(SMPLSIM_EINVAL, "smplsim_rollout: unknown mode");
-  if (mode == SMPLSIM_ROLLOUT_CTRL && nsub < 1) return fail(SMPLSIM_EINVAL, "smplsim_rollout: SMPLSIM_ROLLOUT_CTRL needs nsub >= 1");
+// the argument checks and row arguments of smplsim_rollout and smplsim_rollout_feedback (fn: the caller, for the error texts).
+// *empty: n == 0, nothing to launch.
+static int roll_args(SmplsimHandle* h, const char* fn, int mode, int nsub, const float* qpos0_dev, const float* qvel0_dev,
+                     const float* qacc_warmstart_dev, const float* qpos_fwd0_dev, const float* qvel_fwd0_dev, const float* control_dev, int n,
+                     int nstep, float* qpos_dev, float* qvel_dev, uint8_t* status_dev, float* xpos_dev, float* xquat_dev, LRollArgs& a, bool* empty) {
+  const std::string f(fn);
+  *empty = false;
+  if (!h || n < 0 || nstep < 1) return fail(SMPLSIM_EINVAL, f + ": null handle, n < 0 or nstep < 1");
+  if (mode != SMPLSIM_ROLLOUT_ACTION && mode != SMPLSIM_ROLLOUT_CTRL) return fail(SMPLSIM_EINVAL, f + ": unknown mode");
+  if (mode == SMPLSIM_ROLLOUT_CTRL && nsub < 1) return fail(SMPLSIM_EINVAL, f + ": SMPLSIM_ROLLOUT_CTRL needs nsub >= 1");
   if (mode == SMPLSIM_ROLLOUT_ACTION && nsub != 0)
-    return fail(SMPLSIM_EINVAL, "smplsim_rollout: SMPLSIM_ROLLOUT_ACTION takes nsub = 0 (an action step runs cfg.env.nsubsteps substeps)");
-  if (!xpos_dev != !xquat_dev) return fail(SMPLSIM_EINVAL, "smplsim_rollout: give both xpos and xquat, or neither");
+    return fail(SMPLSIM_EINVAL, f + ": SMPLSIM_ROLLOUT_ACTION takes nsub = 0 (an action step runs cfg.env.nsubsteps substeps)");
+  if (!xpos_dev != !xquat_dev) return fail(SMPLSIM_EINVAL, f + ": give both xpos and xquat, or neither");
   if (h->selfcol)
-    return fail(SMPLSIM_EUNSUPPORTED, "smplsim_rollout: the rollout on caller rows does not build geom-geom contacts (handle created with self_collision = 1)");
+    return fail(SMPLSIM_EUNSUPPORTED, f + ": the rollout on caller rows does not build geom-geom contacts (handle created with self_collision = 1)");
   const LHdr& H = *h->img.hdr();
   if (mode == SMPLSIM_ROLLOUT_ACTION && H.cfg.control_mode == SMPLSIM_CTRL_SIMPLE_PID)
-    return fail(SMPLSIM_EUNSUPPORTED, "smplsim_rollout: control_mode simple_pid keeps its integral / last error in env state, which rollout rows do not have");
-  if (n == 0) return SMPLSIM_OK;   // nothing is read: empty tensors may come as NULL
+    return fail(SMPLSIM_EUNSUPPORTED, f + ": control_mode simple_pid keeps its integral / last error in env state, which rollout rows do not have");
+  if (n == 0) { *empty = true; return SMPLSIM_OK; }   // nothing is read: empty tensors may come as NULL
   if (!qpos0_dev || !qvel0_dev || !control_dev || !qpos_dev || !qvel_dev)
-    return fail(SMPLSIM_EINVAL, "smplsim_rollout: null argument (qpos0, qvel0, control, qpos and qvel are required)");
-  if (int rc = env_rows(h, n, "smplsim_rollout", true)) return rc;
-  DeviceGuard guard(h->device);
-  const size_t nq = H.nv + 1, nv = H.nv, nu = H.nu, nb = H.nb, T = (size_t)nstep, N = (size_t)h->num_envs;
-  LRollArgs a; std::memset(&a, 0, sizeof a);
+    return fail(SMPLSIM_EINVAL, f + ": null argument (qpos0, qvel0, control, qpos and qvel are required)");
+  if (int rc = env_rows(h, n, fn, true)) return rc;
+  const size_t nq = H.nv + 1, nv = H.nv, N = (size_t)h->num_envs;
+  std::memset(&a, 0, sizeof a);
   a.qpos0 = qpos0_dev; a.qvel0 = qvel0_dev; a.qacc_warm0 = qacc_warmstart_dev; a.control = control_dev;
   a.qpos_fwd0 = qpos_fwd0_dev ? qpos_fwd0_dev : qpos0_dev; a.qvel_fwd0 = qvel_fwd0_dev ? qvel_fwd0_dev : qvel0_dev;   // as set_state marks
   a.qpos = qpos_dev; a.qvel = qvel_dev; a.status = status_dev; a.xpos = xpos_dev; a.xquat = xquat_dev;
   a.scr.qpos = h->groll; a.scr.qvel = a.scr.qpos + N * nq; a.scr.qpos_fwd = a.scr.qvel + N * nv; a.scr.qvel_fwd = a.scr.qpos_fwd + N * nq;
   a.gscr = h->gscr; a.map = h->map(); a.n = n; a.nstep = nstep; a.mode = mode;
   a.nsub = mode == SMPLSIM_ROLLOUT_ACTION ? H.cfg.nsubsteps : nsub;
-  auto advance = [nq, nv, nu, nb, T](LRollArgs& c, size_t r) {
-    c.qpos0 += r * nq; c.qvel0 += r * nv; c.qpos_fwd0 += r * nq; c.qvel_fwd0 += r * nv; c.control += r * T * nu;
-    if (c.qacc_warm0) c.qacc_warm0 += r * nv;
-    c.qpos += r * T * nq; c.qvel += r * T * nv;
-    if (c.status) c.status += r * T;
-    if (c.xpos) { c.xpos += r * T * nb * 3; c.xquat += r * T * nb * 4; }
-  };
+  return SMPLSIM_OK;
+}
+// moves every row pointer of a rollout launch to row r
+static void roll_advance(const LHdr& H, LRollArgs& c, size_t r) {
+  const size_t nq = H.nv + 1, nv = H.nv, nu = H.nu, nb = H.nb, T = (size_t)c.nstep;
+  c.qpos0 += r * nq; c.qvel0 += r * nv; c.qpos_fwd0 += r * nq; c.qvel_fwd0 += r * nv; c.control += r * T * nu;
+  if (c.qacc_warm0) c.qacc_warm0 += r * nv;
+  c.qpos += r * T * nq; c.qvel += r * T * nv;
+  if (c.status) c.status += r * T;
+  if (c.xpos) { c.xpos += r * T * nb * 3; c.xquat += r * T * nb * 4; }
+}
+
+extern "C" int smplsim_rollout(SmplsimHandle* h, int mode, int nsub, const float* qpos0_dev, const float* qvel0_dev, const float* qacc_warmstart_dev,
+                               const float* qpos_fwd0_dev, const float* qvel_fwd0_dev, const float* control_dev, int n, int nstep,
+                               float* qpos_dev, float* qvel_dev, uint8_t* status_dev, float* xpos_dev, float* xquat_dev, void* stream) {
+  LRollArgs a; bool empty;
+  if (int rc = roll_args(h, "smplsim_rollout", mode, nsub, qpos0_dev, qvel0_dev, qacc_warmstart_dev, qpos_fwd0_dev, qvel_fwd0_dev, control_dev,
+                         n, nstep, qpos_dev, qvel_dev, status_dev, xpos_dev, xquat_dev, a, &empty)) return rc;
+  if (empty) return SMPLSIM_OK;
+  DeviceGuard guard(h->device);
+  const LHdr& H = *h->img.hdr();
+  auto advance = [&H](LRollArgs& c, size_t r) { roll_advance(H, c, r); };
   L_DISPATCH(h, state_rows<C_>(h, lane_kernels<C_>().roll, a, advance, (cudaStream_t)stream));
+  CUDA_TRY(cudaGetLastError());
+  return SMPLSIM_OK;
+}
+
+extern "C" int smplsim_rollout_feedback(SmplsimHandle* h, int mode, int nsub, const float* qpos0_dev, const float* qvel0_dev,
+                                        const float* qacc_warmstart_dev, const float* qpos_fwd0_dev, const float* qvel_fwd0_dev,
+                                        const float* control_dev, int n, int nstep, float* qpos_dev, float* qvel_dev, uint8_t* status_dev,
+                                        float* xpos_dev, float* xquat_dev, const float* gain_dev, const float* qpos_ref_dev,
+                                        const float* qvel_ref_dev, int ref_rows, int clip_actions, float* control_applied_dev, void* stream) {
+  LRollFbArgs a; bool empty;
+  std::memset(&a, 0, sizeof a);
+  if (int rc = roll_args(h, "smplsim_rollout_feedback", mode, nsub, qpos0_dev, qvel0_dev, qacc_warmstart_dev, qpos_fwd0_dev, qvel_fwd0_dev,
+                         control_dev, n, nstep, qpos_dev, qvel_dev, status_dev, xpos_dev, xquat_dev, a.r, &empty)) return rc;
+  if (ref_rows != 1 && ref_rows != n)
+    return fail(SMPLSIM_EINVAL, "smplsim_rollout_feedback: ref_rows must be 1 (one schedule for every row) or n (one per row)");
+  if (empty) return SMPLSIM_OK;
+  if (!gain_dev || !qpos_ref_dev || !qvel_ref_dev)
+    return fail(SMPLSIM_EINVAL, "smplsim_rollout_feedback: null argument (gain, qpos_ref and qvel_ref are required)");
+  DeviceGuard guard(h->device);
+  const LHdr& H = *h->img.hdr();
+  const size_t nq = H.nv + 1, nv = H.nv, nu = H.nu, T = (size_t)nstep;
+  a.gain = gain_dev; a.qpos_ref = qpos_ref_dev; a.qvel_ref = qvel_ref_dev; a.control_applied = control_applied_dev;
+  a.dx = h->gfb; a.uscr = h->gfb + (size_t)2 * nv * h->num_envs;
+  a.shared_ref = ref_rows == 1; a.clip = clip_actions != 0;
+  auto advance = [&H, nq, nv, nu, T](LRollFbArgs& c, size_t r) {
+    roll_advance(H, c.r, r);
+    if (c.control_applied) c.control_applied += r * T * nu;
+    if (!c.shared_ref) { c.gain += r * T * nu * 2 * nv; c.qpos_ref += r * T * nq; c.qvel_ref += r * T * nv; }
+  };
+  L_DISPATCH(h, state_rows<C_>(h, lane_kernels<C_>().rollfb, a, advance, (cudaStream_t)stream));
   CUDA_TRY(cudaGetLastError());
   return SMPLSIM_OK;
 }
@@ -1120,6 +1175,7 @@ extern "C" int smplsim_debug_stats(int* out, int reset) {   // out: L_NSTATS cou
 
 #ifdef SMPLSIM_EMU
 #include "rollout_kernels.cu"   // the device build compiles it as a translation unit of its own (_lib.build)
+#include "rollout_feedback_kernels.cu"   // as rollout_kernels.cu
 #include "inverse_fd_kernels.cu"   // as rollout_kernels.cu
 #include "centroidal_kernels.cu"   // as rollout_kernels.cu
 #include "rne_post_kernels.cu"   // as rollout_kernels.cu

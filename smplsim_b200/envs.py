@@ -132,6 +132,37 @@ def rollout(model, data, initial_state, control, nstep=None):
     return data._rollout_fn(initial_state, control, nstep)
 
 
+def mj_differentiatePos(model, qvel, dt, qpos1, qpos2):
+    """``mujoco.mj_differentiatePos``: ``qvel = (qpos2 (-) qpos1) / dt`` in place, fp64, for this model's joints (one free root joint,
+    then hinges).  The root rotation is ``mju_subQuat``: ``log(normalise(q1)^-1 * normalise(q2))`` on the shortest arc, in ``q1``'s
+    body frame -- the tangent of ``mjd_transitionFD`` and of ``HumanoidBatchB200.rollout``'s feedback law.  ``model`` is accepted
+    for the signature (the layout follows from the lengths)."""
+    q1, q2 = np.asarray(qpos1, dtype=np.float64).ravel(), np.asarray(qpos2, dtype=np.float64).ravel()
+    b, c = q1[3:7] / np.linalg.norm(q1[3:7]), q2[3:7] / np.linalg.norm(q2[3:7])
+    rw = b[0] * c[0] + b[1:] @ c[1:]
+    rv = b[0] * c[1:] - c[0] * b[1:] - np.cross(b[1:], c[1:])
+    if rw < 0:
+        rw, rv = -rw, -rv
+    s = np.linalg.norm(rv)
+    d = np.concatenate([q2[0:3] - q1[0:3], rv * (2 * np.arctan2(s, rw) / s) if s > 0 else np.zeros(3), q2[7:] - q1[7:]])
+    qvel.reshape(-1)[:] = d / dt
+
+
+def mj_integratePos(model, qpos, qvel, dt):
+    """``mujoco.mj_integratePos``: ``qpos <- qpos (+) qvel dt`` in place, fp64; the root rotation as ``q * exp(qvel[3:6] dt)`` (body
+    frame), normalised.  The inverse of ``mj_differentiatePos``.  ``model`` is accepted for the signature."""
+    q = qpos.reshape(-1)
+    d = np.asarray(qvel, dtype=np.float64).ravel() * dt
+    w = d[3:6]
+    th = np.linalg.norm(w)
+    e = np.concatenate([[np.cos(th / 2)], np.sin(th / 2) / th * w if th > 0 else np.zeros(3)])
+    a = q[3:7].astype(np.float64)
+    r = np.concatenate([[a[0] * e[0] - a[1:] @ e[1:]], a[0] * e[1:] + e[0] * a[1:] + np.cross(a[1:], e[1:])])
+    q[0:3] += d[0:3]
+    q[3:7] = r / np.linalg.norm(r)
+    q[7:] += d[6:]
+
+
 def mj_subtreeVel(model, data):
     """``mujoco.mj_subtreeVel`` for an env's ``mj_data``: fills ``data.subtree_linvel`` and ``data.subtree_angmom`` [nbody + 1, 3]
     (MuJoCo body order; row 0, the world's subtree, is the whole robot's), the velocity of each subtree's centre of mass and the
