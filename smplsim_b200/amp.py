@@ -61,15 +61,7 @@ def amp_config(amp_cfg: Optional[Dict[str, Any]] = None) -> Dict[str, Any]:
 
 def amp_c_cfg(model, amp_cfg: Dict[str, Any]):
     """The ``SmplsimAmpCfg`` of a config, and the key-body array it points at (keep both alive while the struct is used)."""
-    keys = []
-    for x in amp_cfg["key_bodies"]:
-        if isinstance(x, str):
-            if x not in model.body_names:
-                raise ValueError(f"unknown key body name {x!r}")
-            x = list(model.body_names).index(x)
-        if isinstance(x, bool) or not isinstance(x, (int, np.integer)):
-            raise ValueError(f"key_bodies entries must be body names or indices, got {x!r}")
-        keys.append(int(x))
+    keys = [model.body_index(x, "key_bodies entries must be body names or indices", kind="key body") for x in amp_cfg["key_bodies"]]
     arr = np.ascontiguousarray(np.asarray(keys, dtype=np.int32))
     c = SmplsimAmpCfgC(num_steps=int(amp_cfg["num_amp_obs_steps"]), num_key_bodies=len(keys), key_bodies=arr.ctypes.data if keys else None,
                        local_root_obs=int(bool(amp_cfg["local_root_obs"])), root_height_obs=int(bool(amp_cfg["root_height_obs"])),

@@ -29,6 +29,9 @@ def _fd_eps(**eps: float):
     return [float(e) for e in eps.values()]
 
 
+_NO_ENVS = object()     # HumanoidBatchB200._env_mask of an empty index tensor: the call selects no env
+
+
 class HumanoidBatchB200:
     """N independent SMPL humanoid envs stepped in lockstep on one GPU.
 
@@ -159,15 +162,9 @@ class HumanoidBatchB200:
     def reset(self, env_ids: Optional[torch.Tensor] = None, init_mode: int = -1, qpos0: Optional[torch.Tensor] = None,
               qvel0: Optional[torch.Tensor] = None):
         """HumanoidTask.reset for ``env_ids`` (None = all; an index tensor or a uint8/bool mask)."""
-        mask = None
-        if env_ids is not None:
-            if env_ids.dtype in (torch.bool, torch.uint8) and env_ids.numel() == self.num_envs:
-                mask = env_ids.to(torch.uint8).contiguous()
-            else:
-                if env_ids.numel() == 0:
-                    return self.obs_buf
-                mask = torch.zeros(self.num_envs, dtype=torch.uint8, device=self.device)
-                mask[env_ids.long()] = 1
+        mask = self._env_mask(env_ids)
+        if mask is _NO_ENVS:
+            return self.obs_buf
         if qpos0 is not None:
             qpos0 = qpos0.to(self.device, torch.float32).contiguous()
             qvel0 = qvel0.to(self.device, torch.float32).contiguous()
@@ -176,6 +173,20 @@ class HumanoidBatchB200:
         self.gpu_launches += 1
         self._keep = (mask, qpos0, qvel0)
         return self.obs_buf
+
+    def _env_mask(self, env_ids):
+        """The uint8 [num_envs] mask of an env selection: None (all envs) stays None, a bool / uint8 mask of num_envs entries is
+        converted where it is (a contiguous uint8 mask is returned as it is, so ``reset(self.reset_buf)`` allocates, copies and syncs
+        nothing), an index tensor is scattered into a new mask on this batch's device, and an empty index tensor gives ``_NO_ENVS``."""
+        if env_ids is None:
+            return None
+        if env_ids.dtype in (torch.bool, torch.uint8) and env_ids.numel() == self.num_envs:
+            return env_ids.to(torch.uint8).contiguous()
+        if env_ids.numel() == 0:
+            return _NO_ENVS
+        mask = torch.zeros(self.num_envs, dtype=torch.uint8, device=self.device)
+        mask[env_ids.long()] = 1
+        return mask
 
     def reset_done(self):
         """Reset every env whose reset_buf is set (in-stream, no host sync)."""
@@ -210,20 +221,8 @@ class HumanoidBatchB200:
 
     @xfrc_applied.setter
     def xfrc_applied(self, t: Optional[torch.Tensor]):
-        if t is not None:
-            shape = (self.num_envs, self.model.nbody, 6)
-            if not isinstance(t, torch.Tensor):
-                raise ValueError(f"xfrc_applied must be a torch.Tensor of shape {shape} or None, got {type(t).__name__}")
-            if tuple(t.shape) != shape:
-                raise ValueError(f"xfrc_applied must have shape {shape} (envs, robot bodies, force + torque), got {tuple(t.shape)}")
-            if t.dtype != torch.float32:
-                raise ValueError(f"xfrc_applied must be float32, got {t.dtype}")
-            dv = self.device
-            if t.device.type != dv.type or (dv.index is not None and t.device.index != dv.index):
-                raise ValueError(f"xfrc_applied must live on {dv}, got {t.device}")
-            if not t.is_contiguous():
-                raise ValueError("xfrc_applied must be contiguous")
-        self._xfrc = t
+        shape = (self.num_envs, self.model.nbody, 6)
+        self._xfrc = self._checked("xfrc_applied", t, shape, optional=True, want=f"{shape} (envs, robot bodies, force + torque)")
 
     def _set_xfrc(self):
         """The wrench pointer of this call (NULL: none); the tensor is kept referenced until the next call."""
@@ -259,30 +258,10 @@ class HumanoidBatchB200:
         step.  ``step``, ``mj_step``, ``reset``, ``inverse``, ``dynamics`` and ``render`` (TRACKCOM) use the values from the next call on;
         ``inverse`` and ``dynamics`` then take ``n == num_envs`` rows (row i = env i).  ``clear_env_params`` goes back to the model."""
         vals = {"friction": friction, "gravity": gravity, "kp": kp, "kd": kd, "torque_limit": torque_limit, "body_mass_scale": body_mass_scale}
-        shapes, dv = self._env_param_shapes(), self.device
-        given = {}
-        for name, t in vals.items():
-            if t is None:
-                continue
-            if not isinstance(t, torch.Tensor):
-                raise ValueError(f"{name} must be a torch.Tensor, got {type(t).__name__}")
-            if tuple(t.shape) != shapes[name]:
-                raise ValueError(f"{name} must have shape {shapes[name]}, got {tuple(t.shape)}")
-            if t.dtype != torch.float32:
-                raise ValueError(f"{name} must be float32, got {t.dtype}")
-            if t.device.type != dv.type or (dv.index is not None and t.device.index != dv.index):
-                raise ValueError(f"{name} must live on {dv}, got {t.device}")
-            given[name] = t.contiguous()
-        mask = None
-        if env_ids is not None:
-            if env_ids.dtype in (torch.bool, torch.uint8) and env_ids.numel() == self.num_envs:
-                mask = env_ids.to(dv, torch.uint8).contiguous()
-            else:
-                if env_ids.numel() == 0:
-                    return
-                mask = torch.zeros(self.num_envs, dtype=torch.uint8, device=dv)
-                mask[env_ids.to(dv).long()] = 1
-        if not given:
+        shapes = self._env_param_shapes()
+        given = {name: self._checked(name, t, shapes[name], copy=True, want=str(shapes[name])) for name, t in vals.items() if t is not None}
+        mask = self._env_mask(None if env_ids is None else env_ids.to(self.device))
+        if mask is _NO_ENVS or not given:
             return
         sel = None if mask is None else mask.bool()
         bad = []
@@ -340,23 +319,39 @@ class HumanoidBatchB200:
         self.gpu_launches += 1
         return xpos, xquat
 
-    def _rows(self, args):
-        """Caller state rows (name, tensor, width) checked for shape [n, width] with the n of the first, float32 and this batch's device;
-        returned contiguous."""
-        rows = []
-        n = args[0][1].shape[0] if isinstance(args[0][1], torch.Tensor) else None
-        for name, t, w in args:
-            if not isinstance(t, torch.Tensor):
-                raise ValueError(f"{name} must be a torch.Tensor, got {type(t).__name__}")
-            if t.dim() != 2 or t.shape[1] != w or t.shape[0] != n:
-                raise ValueError(f"{name} must have shape [n, {w}] with the same n as qpos, got {tuple(t.shape)}")
-            if t.dtype != torch.float32:
-                raise ValueError(f"{name} must be float32, got {t.dtype}")
-            dv = self.device
-            if t.device.type != dv.type or (dv.index is not None and t.device.index != dv.index):
-                raise ValueError(f"{name} must live on {dv}, got {t.device}")
-            rows.append(t.contiguous())
-        return rows
+    def _checked(self, name, t, shape, copy=False, optional=False, want=None):
+        """Caller tensor ``t`` checked for ``shape`` (None entries free), float32 and this batch's device, and returned.  A tensor that is
+        not contiguous is refused, or with ``copy`` returned as a contiguous copy (for inputs the call only reads; a tensor the batch
+        keeps, as ``xfrc_applied``, must stay the caller's).  With ``optional`` None (the argument left out) is returned as None.
+        ``want``: the shape as the refusal states it (default: ``shape``, free entries as n)."""
+        if t is None and optional:
+            return None
+        if not isinstance(t, torch.Tensor):
+            raise ValueError(f"{name} must be a torch.Tensor{' or None' if optional else ''}, got {type(t).__name__}")
+        if t.dim() != len(shape) or any(s is not None and t.shape[i] != s for i, s in enumerate(shape)):
+            want = want or "[" + ", ".join("n" if s is None else str(s) for s in shape) + "]"
+            raise ValueError(f"{name} must have shape {want}, got {tuple(t.shape)}")
+        if t.dtype != torch.float32:
+            raise ValueError(f"{name} must be float32, got {t.dtype}")
+        dv = self.device
+        if t.device.type != dv.type or (dv.index is not None and t.device.index != dv.index):
+            raise ValueError(f"{name} must live on {dv}, got {t.device}")
+        if t.is_contiguous():
+            return t
+        if not copy:
+            raise ValueError(f"{name} must be contiguous")
+        return t.contiguous()
+
+    def _rows(self, *rows, n=None, optional=False):
+        """Caller state rows ``(name, tensor, width)``, each ``[n, width]`` with the n of qpos (``n``, or the first row's), checked by
+        ``_checked`` and returned contiguous; with ``optional`` a row given as None is returned as None."""
+        out = []
+        for name, t, w in rows:
+            t = self._checked(name, t, (n, w), copy=True, optional=optional, want=f"[n, {w}] with the same n as qpos")
+            if n is None:
+                n = t.shape[0]
+            out.append(t)
+        return out
 
     def inverse(self, qpos: torch.Tensor, qvel: torch.Tensor, qacc: torch.Tensor, contact_wrench: bool = False):
         """mujoco.mj_inverse on caller rows: ``qfrc_inverse [n, nv]`` (and ``contact_wrench [n, nbody, 6]`` when asked), the generalized
@@ -367,7 +362,7 @@ class HumanoidBatchB200:
         batch, n == num_envs with per-env shapes (row i uses env i's shape).  Reads no env state and changes none; ``xfrc_applied``
         is not taken.  Not available with ``cfg.env.self_collision``."""
         m = self.model
-        q, v, a = self._rows((("qpos", qpos, m.nq), ("qvel", qvel, m.nv), ("qacc", qacc, m.nv)))
+        q, v, a = self._rows(("qpos", qpos, m.nq), ("qvel", qvel, m.nv), ("qacc", qacc, m.nv))
         n = q.shape[0]
         out = torch.empty(n, m.nv, dtype=torch.float32, device=self.device)
         cw = torch.empty(n, m.nbody, 6, dtype=torch.float32, device=self.device) if contact_wrench else None
@@ -386,13 +381,9 @@ class HumanoidBatchB200:
         Float32 tensors on this batch's device; row rules of ``inverse``.  Reads no env state and changes none; ``xfrc_applied`` is not
         taken.  Not available with ``cfg.env.self_collision``."""
         m = self.model
-        args = (("qpos", qpos, m.nq), ("qvel", qvel, m.nv), ("ctrl", ctrl, m.nu))
-        if qacc_warmstart is not None:
-            args += (("qacc_warmstart", qacc_warmstart, m.nv),)
-        rows = self._rows(args)
-        q, v, u = rows[:3]
-        w = rows[3] if qacc_warmstart is not None else None
+        q, v, u = self._rows(("qpos", qpos, m.nq), ("qvel", qvel, m.nv), ("ctrl", ctrl, m.nu))
         n, dv = q.shape[0], self.device
+        (w,) = self._rows(("qacc_warmstart", qacc_warmstart, m.nv), n=n, optional=True)
         out = {"qacc": torch.empty(n, m.nv, dtype=torch.float32, device=dv), "contact_mask": torch.empty(n, dtype=torch.int64, device=dv),
                "solver_iter": torch.empty(n, dtype=torch.int32, device=dv), "status": torch.empty(n, dtype=torch.uint8, device=dv)}
         if contact_wrench:
@@ -423,7 +414,7 @@ class HumanoidBatchB200:
         changes none."""
         m = self.model
         eps = _fd_eps(eps_qpos=eps_qpos, eps_qvel=eps_qvel, eps_ctrl=eps_ctrl)
-        q, v, u = self._rows((("qpos", qpos, m.nq), ("qvel", qvel, m.nv), ("ctrl", ctrl, m.nu)))
+        q, v, u = self._rows(("qpos", qpos, m.nq), ("qvel", qvel, m.nv), ("ctrl", ctrl, m.nu))
         n, nx, f32 = q.shape[0], 2 * m.nv, dict(dtype=torch.float32, device=self.device)
         ncol = nx + m.nu
         out = {"qacc": torch.empty(n, m.nv, **f32), "A": torch.empty(n, nx, nx, **f32), "B": torch.empty(n, nx, m.nu, **f32),
@@ -455,7 +446,7 @@ class HumanoidBatchB200:
         otherwise), not with ``cfg.env.self_collision``.  Reads no env state and changes none."""
         m = self.model
         eps = _fd_eps(eps_qpos=eps_qpos, eps_qvel=eps_qvel, eps_qacc=eps_qacc)
-        q, v, a = self._rows((("qpos", qpos, m.nq), ("qvel", qvel, m.nv), ("qacc", qacc, m.nv)))
+        q, v, a = self._rows(("qpos", qpos, m.nq), ("qvel", qvel, m.nv), ("qacc", qacc, m.nv))
         n, ncol, f32 = q.shape[0], 3 * m.nv, dict(dtype=torch.float32, device=self.device)
         out = {"qfrc_inverse": torch.empty(n, m.nv, **f32), "dfrc": torch.empty(n, m.nv, ncol, **f32),
                "flags": torch.empty(n, ncol, dtype=torch.uint8, device=self.device)}
@@ -516,12 +507,11 @@ class HumanoidBatchB200:
             ns = 1 if nsub is None else nsub
             if isinstance(ns, bool) or not isinstance(ns, (int, np.integer)) or ns < 1:
                 raise ValueError(f"nsub must be an int >= 1, got {nsub!r}")
-        args = (("qpos", qpos, m.nq), ("qvel", qvel, m.nv))
-        opt = [(k, t, w) for k, t, w in (("qacc_warmstart", qacc_warmstart, m.nv), ("qpos_fwd", qpos_fwd, m.nq), ("qvel_fwd", qvel_fwd, m.nv))
-               if t is not None]
-        rows = dict(zip([a[0] for a in args + tuple(opt)], self._rows(args + tuple(opt))))
-        n = rows["qpos"].shape[0]
-        u = self._checked("control", control.contiguous() if isinstance(control, torch.Tensor) else control, (n, None, m.nu))
+        q, v = self._rows(("qpos", qpos, m.nq), ("qvel", qvel, m.nv))
+        n = q.shape[0]
+        w, qf, vf = self._rows(("qacc_warmstart", qacc_warmstart, m.nv), ("qpos_fwd", qpos_fwd, m.nq), ("qvel_fwd", qvel_fwd, m.nv), n=n,
+                               optional=True)
+        u = self._checked("control", control, (n, None, m.nu), copy=True)
         T = u.shape[1]
         if T < 1:
             raise ValueError("control must hold at least one step ([n, T, nu] with T >= 1)")
@@ -529,12 +519,12 @@ class HumanoidBatchB200:
             if qpos_ref is None or qvel_ref is None:
                 raise ValueError("gains need qpos_ref and qvel_ref (the reference state of the feedback law)")
             nx = 2 * m.nv
-            K = self._checked("gains", gains.contiguous() if isinstance(gains, torch.Tensor) else gains, (None, T, m.nu, nx))
+            K = self._checked("gains", gains, (None, T, m.nu, nx), copy=True)
             r = K.shape[0]
             if r not in (1, n):
                 raise ValueError(f"gains, qpos_ref and qvel_ref must have leading dimension 1 (shared) or n = {n}, got {r}")
-            qr = self._checked("qpos_ref", qpos_ref.contiguous() if isinstance(qpos_ref, torch.Tensor) else qpos_ref, (r, T, m.nq))
-            vr = self._checked("qvel_ref", qvel_ref.contiguous() if isinstance(qvel_ref, torch.Tensor) else qvel_ref, (r, T, m.nv))
+            qr = self._checked("qpos_ref", qpos_ref, (r, T, m.nq), copy=True)
+            vr = self._checked("qvel_ref", qvel_ref, (r, T, m.nv), copy=True)
         elif mode == "action" and bool(self.cfg.env.clip_actions):
             u = torch.clamp(u, -1.0, 1.0)
         dv, f32 = self.device, dict(dtype=torch.float32, device=self.device)
@@ -545,16 +535,14 @@ class HumanoidBatchB200:
             out["xpos"] = torch.empty(n, T, m.nbody, 3, **f32)
             out["xquat"] = torch.empty(n, T, m.nbody, 4, **f32)
         if gains is None:
-            self._check(self._L().smplsim_rollout(self._h, self.ROLLOUT_MODES[mode], int(ns), _ptr(rows["qpos"]), _ptr(rows["qvel"]),
-                                                  _ptr(rows.get("qacc_warmstart")), _ptr(rows.get("qpos_fwd")), _ptr(rows.get("qvel_fwd")), _ptr(u),
-                                                  n, T, _ptr(out["qpos"]), _ptr(out["qvel"]), _ptr(out.get("status")), _ptr(out.get("xpos")),
-                                                  _ptr(out.get("xquat")), self._stream()))
+            self._check(self._L().smplsim_rollout(self._h, self.ROLLOUT_MODES[mode], int(ns), _ptr(q), _ptr(v), _ptr(w), _ptr(qf), _ptr(vf),
+                                                  _ptr(u), n, T, _ptr(out["qpos"]), _ptr(out["qvel"]), _ptr(out.get("status")),
+                                                  _ptr(out.get("xpos")), _ptr(out.get("xquat")), self._stream()))
         else:
             out["control"] = torch.empty(n, T, m.nu, **f32)
             self._check(self._L().smplsim_rollout_feedback(
-                self._h, self.ROLLOUT_MODES[mode], int(ns), _ptr(rows["qpos"]), _ptr(rows["qvel"]), _ptr(rows.get("qacc_warmstart")),
-                _ptr(rows.get("qpos_fwd")), _ptr(rows.get("qvel_fwd")), _ptr(u), n, T, _ptr(out["qpos"]), _ptr(out["qvel"]),
-                _ptr(out.get("status")), _ptr(out.get("xpos")), _ptr(out.get("xquat")), _ptr(K), _ptr(qr), _ptr(vr), r,
+                self._h, self.ROLLOUT_MODES[mode], int(ns), _ptr(q), _ptr(v), _ptr(w), _ptr(qf), _ptr(vf), _ptr(u), n, T, _ptr(out["qpos"]),
+                _ptr(out["qvel"]), _ptr(out.get("status")), _ptr(out.get("xpos")), _ptr(out.get("xquat")), _ptr(K), _ptr(qr), _ptr(vr), r,
                 int(bool(self.cfg.env.clip_actions)), _ptr(out["control"]), self._stream()))
         self.gpu_launches += 1
         return out
@@ -614,18 +602,9 @@ class HumanoidBatchB200:
         m = self.model
         if bias and qvel is None:
             raise ValueError("bias=True needs qvel")
-        args = (("qpos", qpos, m.nq),) + ((("qvel", qvel, m.nv),) if qvel is not None else ())
-        rows = self._rows(args)
-        q, v = rows[0], (rows[1] if qvel is not None else None)
-        bodies = []
-        for b in (jac_bodies if jac_bodies is not None else []):
-            if isinstance(b, str):
-                if b not in m.body_names:
-                    raise ValueError(f"unknown body name {b!r}")
-                b = list(m.body_names).index(b)
-            if isinstance(b, bool) or not isinstance(b, (int, np.integer)) or not 0 <= int(b) < m.nbody:
-                raise ValueError(f"jac_bodies entries must be body names or indices in [0, {m.nbody}), got {b!r}")
-            bodies.append(int(b))
+        (q,) = self._rows(("qpos", qpos, m.nq))
+        (v,) = self._rows(("qvel", qvel, m.nv), n=q.shape[0], optional=True)
+        bodies = [self._body("jac_bodies entries", b) for b in (jac_bodies if jac_bodies is not None else [])]
         n, f32 = q.shape[0], dict(dtype=torch.float32, device=self.device)
         out = {}
         if mass_matrix:
@@ -667,18 +646,9 @@ class HumanoidBatchB200:
         m = self.model
         if velocity and qvel is None:
             raise ValueError("velocity=True needs qvel")
-        args = (("qpos", qpos, m.nq),) + ((("qvel", qvel, m.nv),) if qvel is not None else ())
-        rows = self._rows(args)
-        q, v = rows[0], (rows[1] if qvel is not None else None)
-        bodies = []
-        for b in (jac_com_bodies if jac_com_bodies is not None else []):
-            if isinstance(b, str):
-                if b not in m.body_names:
-                    raise ValueError(f"unknown body name {b!r}")
-                b = list(m.body_names).index(b)
-            if isinstance(b, bool) or not isinstance(b, (int, np.integer)) or not 0 <= int(b) < m.nbody:
-                raise ValueError(f"jac_com_bodies entries must be body names or indices in [0, {m.nbody}), got {b!r}")
-            bodies.append(int(b))
+        (q,) = self._rows(("qpos", qpos, m.nq))
+        (v,) = self._rows(("qvel", qvel, m.nv), n=q.shape[0], optional=True)
+        bodies = [self._body("jac_com_bodies entries", b) for b in (jac_com_bodies if jac_com_bodies is not None else [])]
         n, f32 = q.shape[0], dict(dtype=torch.float32, device=self.device)
         out = {}
         if com:
@@ -701,6 +671,14 @@ class HumanoidBatchB200:
             self.gpu_launches += 1
         return out
 
+    def _body(self, what, b):
+        """``ModelDesc.body_index`` of ``b`` checked against [0, nbody); ``what`` names the argument in the messages."""
+        rule = f"{what} must be body names or indices in [0, {self.model.nbody})"
+        i = self.model.body_index(b, rule)
+        if not 0 <= i < self.model.nbody:
+            raise ValueError(f"{rule}, got {b!r}")
+        return i
+
     RNE_POST_MAX_SITES = 64
 
     def _imu_sites(self, imu_sites):
@@ -718,18 +696,13 @@ class HumanoidBatchB200:
             if not isinstance(s, (tuple, list)) or len(s) != 3:
                 raise ValueError(f"imu_sites entries must be (body name or index, pos[3], quat[4]), got {s!r}")
             b, p, q = s
-            if isinstance(b, str):
-                if b not in m.body_names:
-                    raise ValueError(f"unknown body name {b!r}")
-                b = list(m.body_names).index(b)
-            if isinstance(b, bool) or not isinstance(b, (int, np.integer)) or not 0 <= int(b) < m.nbody:
-                raise ValueError(f"imu_sites bodies must be body names or indices in [0, {m.nbody}), got {b!r}")
+            b = self._body("imu_sites bodies", b)
             p, q = np.asarray(p, dtype=np.float64), np.asarray(q, dtype=np.float64)
             if p.shape != (3,) or not np.all(np.isfinite(p)):
                 raise ValueError(f"imu_sites pos must be 3 finite numbers, got {s[1]!r}")
             if q.shape != (4,) or not abs(float(np.linalg.norm(q)) - 1.0) <= 1e-3:
                 raise ValueError(f"imu_sites quat must be a unit quaternion (w, x, y, z), got {s[2]!r}")
-            sb.append(int(b)); sp.append(p); sq.append(q)
+            sb.append(b); sp.append(p); sq.append(q)
         return (np.ascontiguousarray(np.asarray(sb, dtype=np.int32)), np.ascontiguousarray(np.asarray(sp, dtype=np.float32).reshape(-1, 3)),
                 np.ascontiguousarray(np.asarray(sq, dtype=np.float32).reshape(-1, 4)))
 
@@ -754,9 +727,9 @@ class HumanoidBatchB200:
         one-shape batch without per-env parameters, n == num_envs otherwise (row i uses env i's shape, gravity and mass scales).  Reads no
         env state and changes none.  Not available with ``cfg.env.self_collision``."""
         m = self.model
-        q, v, a = self._rows((("qpos", qpos, m.nq), ("qvel", qvel, m.nv), ("qacc", qacc, m.nv)))
+        q, v, a = self._rows(("qpos", qpos, m.nq), ("qvel", qvel, m.nv), ("qacc", qacc, m.nv))
         n, f32 = q.shape[0], dict(dtype=torch.float32, device=self.device)
-        xf = None if xfrc_applied is None else self._checked("xfrc_applied", xfrc_applied, (n, m.nbody, 6))
+        xf = self._checked("xfrc_applied", xfrc_applied, (n, m.nbody, 6), optional=True)
         sb, sp, sq = self._imu_sites(imu_sites) if imu_sites is not None else (None, None, None)
         ns = 0 if sb is None else len(sb)
         out = {}
@@ -776,22 +749,6 @@ class HumanoidBatchB200:
         return out
 
     # ------------------------------------------------------------------ ray casting and cameras (mj_ray, mujoco.Renderer)
-    def _checked(self, name, t, shape):
-        """A caller tensor checked as xfrc_applied is: shape (None entries free), float32, this batch's device, contiguous."""
-        if not isinstance(t, torch.Tensor):
-            raise ValueError(f"{name} must be a torch.Tensor, got {type(t).__name__}")
-        if t.dim() != len(shape) or any(s is not None and t.shape[i] != s for i, s in enumerate(shape)):
-            want = "[" + ", ".join("n" if s is None else str(s) for s in shape) + "]"
-            raise ValueError(f"{name} must have shape {want}, got {tuple(t.shape)}")
-        if t.dtype != torch.float32:
-            raise ValueError(f"{name} must be float32, got {t.dtype}")
-        dv = self.device
-        if t.device.type != dv.type or (dv.index is not None and t.device.index != dv.index):
-            raise ValueError(f"{name} must live on {dv}, got {t.device}")
-        if not t.is_contiguous():
-            raise ValueError(f"{name} must be contiguous")
-        return t
-
     def _poses(self, xpos, xquat):
         """Body poses of the call: the batch's own post-step xpos / xquat by default."""
         if (xpos is None) != (xquat is None):

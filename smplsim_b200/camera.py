@@ -102,20 +102,13 @@ def trackcom(model, pos, xyaxes, fovy: float = DEFAULT_FOVY, zfar: float = DEFAU
     return Camera(TRACKCOM, off, xyaxes_mat(xyaxes), fovy=fovy, zfar=zfar, name=name)
 
 
-def _body_index(model, body: Union[int, str]) -> int:
-    if isinstance(body, str):
-        if body not in model.body_names:
-            raise ValueError(f"unknown body name {body!r}")
-        return list(model.body_names).index(body)
-    if isinstance(body, bool) or not isinstance(body, (int, np.integer)) or not 0 <= int(body) < model.nbody:
-        raise ValueError(f"body must be a name or an index in [0, {model.nbody}), got {body!r}")
-    return int(body)
-
-
 def body(model, name: Union[int, str], pos=(0.0, 0.0, 0.0), xyaxes=(1.0, 0.0, 0.0, 0.0, 1.0, 0.0), fovy: float = DEFAULT_FOVY,
          zfar: float = DEFAULT_ZFAR, exclude: bool = True) -> Camera:
     """A camera riding on robot body ``name`` (pose in the body frame).  ``exclude``: that body's own geoms are not drawn."""
-    b = _body_index(model, name)
+    rule = f"body must be a name or an index in [0, {model.nbody})"
+    b = model.body_index(name, rule)
+    if not 0 <= b < model.nbody:
+        raise ValueError(f"{rule}, got {name!r}")
     return Camera(BODY, np.asarray(pos, dtype=np.float64), xyaxes_mat(xyaxes), body=b, exclude_body=b if exclude else -1, fovy=fovy,
                   zfar=zfar, name=name if isinstance(name, str) else None)
 

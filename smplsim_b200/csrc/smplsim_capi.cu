@@ -54,6 +54,12 @@ struct SmplsimHandle {
 
 static thread_local std::string g_err;
 static int fail(int code, const std::string& msg) { g_err = msg; return code; }
+// every entry of the caller's body list body[0, n) is a robot body index in [0, nb)
+static bool bodies_in_range(const int32_t* body, int n, int nb) {
+  for (int j = 0; j < n; j++)
+    if (body[j] < 0 || body[j] >= nb) return false;
+  return true;
+}
 #define CUDA_TRY(x)                                                                                     \
   do {                                                                                                  \
     cudaError_t e_ = (x);                                                                               \
@@ -422,8 +428,7 @@ extern "C" int smplsim_dynamics(SmplsimHandle* h, const float* qpos_dev, const f
   const LHdr& H = *h->img.hdr();
   if (njac > H.nb) return fail(SMPLSIM_EINVAL, "smplsim_dynamics: njac > nbody");
   if (njac > 0 && !jac_body) return fail(SMPLSIM_EINVAL, "smplsim_dynamics: njac > 0 needs jac_body");
-  for (int j = 0; j < njac; j++)
-    if (jac_body[j] < 0 || jac_body[j] >= H.nb) return fail(SMPLSIM_EINVAL, "smplsim_dynamics: jac_body entry out of range [0, nbody)");
+  if (!bodies_in_range(jac_body, njac, H.nb)) return fail(SMPLSIM_EINVAL, "smplsim_dynamics: jac_body entry out of range [0, nbody)");
   if (qfrc_bias_dev && !qvel_dev) return fail(SMPLSIM_EINVAL, "smplsim_dynamics: qfrc_bias needs qvel");
   if (n == 0) return SMPLSIM_OK;   // nothing is read: empty tensors may come as NULL
   if (njac > 0 && !jac_dev) return fail(SMPLSIM_EINVAL, "smplsim_dynamics: njac > 0 needs jac_dev");
@@ -456,8 +461,7 @@ extern "C" int smplsim_centroidal(SmplsimHandle* h, const float* qpos_dev, const
   const LHdr& H = *h->img.hdr();
   if (njac > H.nb) return fail(SMPLSIM_EINVAL, "smplsim_centroidal: njac > nbody");
   if (njac > 0 && !jac_body) return fail(SMPLSIM_EINVAL, "smplsim_centroidal: njac > 0 needs jac_body");
-  for (int j = 0; j < njac; j++)
-    if (jac_body[j] < 0 || jac_body[j] >= H.nb) return fail(SMPLSIM_EINVAL, "smplsim_centroidal: jac_body entry out of range [0, nbody)");
+  if (!bodies_in_range(jac_body, njac, H.nb)) return fail(SMPLSIM_EINVAL, "smplsim_centroidal: jac_body entry out of range [0, nbody)");
   if ((subtree_linvel_dev || subtree_angmom_dev || cmm_bias_dev) && !qvel_dev)
     return fail(SMPLSIM_EINVAL, "smplsim_centroidal: subtree_linvel, subtree_angmom and cmm_bias need qvel");
   if (n == 0) return SMPLSIM_OK;   // nothing is read: empty tensors may come as NULL
@@ -499,6 +503,8 @@ extern "C" int smplsim_rne_post(SmplsimHandle* h, const float* qpos_dev, const f
   if (nsite > LRNEP_MAXS) return fail(SMPLSIM_EINVAL, "smplsim_rne_post: nsite > 64");
   if (nsite > 0 && (!site_body || !site_pos || !site_quat))
     return fail(SMPLSIM_EINVAL, "smplsim_rne_post: nsite > 0 needs site_body, site_pos and site_quat");
+  // not bodies_in_range: each site's body is checked with its quaternion, so a call with a bad quaternion before a bad body reports
+  // the quaternion
   for (int s = 0; s < nsite; s++) {
     if (site_body[s] < 0 || site_body[s] >= H.nb) return fail(SMPLSIM_EINVAL, "smplsim_rne_post: site_body entry out of range [0, nbody)");
     const float* q = site_quat + 4 * s;
@@ -957,9 +963,8 @@ static int imitation(SmplsimHandle* h, const SmplsimImitationCfg* cfg, const Smp
   const LHdr& H = *h->img.hdr();
   if (cfg->num_tracked < 1 || cfg->num_tracked > H.nb) return fail(SMPLSIM_EINVAL, "smplsim_imitation: num_tracked outside [1, nbody]");
   if (!cfg->tracked_bodies && cfg->num_tracked != H.nb) return fail(SMPLSIM_EINVAL, "smplsim_imitation: tracked_bodies NULL needs num_tracked == nbody");
-  if (cfg->tracked_bodies)
-    for (int j = 0; j < cfg->num_tracked; j++)
-      if (cfg->tracked_bodies[j] < 0 || cfg->tracked_bodies[j] >= H.nb) return fail(SMPLSIM_EINVAL, "smplsim_imitation: tracked body out of range [0, nbody)");
+  if (cfg->tracked_bodies && !bodies_in_range(cfg->tracked_bodies, cfg->num_tracked, H.nb))
+    return fail(SMPLSIM_EINVAL, "smplsim_imitation: tracked body out of range [0, nbody)");
   // every table check, NULL tables included, precedes the self_obs_dim check: a call with both wrong reports the tables
   ImArgs a; std::memset(&a, 0, sizeof a);
   const std::string why = motion_tables(H, tab, a);
@@ -1031,9 +1036,8 @@ extern "C" int smplsim_track_eval(SmplsimHandle* h, const SmplsimTrackEvalCfg* c
   const LHdr& H = *h->img.hdr();
   if (cfg->num_bodies < 3 || cfg->num_bodies > H.nb) return fail(SMPLSIM_EINVAL, "smplsim_track_eval: num_bodies outside [3, nbody]");
   if (!cfg->bodies && cfg->num_bodies != H.nb) return fail(SMPLSIM_EINVAL, "smplsim_track_eval: bodies NULL needs num_bodies == nbody");
-  if (cfg->bodies)
-    for (int j = 0; j < cfg->num_bodies; j++)
-      if (cfg->bodies[j] < 0 || cfg->bodies[j] >= H.nb) return fail(SMPLSIM_EINVAL, "smplsim_track_eval: eval body out of range [0, nbody)");
+  if (cfg->bodies && !bodies_in_range(cfg->bodies, cfg->num_bodies, H.nb))
+    return fail(SMPLSIM_EINVAL, "smplsim_track_eval: eval body out of range [0, nbody)");
   TeArgs t; std::memset(&t, 0, sizeof t);
   ImArgs& a = t.im;
   const std::string why = motion_tables(H, tab, a);
@@ -1073,8 +1077,7 @@ static std::string amp_check(const SmplsimHandle* h, const SmplsimAmpCfg* cfg, i
   if (cfg->interpolate != 0 && cfg->interpolate != 1) return "interpolate must be 0 or 1";
   if (cfg->num_key_bodies < 0 || cfg->num_key_bodies > H.nb) return "num_key_bodies outside [0, nbody]";
   if (cfg->num_key_bodies > 0 && !cfg->key_bodies) return "key_bodies NULL with num_key_bodies > 0";
-  for (int k = 0; k < cfg->num_key_bodies; k++)
-    if (cfg->key_bodies[k] < 0 || cfg->key_bodies[k] >= H.nb) return "key body out of range [0, nbody)";
+  if (!bodies_in_range(cfg->key_bodies, cfg->num_key_bodies, H.nb)) return "key body out of range [0, nbody)";
   // dof_to_obs takes every non-root joint as a 3-dof exp map (the reference asserts on any other joint)
   bool hinge3 = H.nv == 6 + 3 * (H.nb - 1);
   for (int b = 1; b < H.nb && hinge3; b++) hinge3 = h->img.bodies()[b].dofadr == 6 + 3 * (b - 1);

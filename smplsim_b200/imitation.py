@@ -72,7 +72,7 @@ class HumanoidImB200:
             if lib.tables[k].shape[1] != w * m.nbody:
                 raise ValueError(f"motion table {k!r} has {lib.tables[k].shape[1]} columns, the model needs {w * m.nbody}")
         tb = tracked_bodies if tracked_bodies is not None else e.get("tracked_bodies", None)
-        bodies = list(range(m.nbody)) if tb is None else [self._body_index(x) for x in tb]
+        bodies = list(range(m.nbody)) if tb is None else [m.body_index(x, "tracked_bodies entries must be body names or indices") for x in tb]
         self.tracked_bodies = bodies
         self._bodies = np.ascontiguousarray(np.asarray(bodies, dtype=np.int32))
         L = b._L()
@@ -141,16 +141,6 @@ class HumanoidImB200:
                 self.fall_qpos[r].copy_(b.qpos)
                 self.fall_qvel[r].copy_(b.qvel)
             self._env_index = torch.arange(N, device=dv)
-
-    def _body_index(self, x):
-        m = self.batch.model
-        if isinstance(x, str):
-            if x not in m.body_names:
-                raise ValueError(f"unknown body name {x!r}")
-            return list(m.body_names).index(x)
-        if isinstance(x, bool) or not isinstance(x, (int, np.integer)):
-            raise ValueError(f"tracked_bodies entries must be body names or indices, got {x!r}")
-        return int(x)
 
     @property
     def gpu_launches(self) -> int:
@@ -297,7 +287,8 @@ class HumanoidImB200:
         if ids.size == 0 or ids.min() < 0 or ids.max() >= K:
             raise ValueError(f"motion_ids must be a non-empty list of clips in [0, {K})")
         nb = self.model.nbody
-        bodies = list(range(nb)) if eval_bodies is None else [self._body_index(x) for x in eval_bodies]
+        rule = "eval_bodies entries must be body names or indices"
+        bodies = list(range(nb)) if eval_bodies is None else [self.model.body_index(x, rule) for x in eval_bodies]
         ebodies = np.ascontiguousarray(np.asarray(bodies, dtype=np.int32))
         J, M = len(bodies), ids.size
         tcfg = SmplsimTrackEvalCfgC(num_bodies=J, bodies=ebodies.ctypes.data if J else None, interpolate=int(self.interpolate), dt=0.0)

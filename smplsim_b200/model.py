@@ -147,6 +147,19 @@ class ModelDesc:
     def nbody(self):
         return len(self.body_names)
 
+    def body_index(self, body, rule: str, kind: str = "body") -> int:
+        """The index of ``body``: a name in ``body_names``, or an integer, returned as an int without a range check (each caller checks
+        [0, nbody) or leaves it to the C ABI).  Raises ``ValueError`` for an unknown name (``"unknown {kind} name ..."``) and for a bool
+        or any other value (``"{rule}, got ..."``).  ``rule`` is the caller's statement of what its argument must be, naming the
+        argument (``"jac_bodies entries must be body names or indices in [0, 24)"``); a range-checking caller raises it too."""
+        if isinstance(body, str):
+            if body not in self.body_names:
+                raise ValueError(f"unknown {kind} name {body!r}")
+            return list(self.body_names).index(body)
+        if isinstance(body, bool) or not isinstance(body, (int, np.integer)):
+            raise ValueError(f"{rule}, got {body!r}")
+        return int(body)
+
     @property
     def nv(self):
         return int(self.dof_armature.shape[0])
